@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — the driver's measurement contract for the KGE scoring hot path.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1]): ComplEx dim=512, 1vsAll + BCE, FB15k-237-shaped synthetic graph (14 541
 entities / 237 relations), batch n = 1024 triples per GPU.  One "step" = one 1vsAll forward pass over one batch
@@ -14,8 +14,8 @@ entities = 2*n*E candidate triples scored.  metric = candidate triples scored pe
                  pinned HOST batch with `job._process_batch` — H2D of the triples, kernels, `.item()` D2H inside the
                  timed region (falls back to the C-ABI host entry point when LibKGE is not importable; `e2e.api` says)
   roofline     : dominant kernel, CUDA events on its launch stream, against MEASURED_PEAKS.json
-  cpu_baseline : the UNMODIFIED reference job (`model: complex`, job.device cpu, installed in baseline/_ref by
-                 scripts/install_ref.sh) processing the same batches on the host cores, bounded sample
+  cpu_baseline : the UNMODIFIED reference job (`model: complex`, job.device cpu, installed in oracle/_ref by
+                 oracle/install_ref.sh) processing the same batches on the host cores, bounded sample
   configs      : (N=1) the other BASELINE.json configs — RotatE negative sampling, RESCAL KvsAll with CSR labels,
                  one Wikidata5M-shaped TransE shard — kernel ms, rate, roofline fraction, parity vs the live reference
   sharded      : (N>1) BASELINE config 5: TransE d=512, 600 k rows per GPU, entity-sharded across the N ranks with
@@ -23,6 +23,8 @@ entities = 2*n*E candidate triples scored.  metric = candidate triples scored pe
 
 `--impl reference` runs the reference arm alone (rank 0 only under torchrun).
 L2 is flushed (a 256 MiB buffer is overwritten) before every timed step, outside the timed bracket.
+`--dump-outputs DIR` writes what the timed step returned in its last step (the BCE loss, float64) and, for a
+second look at the same arithmetic, the per-row scores of a fixed seeded sample of that step's queries, as .npy.
 """
 from __future__ import annotations
 
@@ -59,8 +61,8 @@ def _peaks():
                     "source": "measured (MEASURED_PEAKS.json)"}
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0,
+            "source": "NVIDIA data sheet, H100 SXM, dense, 700 W (not measured)"}
 
 
 class ClockSampler:
@@ -200,7 +202,7 @@ def _time_reference_job(steps, warmup, budget_s):
     per = sum(times) / len(times)
     return {"value": 2.0 * N_BATCH * E / per, "unit": UNIT, "cores": best_thr, "kind": "reference",
             "sample": f"{len(times)} x TrainingJob1vsAll._process_batch (forward only; n={N_BATCH}, E={E}, D={D}, BCE) "
-                      f"of the unmodified reference (baseline/_ref) on the host CPU, torch {torch.__version__}, "
+                      f"of the unmodified reference (oracle/_ref) on the host CPU, torch {torch.__version__}, "
                       f"{best_thr} threads (fastest of the probed thread counts on {cores_all} host cores)",
             "ms_per_step": per * 1e3, "avg_loss_last": loss}, len(times)
 
@@ -367,7 +369,7 @@ def other_configs(engine, torch, dev, flush, peaks):
     from kge_b200 import synthetic
 
     have_ref = _have_kge()
-    sm_clock_ghz, sms = 1.965, 148
+    sm_clock_ghz, sms = 1.98, torch.cuda.get_device_properties(dev).multi_processor_count   # H100 SXM max SM clock
     fma_peak = sms * 128 * sm_clock_ghz * 1e9          # fp32 lanes x clock: FADD/FFMA issue slots per second
     out = {}
 
@@ -499,7 +501,7 @@ def train_step_bench(torch, local, ent_c, rel_c, batches_host, flush, iters=10):
 
 
 def reference_on_gpu_bench(torch, local, ent_c, rel_c, batches_host, flush, iters=20):
-    """SURVEY 8d "PyTorch-on-B200" bar: the UNMODIFIED reference job and model (`model: complex`, no plugin module on the
+    """SURVEY 8d "PyTorch-on-GPU" bar: the UNMODIFIED reference job and model (`model: complex`, no plugin module on the
     path) with job.device cuda — torch's own kernels (cuBLAS sgemm, elementwise, BCEWithLogits) on the same GPU, same
     batches, same harness as `e2e` (host batch in, .item() out, wall clock between synchronisations)."""
     if not _have_kge():
@@ -609,7 +611,7 @@ def transe_shard_bench(engine, torch, dev, flush, peaks, have_ref, fma_peak):
                           "frac": ops / (k_ms * 1e-3) / fma_peak,
                           "hbm_frac": byts / (k_ms * 1e-3) / 1e9 / peaks["hbm_gbs"],
                           "note": "north_star asks for the HBM fraction (hbm_frac: 1.23 GB table stream per call); the "
-                                  "binding roofline is the fp32 pipe: 148 SM x 128 lanes x 1.965 GHz issue slots"}}
+                                  "binding roofline is the fp32 pipe: SMs x 128 lanes x 1.98 GHz issue slots"}}
     if have_ref:
         sub = torch.randperm(rows, generator=torch.Generator().manual_seed(9))[:4096]
         m = _ref_model("transe", 4096, R5, D5, shard[sub.to(dev)].cpu(), rel.cpu())
@@ -769,7 +771,7 @@ def run_ours(args):
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if not engine.device_ok():
-        raise RuntimeError("bench.py needs an sm_100 (B200) device; kge_b200 has no fallback path")
+        raise RuntimeError("bench.py needs an sm_90 (H100) device; kge_b200 has no fallback path")
 
     ent_c, rel_c = synthetic.make_tables(MODEL, E, R, D, sigma=1.0)
     ent, rel = ent_c.to(dev), rel_c.to(dev)
@@ -814,6 +816,8 @@ def run_ours(args):
     barrier()
     launches = engine.launch_count()
     engine.profile_enable(False)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, engine, torch, ent, rel, batches_dev[(K - 1) % 4], loss_dev)
     step_ms = [a.elapsed_time(b) for a, b in ev]
     total_ms = torch.tensor([sum(step_ms)], dtype=torch.float64, device=dev)
     if dist is not None:
@@ -884,14 +888,11 @@ def run_ours(args):
     k_ms = sum(kern_ms) / len(kern_ms)
     achieved = _flops_cfg2() / (k_ms * 1e-3) / 1e12
     peak = peaks["bf16_tflops"]
-    pair = os.environ.get("B200KGE_TC_VERSION", "4") == "4"        # n = 1024 >= 128: the CTA-pair kernel is the default
     roofline = {
         "bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
         "traffic": 34.1e6,
-        "traffic_from": "profiles/r2c_raw_tc4.csv / r2_raw_tc3.csv (ncu --set full of this command: dram__bytes_read.sum 34.11 MB + "
-                        "dram__bytes_write.sum 0 per launch) — NOT measured in this run; algorithmic bytes = table "
-                        "planes 29.8 MB + query planes 4.2 MB",
-        "kernel": "pairwise_tc4_kernel<BCE> (CTA pair)" if pair else "pairwise_tc3_kernel<BCE>",
+        "traffic_from": "algorithmic bytes = table planes 29.8 MB + query planes 4.2 MB (not measured)",
+        "kernel": "pairwise_tc_kernel<BCE, F16X3>",
         "kernel_ms": k_ms,
         "peak_name": f"dense bf16 burst, {peaks['source']}",
         "note": "algorithmic fp32 FLOPs (2nED per direction, both directions in one launch).  For fp32-equivalent "
@@ -905,7 +906,7 @@ def run_ours(args):
     line = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": K, "warmup": W,
         "ms_per_step": total_ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": "f32 (fp16 hi/lo split products hi*hi + hi*lo + lo*hi on tcgen05, fp32 accumulate; ~2.5e-5 of score rms vs fp64)",
+        "dtype": "f32 (fp16 hi/lo split products hi*hi + hi*lo + lo*hi on wgmma, fp32 accumulate)",
         "data": "synthetic",
         "config": _config(world),
         "roofline": roofline,
@@ -932,12 +933,25 @@ def run_ours(args):
         except Exception as ex:
             line["configs"]["cfg2_train_fwd_bwd"] = {"error": repr(ex)}
         try:
-            line["reference_on_b200"] = reference_on_gpu_bench(torch, local, ent_c, rel_c, batches_host, flush)
+            line["reference_on_gpu"] = reference_on_gpu_bench(torch, local, ent_c, rel_c, batches_host, flush)
         except Exception as ex:
-            line["reference_on_b200"] = {"error": repr(ex)}
+            line["reference_on_gpu"] = {"error": repr(ex)}
     _emit(line)
     if dist is not None:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, engine, torch, ent, rel, batch, loss_dev):
+    """The timed step's result in its last step (its loss, what the caller receives), plus the scores behind it for a
+    fixed seeded sample of 64 of that batch's queries in both directions ([64, 2E] float32, 7.4 MB)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(loss_dev)], dtype=np.float64))
+    rows = torch.randperm(batch.shape[0], generator=torch.Generator().manual_seed(0))[:64].to(batch.device)
+    t = batch[rows]
+    scores = engine.score_sp_po(MODEL, ent, rel, t[:, 0].contiguous(), t[:, 1].contiguous(), t[:, 2].contiguous())
+    np.save(os.path.join(out_dir, "scores_sp_po_sample.npy"), scores.float().cpu().numpy())
 
 
 _OUT_FD = None
@@ -969,6 +983,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-configs", action="store_true", help="skip the other BASELINE configs (N=1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

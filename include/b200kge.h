@@ -1,5 +1,5 @@
 /*
- * b200kge.h — C ABI of the B200-native KGE scoring engine (libb200kge.so).
+ * b200kge.h — C ABI of the H100-native KGE scoring engine (libb200kge.so).
  *
  * This is the drop-in boundary for ONE path of uma-pi1/kge (LibKGE): embedding-row gather +
  * relational scorer forward (+ fused BCE/KL loss, rank/tie counting, negative-sample scoring)
@@ -44,7 +44,7 @@ typedef enum {
   B200KGE_ERR_UNSUPPORTED = -2, /* valid but not handled by this build (e.g. D % 4 != 0)   */
   B200KGE_ERR_CUDA = -3,        /* CUDA runtime error; message holds cudaGetErrorString    */
   B200KGE_ERR_WORKSPACE = -4,   /* workspace too small; see b200kge_workspace_bytes        */
-  B200KGE_ERR_NO_DEVICE = -5    /* no sm_100 device: the library never falls back to a CPU */
+  B200KGE_ERR_NO_DEVICE = -5    /* no sm_90 device: the library never falls back to a CPU */
 } b200kge_status;
 
 /* Scorers on the path (kge/model/<name>.py). */
@@ -103,7 +103,7 @@ typedef struct {
 /* Library / device ---------------------------------------------------------------------------- */
 int b200kge_version(void);
 const char* b200kge_last_error(void);
-/* 0 if the current device is sm_100 (B200), else B200KGE_ERR_NO_DEVICE. */
+/* 0 if the current device is sm_90 (H100), else B200KGE_ERR_NO_DEVICE. */
 int b200kge_device_ok(void);
 /* Number of kernel launches issued by this library on the calling thread since the last reset
  * (bench.py reports it as gpu_launches). */
@@ -302,7 +302,7 @@ int b200kge_kvsall_gather(const int64_t* keys, const int64_t* offsets, const int
                           int64_t num_keys, const int64_t* examples, int64_t nb,
                           int64_t* queries_out, int64_t* offsets_out, int64_t* cols_out);
 
-/* ---- SURVEY 8(f) rows: gradients, penalties, CSR labels (validated on a B200 in round 2) -------------
+/* ---- SURVEY 8(f) rows: gradients, penalties, CSR labels -------------
  *
  * b200kge_gemm_nt: C[M,N] = A[M,K] * B[N,K]^T, fp32 in / fp32 out, computed on the f16 tensor pipe from
  * hi/lo fp16 planes split once in HBM (presplit.cu + pairwise_tc3.cu) — the building block of the

@@ -1,8 +1,8 @@
-"""kge_b200 — B200-native scoring engine for knowledge-graph embeddings.
+"""kge_b200 — H100-native scoring engine for knowledge-graph embeddings.
 
-One hot path of uma-pi1/kge (LibKGE), rebuilt as hand-written sm_100a CUDA behind a C ABI
+One hot path of uma-pi1/kge (LibKGE), rebuilt as hand-written sm_90a CUDA behind a C ABI
 (include/b200kge.h): embedding gather + relational scorer forward for ComplEx / DistMult / SimplE /
-CP / RESCAL (tcgen05 3xTF32) and TransE / RotatE (CUDA-core distance kernels), fused with BCE/KL
+CP / RESCAL (wgmma tensor-core kernels, fp32-equivalent via an operand split) and TransE / RotatE (CUDA-core distance kernels), fused with BCE/KL
 loss, rank/tie counting and negative-sample gather+score.  No CPU fallback.
 """
 from . import _lib, engine, indexing  # noqa: F401

@@ -1,7 +1,7 @@
 """ctypes binding of libb200kge.so (the C ABI declared in include/b200kge.h).
 
-The library is built in-tree by kge_b200.build (nvcc, sm_100a).  There is NO CPU fallback: if the
-shared object is missing or no sm_100 device is present, calls raise.
+The library is built in-tree by kge_b200.build (nvcc, sm_90a).  There is NO CPU fallback: if the
+shared object is missing or no sm_90 device is present, calls raise.
 """
 from __future__ import annotations
 

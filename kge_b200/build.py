@@ -1,4 +1,4 @@
-"""Builds libb200kge.so (sm_100a) in-tree with nvcc.  No torch headers, no CPU fallback."""
+"""Builds libb200kge.so (sm_90a) in-tree with nvcc.  No torch headers, no CPU fallback."""
 from __future__ import annotations
 
 import hashlib
@@ -10,10 +10,10 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200kge.so")
-SOURCES = ["capi.cu", "fold.cu", "pairwise_simt.cu", "pairwise_tc.cu", "presplit.cu", "pairwise_tc3.cu", "pairwise_tc4.cu", "rowwise.cu", "epilogue_dense.cu", "hostindex.cu", "grad.cu", "grad_distance.cu", "csr_loss.cu"]
+SOURCES = ["capi.cu", "fold.cu", "pairwise_simt.cu", "pairwise_tc.cu", "presplit.cu", "rowwise.cu", "epilogue_dense.cu", "hostindex.cu", "grad.cu", "grad_distance.cu", "csr_loss.cu"]
 HEADERS = ["common.cuh", "fold.cuh", "ptx.cuh", "tc_common.cuh", os.path.join("..", "..", "include", "b200kge.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ]
 
@@ -59,7 +59,7 @@ def build_native(force: bool = False, verbose: bool = False) -> str:
             print(f"--- nvcc {s} ---\n{out}")
     if failed:
         raise RuntimeError("nvcc failed building libb200kge.so")
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout)

@@ -45,19 +45,6 @@ void profile_end(cudaStream_t st) {
 
 namespace {
 
-// Which pre-split kernel scores a block with n query rows PER DIRECTION and reduction length K: the CTA-pair kernel
-// (pairwise_tc4.cu) for n >= 128 and K > 448 (two 128-row halves per cluster tile; 65.8 vs 67.6 us at the FB15k-237
-// headline shape, K = 512), the 1-CTA kernel (pairwise_tc3.cu) otherwise (short reductions make the pair's per-tile
-// cross-CTA hand-over visible: RESCAL d=200 KvsAll 0.186 vs 0.146 ms).  Depends on n and K only — never on the
-// candidate count or on stacking — so every call of one batch (true scores on the unique targets, chunk scores, fused
-// forms) runs the same kernel.  B200KGE_TC_VERSION=3 | 4 forces one of them.
-bool use_pair_kernel(int64_t n, int K) {
-  const char* env_v = getenv("B200KGE_TC_VERSION");
-  if (env_v && atoi(env_v) == 3) return false;
-  if (env_v && atoi(env_v) == 4) return true;
-  return n >= 128 && K > 448;
-}
-
 // bump allocator over the caller's workspace
 struct Arena {
   uint8_t* base;
@@ -122,10 +109,9 @@ int run_block(const Block& B, float l_norm, int precision, int epi_kind, EpiPara
   // Path selection depends on the model, K, the table and the PER-DIRECTION row count n only — never on whether
   // the two directions are stacked — so score_sp / score_po / score_sp_po / the fused forms of one batch all run
   // the same arithmetic (EntityRankingJob compares them, eval_entity_ranking.py:192-203,242-274).
-  //   AUTO    -> F16X3 (pre-split fp16 planes, pairwise_tc3.cu) for dot-product scorers with 32 <= K <= 1024 and
+  //   AUTO    -> F16X3 (pre-split fp16 planes, pairwise_tc.cu) for dot-product scorers with 32 <= K <= 1024 and
   //              n >= 16; fp32 SIMT otherwise (beyond K = 1024 the tensor core's fp32 accumulator error, which
   //              grows with the reduction length — 2.8e-4 of rms at K = 14541 — leaves too little margin)
-  //   F16X3   -> pairwise_tc4.cu (CTA pair) for n >= 128 and K > 448, else pairwise_tc3.cu (use_pair_kernel)
   //   TF32_BF16X2 / 3XTF32 / TF32 -> pairwise_tc.cu (in-kernel split of raw fp32 tiles; needs TMA-able tables)
   int tc_kind = 0;       // 0 SIMT, 1 in-kernel split (pairwise_tc.cu), 3 pre-split planes
   if (f0.pair_op == PAIR_DOT && precision != B200KGE_PREC_FP32 && !cols_differ) {
@@ -179,9 +165,8 @@ int run_block(const Block& B, float l_norm, int precision, int epi_kind, EpiPara
       Q = Qw;
     }
     if (tc_kind == 3) {
-      // pre-split fp16 path (presplit.cu + pairwise_tc3.cu | pairwise_tc4.cu): one launch derives the hi/lo planes of
-      // the folded queries and of the (gathered) candidate rows, one launch scores them.
-      const bool pair = use_pair_kernel(n, K);
+      // pre-split fp16 path (presplit.cu + pairwise_tc.cu): one launch derives the hi/lo planes of the folded queries
+      // and of the (gathered) candidate rows, one launch scores them.
       const int Kp = (int)round_up(K, 64);
       SplitSet SQ{Q, ldq, nullptr, 0, nq, nq, K, Kp, nullptr, nullptr, nullptr};
       SplitSet ST{B.cand->base, B.cand->ld, B.cand->idx, f0.col_off, m, m + 32, K, Kp, nullptr, nullptr, nullptr};
@@ -193,7 +178,7 @@ int run_block(const Block& B, float l_norm, int precision, int epi_kind, EpiPara
         set_error("workspace too small for the pre-split operand planes");
         return B200KGE_ERR_WORKSPACE;
       }
-      const int nch3 = pair ? tc4_nchunks(nq, m) : tc3_nchunks(nq, m);
+      const int nch3 = tc_nchunks(nq, m);
       if (epi_kind == EPI_BCE || epi_kind == EPI_KL) {
         const int F = (epi_kind == EPI_BCE) ? 2 : 5;
         P.part = (float*)ws.take((size_t)nq * nch3 * F * 4);
@@ -203,7 +188,6 @@ int run_block(const Block& B, float l_norm, int precision, int epi_kind, EpiPara
       P.nchunks = nch3;
       if (nchunks_out) *nchunks_out = nch3;
       if ((rc = launch_presplit(ST, SQ, st))) return rc;
-      if (pair) return launch_pairwise_tc4(epi_kind, SQ, ST, P, st);
       return launch_pairwise_tc3(epi_kind, SQ, ST, P, st);
     }
     const int passes = (precision == B200KGE_PREC_TF32) ? 1 : (precision == B200KGE_PREC_3XTF32 ? 3 : 2);
@@ -323,14 +307,18 @@ int b200kge_profile_last_ms(float* ms) {
 }
 
 int b200kge_device_ok(void) {
-  int dev = 0, major = 0;
+  int dev = 0, major = 0, minor = 0;
   if (cudaGetDevice(&dev) != cudaSuccess ||
-      cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) {
+      cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess ||
+      cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) {
     cudaGetLastError();
     set_error("no CUDA device available: libb200kge has no CPU fallback");
     return B200KGE_ERR_NO_DEVICE;
   }
-  if (major != 10) { set_error("device compute capability %d.x is not sm_100 (B200)", major); return B200KGE_ERR_NO_DEVICE; }
+  if (major != 9 || minor != 0) {
+    set_error("device compute capability %d.%d is not sm_90 (H100)", major, minor);
+    return B200KGE_ERR_NO_DEVICE;
+  }
   return 0;
 }
 
@@ -595,11 +583,11 @@ int b200kge_train_1vsall_forward(int model, float l_norm, int precision,
     // step is THREE launches — prologue (gather + both folds + operand split of queries and table + labels), the
     // scorer with the loss reduction in its epilogue, and the fixed-order finaliser.
     const char* env_v = getenv("B200KGE_TC_VERSION");
-    const int tcv = (env_v && atoi(env_v) == 1) ? 1 : (use_pair_kernel(n, f0.K) ? 4 : 3);
+    const int tcv = (env_v && atoi(env_v) == 1) ? 1 : 3;
     const int K = f0.K;
     const bool presplit = f0.col_off == f1.col_off && f0.pair_op == PAIR_DOT && model != B200KGE_CP &&
                           (precision == B200KGE_PREC_AUTO || precision == B200KGE_PREC_F16X3) && K >= 32 && K <= 1024 &&
-                          n >= 16 && E.rows < (1ll << 31) && (tcv == 3 || tcv == 4) &&
+                          n >= 16 && E.rows < (1ll << 31) && tcv == 3 &&
                           ((size_t)round_up(K, 64) + (model == B200KGE_RESCAL ? E.dim : 0)) * 4 <= 48 * 1024;
     if (presplit) {
       const int64_t nq = 2 * n, m = E.rows;
@@ -612,7 +600,7 @@ int b200kge_train_1vsall_forward(int model, float l_norm, int precision,
       ST.inv_scale = (float*)ws.take((size_t)(m + 32) * 4);
       int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
       uint8_t* scratch = (uint8_t*)ws.take(1024);
-      const int nch = tcv == 4 ? tc4_nchunks(nq, m) : tc3_nchunks(nq, m);
+      const int nch = tc_nchunks(nq, m);
       const int F = (loss_kind == B200KGE_LOSS_BCE) ? 2 : 5;
       float* part = (float*)ws.take((size_t)nq * nch * F * 4);
       if (!SQ.hi || !SQ.lo || !SQ.inv_scale || !ST.hi || !ST.lo || !ST.inv_scale || !lab || !scratch || !part) {
@@ -625,9 +613,7 @@ int b200kge_train_1vsall_forward(int model, float l_norm, int precision,
       P.label_idx = lab;
       P.offset = (loss_kind == B200KGE_LOSS_BCE) ? offset : 0.f;
       P.part = part; P.nchunks = nch;
-      // (finalising inside the scorer — last CTA per query tile, then last tile — was measured: +8 us in the kernel
-      // against 5.8 us for the separate fixed-order finaliser, profiles/r2_summary.md; the finaliser stays separate)
-      if ((rc = tcv == 4 ? launch_pairwise_tc4(epi, SQ, ST, P, st) : launch_pairwise_tc3(epi, SQ, ST, P, st))) return rc;
+      if ((rc = launch_pairwise_tc3(epi, SQ, ST, P, st))) return rc;
       return launch_loss_finalize(loss_kind, part, nch, nq, loss_out, nullptr, scale, 0, scratch, 1, st);
     }
   }
@@ -712,7 +698,7 @@ int b200kge_train_1vsall_forward_host(int model, float l_norm, int precision,
 
 // ==================================================================================================
 // Pre-split fp16 GEMM, the analytic backward of the 1vsAll step for the dot family (grad.cu), penalties, row
-// normalisation, negative-sampling backward, CSR-label losses: SURVEY 8f rows, validated on a B200 in round 2.
+// normalisation, negative-sampling backward, CSR-label losses: SURVEY 8f rows.
 namespace {
 
 bool take_planes(Arena& ws, SplitSet& S) {

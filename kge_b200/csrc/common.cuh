@@ -1,4 +1,4 @@
-// common.cuh — shared host/device helpers of libb200kge (sm_100a only).
+// common.cuh — shared host/device helpers of libb200kge (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -336,7 +336,7 @@ int launch_pairwise_simt(int epi_kind, int pair_op, float l_norm, const float* Q
                          int64_t nq, const Rows& cand, int col_off, int K, const EpiParams& P,
                          cudaStream_t st);
 int pairwise_simt_nchunks(int64_t nq, int64_t m);
-// tcgen05 path: returns B200KGE_ERR_UNSUPPORTED if the shape cannot be served.
+// tensor-core path: returns B200KGE_ERR_UNSUPPORTED if the shape cannot be served.
 bool tc_supported(int pair_op, int K, const Rows& cand, int col_off);
 int tc_nchunks(int64_t nq, int64_t m);
 int launch_pairwise_tc(int epi_kind, int passes, const float* Q, int64_t ldq,

@@ -1,20 +1,19 @@
 // grad.cu — SURVEY §8 f-1: device pieces of the backward of the fused 1vsAll step for the dot family, of the
-// negative-sampling step, and the penalty / normalisation row kernels.  Validated on a B200 in round 2
-// (tests/test_gpu_backward.py, tests/test_gpu_jobs.py::test_training_epoch_native_backward); the math is pinned on
+// negative-sampling step, and the penalty / normalisation row kernels.  Checked on the GPU by
+// tests/test_gpu_backward.py and tests/test_gpu_jobs.py::test_training_epoch_native_backward; the math is pinned on
 // the CPU (oracle/kge_fold.py against autograd and against gradients of the live reference,
 // tests/test_fold_algebra.py), the kernels below transcribe it.
 //
 //   z  = Q T^T                       recomputed with the validated scorer (plain-store epilogue)
 //   G  = sigmoid(z + off) - y        grad_planes_kernel: written ONCE as fp16 hi/lo planes in both layouts,
 //                                    G [nq, Ep] and G^T [E, Np] (scale 2^14; 1/n rides in the row scale)
-//   dT = G^T Q   [E, K]              pre-split fp16 GEMM (pairwise_tc3.cu, store epilogue) on G^T and Q^T planes
+//   dT = G^T Q   [E, K]              pre-split fp16 GEMM (pairwise_tc.cu, store epilogue) on G^T and Q^T planes
 //   dQ = G  T    [nq, K]             same on G and T^T planes
 //   (da, dp) = unfold(a, p, dQ)      unfold_kernel: row-wise vector-Jacobian products of the relation fold,
 //                                    atomically added into the entity / relation gradient tables
 // This version trades HBM traffic for simplicity (scores and both G layouts are materialised, operands are
-// transposed through HBM).  Both GEMMs run split-K (512-element segments added in fp32, pairwise_tc3.cu): the
-// tensor core's fp32 accumulator error grows with the reduction length (measured 2.8e-4 of rms at K = 14541
-// against 2.4e-5 at K = 512), and dQ = G T reduces over all E entities.
+// transposed through HBM).  Both GEMMs run split-K (512-element segments added in fp32, pairwise_tc.cu): the
+// tensor core's fp32 accumulator error grows with the reduction length, and dQ = G T reduces over all E entities.
 #include <cuda_fp16.h>
 #include "fold.cuh"
 #include "tc_common.cuh"

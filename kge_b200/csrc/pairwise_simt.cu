@@ -8,7 +8,7 @@
 // RotatE (rotate.py:42-65, which materialises [n,E,D/2] intermediates in the reference) — whose
 // inner op is sub/abs/add (or complex modulus), i.e. CUDA-core work with no tensor-core form.  It
 // also serves dot-product scorers in exact-fp32 mode (B200KGE_PREC_FP32) and for shapes the
-// tcgen05 kernel does not take (tiny n, unaligned tables).
+// tensor-core kernel does not take (tiny n, unaligned tables).
 #include "common.cuh"
 
 namespace b200kge {
@@ -298,7 +298,7 @@ int launch_p(int epi, bool vec, dim3 grid, cudaStream_t st, const float* Q, int6
 // bounded so that the per-(row, chunk) partial buffers of the fused losses stay small.
 int pairwise_simt_nchunks(int64_t nq, int64_t m) {
   const int64_t ct = (m + BN - 1) / BN, rt = (nq + BM - 1) / BM;
-  int64_t want = (148 * 6 + rt - 1) / (rt > 0 ? rt : 1);
+  int64_t want = (132 * 6 + rt - 1) / (rt > 0 ? rt : 1);
   if (want < 1) want = 1;
   return (int)(want < ct ? want : ct);
 }

@@ -1,120 +1,149 @@
-// pairwise_tc.cu — tcgen05 tensor-core 1-vs-N scorer for the dot-product family
-// (ComplEx / DistMult / SimplE / CP / RESCAL after folding), fp32-equivalent via an on-chip operand split.
+// pairwise_tc.cu — Hopper (sm_90a) tensor-core 1-vs-N scorer for the dot-product family (ComplEx / DistMult /
+// SimplE / CP / RESCAL after folding), fp32-equivalent through an operand split, with the consumer of the scores
+// (the plain [n,E] store, BCE / KL loss, rank counting) fused into the epilogue.
 //
-//   S[q, e] = sum_k Q[q,k] * T[e,k]          Q: folded queries [nq, K]  (fold.cu, RAW fp32)
-//                                            T: entity table   [m,  K]  streamed RAW from HBM/L2
+//   S[q, e] = sum_k Q[q,k] * T[e,k]          Q: folded queries [nq, K]     T: entity table [m, K]
 //
-// replaces the reference's torch.mm over concatenated operands (complex.py:37,39,
-// distmult.py:19,21, simple.py:25-29, cp.py:24,26, rescal.py:41,47) AND whatever consumes the
-// scores next (BCE / KL loss, rank counting, or the plain [n,E] store) in ONE kernel.
+// replaces the reference's torch.mm over concatenated operands (complex.py:37,39, distmult.py:19,21,
+// simple.py:25-29, cp.py:24,26, rescal.py:41,47) AND whatever consumes the scores next in ONE kernel.
 //
-// Precision (the reference is a true fp32 GEMM; single-pass TF32 misses the 1e-4 bar 40x):
-//   mixed (default)  D += Q*T [tf32, raw tiles: kind::tf32 truncates the low 13 mantissa bits, measured]
-//                         + Q_lo16*T_hi16 + Q_hi16*T_lo16   [bf16, kind::f16]        2.4e-5 of rms
-//   3xTF32           D += Q*T + Q_lo*T + Q*T_lo              [tf32]                   3.0e-5 of rms
-// Nothing derivable on chip crosses the L2->SM fabric: TMA lands RAW fp32 tiles, splitter warps derive
-// the lo / bf16 operand tiles in shared memory (fence.proxy.async before the MMA warp may read them).
+// Operand forms (MODE), one kernel:
+//   F16X3   pre-split fp16 planes (presplit.cu / grad.cu, THE default): S = qs*ts*(Qh*Th + Qh*Tl + Ql*Th), qs / ts
+//           per-row powers of two.  Per 64-wide K chunk TMA lands four 16 KB boxes; nothing else touches smem.
+//   TF32    raw fp32 tiles, one tf32 product (experiments).
+//   TF32X3  raw fp32 tiles, splitter warps derive lo = rn_tf32(x - trunc_tf32(x)) in smem: Q*T + Ql*T + Q*Tl (tf32).
+//   MIXED   raw fp32 tiles, splitter warps derive bf16 hi / lo tiles: Q*T [tf32] + Ql16*Th16 + Qh16*Tl16 [bf16].
+// The reference is a true fp32 GEMM; single-pass TF32 misses the 1e-4 bar, the three split forms meet it.
 //
-// Pipeline (measured: with coupled 2x96 KB stages the three phases TMA 0.034 / split 0.041 / MMA 0.046 ms
-// overlapped poorly, 0.135 ms total).  Raw tiles and derived operand tiles are therefore DECOUPLED rings:
-//   raw[2]  48 KB each: Q tile 16 KB | T tile 32 KB            filled by TMA
-//   op[2]   48 KB each: derived Q operands 16 KB | derived T operands 32 KB   written by the splitters
-//   raw_full[r]  TMA bytes landed                                  -> splitters, MMA (hi*hi)
-//   raw_free[r]  hi*hi MMAs retired (tcgen05.commit) + 6 splitter warps done reading -> TMA producer
-//   op_full[o]   6 splitter warps wrote + fenced the derived tiles -> MMA (cross terms)
-//   op_free[o]   cross-term MMAs retired (tcgen05.commit)          -> splitters
-// so the producer refills a raw buffer half a chunk earlier and the split of chunk c+1 overlaps the
-// cross-term MMAs of chunk c.
-//
-// CTA = 16 warps, one CTA per SM, persistent over (query tile, range of entity tiles):
-//   warp 0      TMA producer (one lane)          warp 1       MMA issuer (one lane), TMEM alloc
-//   warps 2-3   query-tile splitters             warps 12-15  table-tile splitters
-//   warps 4-11  epilogue: tcgen05.ld -> regs -> {transposed coalesced store | BCE | KL | rank}
-//               (2 warps per TMEM lane quadrant, each takes 128 of the 256 accumulator columns)
-// Tile = 128 queries (UMMA M, TMEM lanes) x <=256 entities (UMMA N, TMEM columns), K in chunks of 32
-// floats (one 128-byte swizzle atom), 2 TMEM accumulators of 256 columns so the epilogue of tile i
-// overlaps the MMAs of tile i+1.  TMEM lane = query row, so every per-row reduction is thread-local.
+// CTA = 3 (4 with splitters) warpgroups, one CTA per SM, persistent over (query tile, range of entity tiles):
+//   warpgroup 0   warp 0 lane 0: TMA producer
+//   warpgroups 1-2 consumers: warpgroup g owns query rows [64g, 64g+64) of the 128-row tile; wgmma m64n128 with the
+//                 fp32 accumulator in registers, then the accumulator goes to a shared-memory tile (one row per
+//                 thread) and the same warps run the epilogue: warp w of the group takes rows 32*(w&1) and
+//                 columns 64*(w>>1) of the 128-entity tile
+//   warpgroup 3   (TF32X3 / MIXED) splitters
+// Ring of NSTAGE stages of 64 KB; a stage is one K chunk of both operands in every plane the mode uses.
+//   full[s]    TMA bytes landed                              -> splitters, consumers
+//   split[s]   splitter warps wrote + fenced derived tiles    -> consumers
+//   empty[s]   every consumer warp's wgmmas on s retired      -> producer
+// While the consumers run the epilogue of tile i the producer already fills the ring for tile i+1.
 #include "tc_common.cuh"
 
 namespace b200kge {
 
 namespace {
 
-constexpr int TM = 128;             // queries per tile  (UMMA M)
-constexpr int TN = 256;             // max entities per tile (UMMA N)
-constexpr int TK = 32;              // floats per K chunk (128 B swizzle atom)
-constexpr int NR = 2, NO = 2;       // raw / operand ring depths
-constexpr int A_BYTES = TM * TK * 4;   // 16 KB
-constexpr int B_BYTES = TN * TK * 4;   // 32 KB
-constexpr int RING_BYTES = A_BYTES + B_BYTES;   // one raw or one operand buffer: 48 KB
-using tc::EPI_WARPS;
-using tc::SPLIT_WARPS;
-using tc::NTHREADS;
+enum Mode : int { MODE_F16X3 = 0, MODE_TF32 = 1, MODE_TF32X3 = 2, MODE_MIXED = 3 };
+
+constexpr int TM = 128;             // queries per tile (two consumer warpgroups x 64)
+constexpr int TN = 128;             // entities per tile (wgmma N)
+constexpr int NSTAGE = 2;
+constexpr int STAGE_BYTES = 64 * 1024;
+constexpr int BOX_BYTES = 16 * 1024;        // one 128-row box of 128-byte rows
+constexpr int ACC_LD = TN + 1;              // padded row of the staged accumulator (conflict-free row-per-thread reads)
+constexpr int ACC_BYTES = TM * ACC_LD * 4;
+constexpr int EPI_WARPS = 8;
 using tc::STG_LD;
-constexpr int NSPLIT = SPLIT_WARPS + 2;   // 4 table-tile + 2 query-tile splitter warps
 constexpr int STG_BYTES = EPI_WARPS * 32 * STG_LD * 4;
-constexpr int SMEM_BYTES = 1024 /*align slack*/ + (NR + NO) * RING_BYTES + STG_BYTES + 256 /*barriers*/;
-constexpr int TMEM_COLS = 512;
+constexpr int SMEM_BYTES = 1024 /*align slack*/ + NSTAGE * STAGE_BYTES + ACC_BYTES + STG_BYTES + 256 /*barriers*/;
+static_assert(SMEM_BYTES <= 227 * 1024, "exceeds the H100's 227 KB of shared memory per block");
+
+template <int MODE> struct ModeCfg {
+  static constexpr bool SPLIT = MODE == MODE_TF32X3 || MODE == MODE_MIXED;
+  static constexpr int NTHREADS = (SPLIT ? 4 : 3) * 128;
+  static constexpr int TK = MODE == MODE_F16X3 ? 64 : 32;                        // K elements per chunk
+  static constexpr uint32_t TX = MODE == MODE_F16X3 ? 4 * BOX_BYTES : 2 * BOX_BYTES;   // TMA bytes per stage
+};
 
 struct TcParams {
   int64_t nq, m;
-  int K;            // reduction length (floats)
+  int nk;           // K chunks
   int q_tiles, e_tiles, echunks;
-  int dbg;          // experiments (B200KGE_DBG bit-mask): 1 = skip TMA after the first fills, 2 = skip split
-                    // math, 4 = skip MMAs — isolates the pipeline phases (results are garbage)
-  int tn;           // entities per tile actually used (multiple of 16, <= TN): chosen per problem so that
-                    // ceil(tiles / SMs) * tn — the makespan in columns — is minimal
+  int ksplit;       // > 1: split-K GEMM mode (EPI_STORE only): the reduction is cut into `ksplit` segments of `kseg`
+  int kseg;         //      K chunks; every (tile, segment) is its own work item and ADDS into the zeroed output
+  const float* q_scale;   // F16X3: [nq]
+  const float* t_scale;   // F16X3: [m + 32], zero beyond m
   EpiParams epi;
 };
 
-// PASSES: 1 = single-pass tf32 (experiments), 2 = mixed tf32 + bf16 cross terms, 3 = 3xTF32
-template <int EPI, int PASSES>
-__global__ void __launch_bounds__(NTHREADS, 1)
+// Stage layout (byte offsets).  F16X3: Qh | Th | Ql | Tl.  Raw modes: Q | T | derived tiles:
+//   TF32X3: Ql (16 KB) | Tl (16 KB)      MIXED: Qh16 | Ql16 | Th16 | Tl16 (8 KB each, 64-byte rows)
+template <int MODE>
+__device__ __forceinline__ void mma_chunk(float (&d)[64], uint32_t st, int g) {
+  const uint32_t a = st + (uint32_t)g * (BOX_BYTES / 2), b = st + BOX_BYTES;   // this warpgroup's 64 query rows
+  if constexpr (MODE == MODE_F16X3) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint32_t o = k * 32;
+      ptx::wgmma_f16(d, ptx::wg_desc_sw128(a + o), ptx::wg_desc_sw128(b + o));
+      ptx::wgmma_f16(d, ptx::wg_desc_sw128(a + o), ptx::wg_desc_sw128(b + 2 * BOX_BYTES + o));
+      ptx::wgmma_f16(d, ptx::wg_desc_sw128(a + 2 * BOX_BYTES + o), ptx::wg_desc_sw128(b + o));
+    }
+  } else {
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      ptx::wgmma_tf32(d, ptx::wg_desc_sw128(a + k * 32), ptx::wg_desc_sw128(b + k * 32));
+    if constexpr (MODE == MODE_TF32X3) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        ptx::wgmma_tf32(d, ptx::wg_desc_sw128(a + 2 * BOX_BYTES + k * 32), ptx::wg_desc_sw128(b + k * 32));
+        ptx::wgmma_tf32(d, ptx::wg_desc_sw128(a + k * 32), ptx::wg_desc_sw128(b + 2 * BOX_BYTES + k * 32));
+      }
+    } else if constexpr (MODE == MODE_MIXED) {
+      const uint32_t h = st + 2 * BOX_BYTES + (uint32_t)g * (BOX_BYTES / 4);    // Qh16 rows of this warpgroup
+      const uint32_t l = h + BOX_BYTES / 2;                                      // Ql16
+      const uint32_t th = st + 3 * BOX_BYTES, tl = th + BOX_BYTES / 2;           // Th16, Tl16
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        ptx::wgmma_bf16(d, ptx::wg_desc_sw64(l + k * 32), ptx::wg_desc_sw64(th + k * 32));
+        ptx::wgmma_bf16(d, ptx::wg_desc_sw64(h + k * 32), ptx::wg_desc_sw64(tl + k * 32));
+      }
+    }
+  }
+}
+
+template <int EPI, int MODE>
+__global__ void __launch_bounds__(ModeCfg<MODE>::NTHREADS, 1)
 pairwise_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmT,
+                   const __grid_constant__ CUtensorMap tmQl, const __grid_constant__ CUtensorMap tmTl,
                    const TcParams prm) {
+  using C = ModeCfg<MODE>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* raw_base = smem;
-  uint8_t* op_base = smem + NR * RING_BYTES;
-  float* stg = reinterpret_cast<float*>(smem + (NR + NO) * RING_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (NR + NO) * RING_BYTES + STG_BYTES);
-  uint64_t* raw_full = bars;                    // [NR]
-  uint64_t* raw_free = bars + NR;               // [NR]
-  uint64_t* op_full = bars + 2 * NR;            // [NO]
-  uint64_t* op_free = bars + 2 * NR + NO;       // [NO]
-  uint64_t* tfull = bars + 2 * NR + 2 * NO;     // [2]
-  uint64_t* tempty = tfull + 2;                 // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  float* accs = reinterpret_cast<float*>(smem + NSTAGE * STAGE_BYTES);
+  float* stg = reinterpret_cast<float*>(smem + NSTAGE * STAGE_BYTES + ACC_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NSTAGE * STAGE_BYTES + ACC_BYTES + STG_BYTES);
+  uint64_t* full = bars;                  // [NSTAGE]
+  uint64_t* split = bars + NSTAGE;        // [NSTAGE]
+  uint64_t* empty = bars + 2 * NSTAGE;    // [NSTAGE]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nk = (prm.K + TK - 1) / TK;
-  const int total_work = prm.q_tiles * prm.echunks;
+  const int total_work = prm.q_tiles * prm.echunks * prm.ksplit;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     ptx::prefetch_tensormap(&tmQ);
     ptx::prefetch_tensormap(&tmT);
-    for (int r = 0; r < NR; ++r) {
-      ptx::mbar_init(&raw_full[r], 1);
-      ptx::mbar_init(&raw_free[r], PASSES == 1 ? 1 : 1 + NSPLIT);   // MMA commit (+ splitter warps)
+    if constexpr (MODE == MODE_F16X3) {
+      ptx::prefetch_tensormap(&tmQl);
+      ptx::prefetch_tensormap(&tmTl);
     }
-    for (int o = 0; o < NO; ++o) {
-      ptx::mbar_init(&op_full[o], NSPLIT);
-      ptx::mbar_init(&op_free[o], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      ptx::mbar_init(&tfull[b], 1);
-      ptx::mbar_init(&tempty[b], EPI_WARPS);
+    for (int s = 0; s < NSTAGE; ++s) {
+      ptx::mbar_init(&full[s], 1);
+      ptx::mbar_init(&split[s], 4);
+      ptx::mbar_init(&empty[s], EPI_WARPS);
     }
     ptx::fence_barrier_init();
   }
-  if (warp == 1) ptx::tmem_alloc<TMEM_COLS>(tmem_slot);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // e-tile range of work item w
+  int k0 = 0, k1 = prm.nk;      // K-chunk range of the current work item (split-K mode: one segment)
   auto work_range = [&](int w, int& qt, int& et0, int& et1, int& ec) {
+    if (prm.ksplit > 1) {
+      const int ks = w % prm.ksplit;
+      w /= prm.ksplit;
+      k0 = ks * prm.kseg;
+      k1 = (k0 + prm.kseg < prm.nk) ? k0 + prm.kseg : prm.nk;
+    }
     qt = w / prm.echunks;
     ec = w - qt * prm.echunks;
     const int base = prm.e_tiles / prm.echunks, rem = prm.e_tiles % prm.echunks;
@@ -130,208 +159,160 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         int qt, et0, et1, ec;
         work_range(w, qt, et0, et1, ec);
         for (int et = et0; et < et1; ++et) {
-          for (int kc = 0; kc < nk; ++kc, ++c) {
-            const int r = c % NR;
-            ptx::mbar_wait(&raw_free[r], ((c / NR) & 1) ^ 1);
-            if ((prm.dbg & 1) && c >= (uint32_t)NR) { ptx::mbar_arrive(&raw_full[r]); continue; }
-            uint8_t* rp = raw_base + r * RING_BYTES;
-            ptx::mbar_arrive_expect_tx(&raw_full[r], A_BYTES + prm.tn * TK * 4);
-            ptx::tma_load_2d(rp, &tmQ, &raw_full[r], kc * TK, qt * TM);                  // raw queries
-            ptx::tma_load_2d(rp + A_BYTES, &tmT, &raw_full[r], kc * TK, et * prm.tn);    // raw table tile
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ============================================
-    if (lane == 0) {
-      const uint32_t idesc = ptx::umma_idesc_tf32(TM, prm.tn);
-      const uint32_t idesc16 = ptx::umma_idesc_bf16(TM, prm.tn);
-      const bool do_mma = !(prm.dbg & 4);
-      uint32_t c = 0, it = 0;
-      for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
-        int qt, et0, et1, ec;
-        work_range(w, qt, et0, et1, ec);
-        for (int et = et0; et < et1; ++et, ++it) {
-          const int b = it & 1;
-          ptx::mbar_wait(&tempty[b], ((it >> 1) & 1) ^ 1);   // epilogue drained this accumulator
-          ptx::tc_fence_after();
-          const uint32_t d_tmem = tmem_base + (uint32_t)(b * TN);
-          for (int kc = 0; kc < nk; ++kc, ++c) {
-            const int r = c % NR, o = c % NO;
-            const uint32_t a_raw = ptx::smem_u32(raw_base + r * RING_BYTES);
-            const uint32_t b_raw = a_raw + A_BYTES;
-            const uint32_t a_op = ptx::smem_u32(op_base + o * RING_BYTES);
-            const uint32_t b_op = a_op + A_BYTES;
-            // hi*hi on the raw tiles as soon as they land
-            ptx::mbar_wait(&raw_full[r], (c / NR) & 1);
-            ptx::tc_fence_after();
-#pragma unroll
-            for (int k4 = 0; k4 < TK / 8; ++k4)
-              if (do_mma)
-                ptx::umma_tf32(d_tmem, ptx::umma_desc_sw128(a_raw + k4 * 32), ptx::umma_desc_sw128(b_raw + k4 * 32),
-                               idesc, (kc > 0 || k4 > 0) ? 1u : 0u);
-            if (PASSES == 1) { ptx::umma_commit(&raw_free[r]); continue; }
-            // cross terms on the derived tiles
-            ptx::mbar_wait(&op_full[o], (c / NO) & 1);
-            ptx::tc_fence_after();
-            if (PASSES == 3) {
-              // Q_lo * T_raw needs the raw table tile as well: it is issued before raw_free is committed
-#pragma unroll
-              for (int k4 = 0; k4 < TK / 8; ++k4)
-                if (do_mma)
-                  ptx::umma_tf32(d_tmem, ptx::umma_desc_sw128(a_op + k4 * 32), ptx::umma_desc_sw128(b_raw + k4 * 32), idesc, 1u);
-#pragma unroll
-              for (int k4 = 0; k4 < TK / 8; ++k4)
-                if (do_mma)
-                  ptx::umma_tf32(d_tmem, ptx::umma_desc_sw128(a_raw + k4 * 32), ptx::umma_desc_sw128(b_op + k4 * 32), idesc, 1u);
-              ptx::umma_commit(&raw_free[r]);
-            } else {
-              ptx::umma_commit(&raw_free[r]);        // raw tiles are only read by the hi*hi MMAs above
-              // op buffers hold bf16 tiles (64-B swizzle): [hi16 | lo16] for Q (8 KB each) and T (16 KB each)
-              const uint32_t a16h = a_op, a16l = a_op + A_BYTES / 2;
-              const uint32_t b16h = b_op, b16l = b_op + B_BYTES / 2;
-#pragma unroll
-              for (int k2 = 0; k2 < TK / 16; ++k2) {
-                if (!do_mma) break;
-                ptx::umma_bf16(d_tmem, ptx::umma_desc_sw64(a16l + k2 * 32), ptx::umma_desc_sw64(b16h + k2 * 32), idesc16, 1u);
-                ptx::umma_bf16(d_tmem, ptx::umma_desc_sw64(a16h + k2 * 32), ptx::umma_desc_sw64(b16l + k2 * 32), idesc16, 1u);
-              }
+          for (int kc = k0; kc < k1; ++kc, ++c) {
+            const int s = (int)(c % NSTAGE);
+            ptx::mbar_wait_bounded(&empty[s], ((c / NSTAGE) & 1) ^ 1);
+            uint8_t* sp = smem + s * STAGE_BYTES;
+            ptx::mbar_arrive_expect_tx(&full[s], C::TX);
+            ptx::tma_load_2d(sp, &tmQ, &full[s], kc * C::TK, qt * TM);
+            ptx::tma_load_2d(sp + BOX_BYTES, &tmT, &full[s], kc * C::TK, et * TN);
+            if constexpr (MODE == MODE_F16X3) {
+              ptx::tma_load_2d(sp + 2 * BOX_BYTES, &tmQl, &full[s], kc * C::TK, qt * TM);
+              ptx::tma_load_2d(sp + 3 * BOX_BYTES, &tmTl, &full[s], kc * C::TK, et * TN);
             }
-            ptx::umma_commit(&op_free[o]);
           }
-          ptx::umma_commit(&tfull[b]);             // accumulator complete
         }
       }
     }
-  } else if (warp >= 12 || warp == 2 || warp == 3) {
-    // ================================ splitters =============================================
-    // warps 12-15 derive the table-tile operands, warps 2-3 the query-tile operands
-    if (PASSES != 1) {
-      const bool is_b = warp >= 12;
-      const int t = is_b ? threadIdx.x - 12 * 32 : threadIdx.x - 2 * 32;
+  } else if (warp >= 12) {
+    // ================================ splitters (TF32X3 / MIXED) ============================
+    if constexpr (C::SPLIT) {
+      const int t = threadIdx.x - 12 * 32;
       uint32_t c = 0;
       for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
         int qt, et0, et1, ec;
         work_range(w, qt, et0, et1, ec);
         for (int et = et0; et < et1; ++et) {
-          for (int kc = 0; kc < nk; ++kc, ++c) {
-            const int r = c % NR, o = c % NO;
-            ptx::mbar_wait(&raw_full[r], (c / NR) & 1);
-            ptx::mbar_wait(&op_free[o], ((c / NO) & 1) ^ 1);
-            const uint32_t rp = ptx::smem_u32(raw_base + r * RING_BYTES);
-            const uint32_t opp = ptx::smem_u32(op_base + o * RING_BYTES);
-            if (prm.dbg & 2) {
-              // experiment: no split work
-            } else if (PASSES == 3) {
-              if (is_b) tc::split_tile<B_BYTES, SPLIT_WARPS * 32>(rp + A_BYTES, opp + A_BYTES, t);
-              else      tc::split_tile<A_BYTES, 2 * 32>(rp, opp, t);
+          for (int kc = k0; kc < k1; ++kc, ++c) {
+            const int s = (int)(c % NSTAGE);
+            ptx::mbar_wait_bounded(&full[s], (c / NSTAGE) & 1);
+            const uint32_t sp = ptx::smem_u32(smem + s * STAGE_BYTES);
+            if constexpr (MODE == MODE_TF32X3) {
+              tc::split_tile<BOX_BYTES, 128>(sp, sp + 2 * BOX_BYTES, t);
+              tc::split_tile<BOX_BYTES, 128>(sp + BOX_BYTES, sp + 3 * BOX_BYTES, t);
             } else {
-              if (is_b) tc::split_tile_bf16<TN, SPLIT_WARPS * 32>(rp + A_BYTES, opp + A_BYTES, opp + A_BYTES + B_BYTES / 2, t);
-              else      tc::split_tile_bf16<TM, 2 * 32>(rp, opp, opp + A_BYTES / 2, t);
+              tc::split_tile_bf16<TM, 128>(sp, sp + 2 * BOX_BYTES, sp + 2 * BOX_BYTES + BOX_BYTES / 2, t);
+              tc::split_tile_bf16<TN, 128>(sp + BOX_BYTES, sp + 3 * BOX_BYTES, sp + 3 * BOX_BYTES + BOX_BYTES / 2, t);
             }
             ptx::fence_proxy_async_smem();
             __syncwarp();
-            if (lane == 0) {
-              ptx::mbar_arrive(&op_full[o]);
-              ptx::mbar_arrive(&raw_free[r]);      // this warp is done reading the raw tile
-            }
+            if (lane == 0) ptx::mbar_arrive(&split[s]);
           }
         }
       }
     }
   } else if (warp >= 4) {
-    // ================================ epilogue ==============================================
-    const int quad = warp & 3;                // TMEM lanes [32*quad, +32)
-    const int half = (warp - 4) >> 2;         // columns [128*half, +128) of the accumulator
+    // ================================ consumers: wgmma + epilogue ===========================
+    const int g = (warp - 4) >> 2;            // consumer warpgroup: query rows [64g, +64) of the tile
+    const int wl = warp & 3;                  // warp within the group
+    const int quad = wl & 1, half = wl >> 1;  // epilogue: rows [32*quad, +32) of the group, columns [64*half, +64)
+    const int tg = threadIdx.x & 127;
+    float* acc_g = accs + g * 64 * ACC_LD;
     float* my_stg = stg + (warp - 4) * 32 * STG_LD;
     const EpiParams& P = prm.epi;
-    uint32_t it = 0;
+    uint32_t c = 0;
     for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
       int qt, et0, et1, ec;
       work_range(w, qt, et0, et1, ec);
-      const int64_t row = (int64_t)qt * TM + quad * 32 + lane;   // this thread's query row
+      const int64_t tile_row0 = (int64_t)qt * TM + g * 64 + quad * 32;
+      const int64_t row = tile_row0 + lane;   // this thread's query row in the epilogue
       const bool row_ok = row < prm.nq;
       RowState<EPI> st;
       st.init();
       const float aux = row_ok ? epi_row_aux<EPI>(P, row) : 0.f;
-      for (int et = et0; et < et1; ++et, ++it) {
-        const int b = it & 1;
-        ptx::mbar_wait(&tfull[b], (it >> 1) & 1);
-        ptx::tc_fence_after();
-        // columns beyond this tile's tn entities were never computed: clip the valid range
-        const int64_t tile_end = (int64_t)(et + 1) * prm.tn;
-        tc::epilogue_tile<EPI, 4>(P, st, aux,
-                                  tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(b * TN + half * 128),
-                                  (int64_t)qt * TM + quad * 32, (int64_t)et * prm.tn + half * 128, prm.nq,
-                                  tile_end < prm.m ? tile_end : prm.m, my_stg, lane);
-        ptx::tc_fence_before();
+      const float qs = (MODE == MODE_F16X3 && row_ok) ? __ldg(prm.q_scale + row) : 0.f;
+      const int64_t csr_end = (P.csr_off && row_ok) ? __ldg(P.csr_off + row + 1) : 0;
+      for (int et = et0; et < et1; ++et) {
+        float d[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) d[i] = 0.f;
+        for (int kc = k0; kc < k1; ++kc, ++c) {
+          const int s = (int)(c % NSTAGE);
+          ptx::mbar_wait_bounded(&full[s], (c / NSTAGE) & 1);
+          if constexpr (C::SPLIT) ptx::mbar_wait_bounded(&split[s], (c / NSTAGE) & 1);
+          ptx::wg_fence();
+          mma_chunk<MODE>(d, ptx::smem_u32(smem + s * STAGE_BYTES), g);
+          ptx::wg_commit();
+          if (kc > k0) {
+            ptx::wg_wait<1>();                 // the previous chunk's wgmmas retired: release its stage
+            __syncwarp();
+            if (lane == 0) ptx::mbar_arrive(&empty[(c - 1) % NSTAGE]);
+          }
+        }
+        ptx::wg_wait<0>();
         __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&tempty[b]);
+        if (lane == 0) ptx::mbar_arrive(&empty[(c - 1) % NSTAGE]);
+        // accumulator -> shared tile (one row per thread afterwards)
+        ptx::bar_sync(1 + g, 128);             // the previous tile's epilogue is done reading acc_g
+        {
+          const int r = 16 * (tg >> 5) + ((tg & 31) >> 2), cc = 2 * (tg & 3);
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            acc_g[r * ACC_LD + 8 * j + cc] = d[4 * j];
+            acc_g[r * ACC_LD + 8 * j + cc + 1] = d[4 * j + 1];
+            acc_g[(r + 8) * ACC_LD + 8 * j + cc] = d[4 * j + 2];
+            acc_g[(r + 8) * ACC_LD + 8 * j + cc + 1] = d[4 * j + 3];
+          }
+        }
+        ptx::bar_sync(1 + g, 128);
+        const int64_t tile_end = (int64_t)(et + 1) * TN;
+        tc::epilogue_tile<EPI, 2, MODE == MODE_F16X3>(P, st, aux, acc_g + (quad * 32 + lane) * ACC_LD + half * 64,
+                                                      tile_row0, (int64_t)et * TN + half * 64, prm.nq,
+                                                      tile_end < prm.m ? tile_end : prm.m, my_stg, lane, qs,
+                                                      prm.t_scale, csr_end);
       }
       if constexpr (EPI != EPI_STORE) {
         if (row_ok) epi_flush<EPI>(P, st, row, ec * 2 + half);
       }
     }
   }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc<TMEM_COLS>(tmem_base);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------
 using tc::num_sms;
 
-void plan(int64_t nq, int64_t m, int& q_tiles, int& e_tiles, int& echunks, int& tn) {
+// entity tiles split into `echunks` ranges so that q_tiles * echunks ~ #SMs
+void plan(int64_t nq, int64_t m, int& q_tiles, int& e_tiles, int& echunks) {
   q_tiles = (int)((nq + TM - 1) / TM);
   if (q_tiles < 1) q_tiles = 1;
-  const int units = num_sms();
-  // pick the tile width (multiple of 16 in [128, 256]) minimising the per-SM makespan in columns
-  int64_t best_cost = -1;
-  tn = TN;
-  for (int cand = TN; cand >= 128; cand -= 16) {
-    const int64_t et = (m + cand - 1) / cand;
-    int per = units / q_tiles; if (per < 1) per = 1; if (per > et) per = (int)et;
-    const int64_t tiles_per_cta = (et + per - 1) / per;                  // largest e-range of a work item
-    const int64_t waves = ((int64_t)q_tiles * per + units - 1) / units;  // work items per CTA
-    const int64_t cost = waves * tiles_per_cta * cand + tiles_per_cta * 24;   // + per-tile fixed overhead
-    if (best_cost < 0 || cost < best_cost) { best_cost = cost; tn = cand; }
-  }
-  e_tiles = (int)((m + tn - 1) / tn);
-  int per = units / q_tiles;
+  e_tiles = (int)((m + TN - 1) / TN);
+  int per = num_sms() / q_tiles;
   if (per < 1) per = 1;
   if (per > e_tiles) per = e_tiles;
   echunks = per;
 }
 
-template <int EPI, int PASSES>
-int launch_k(const CUtensorMap& a, const CUtensorMap& c, const TcParams& prm, int grid, cudaStream_t st) {
-  auto kern = pairwise_tc_kernel<EPI, PASSES>;
+template <int EPI, int MODE>
+int launch_k(const CUtensorMap (&maps)[4], const TcParams& prm, cudaStream_t st) {
+  auto kern = pairwise_tc_kernel<EPI, MODE>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(pairwise_tc_kernel)");
+  const int total = prm.q_tiles * prm.echunks * prm.ksplit;
+  const int grid = total < num_sms() ? total : num_sms();
   profile_begin(st);
-  kern<<<grid, NTHREADS, SMEM_BYTES, st>>>(a, c, prm);
+  kern<<<grid, ModeCfg<MODE>::NTHREADS, SMEM_BYTES, st>>>(maps[0], maps[1], maps[2], maps[3], prm);
   profile_end(st);
   B2K_LAUNCH_CHECK("pairwise_tc_kernel");
   return 0;
 }
 
-template <int EPI>
-int launch_e(int passes, const CUtensorMap& a, const CUtensorMap& c, const TcParams& prm, int grid, cudaStream_t st) {
-  if (passes == 3) return launch_k<EPI, 3>(a, c, prm, grid, st);
-  if (passes == 2) return launch_k<EPI, 2>(a, c, prm, grid, st);
-  return launch_k<EPI, 1>(a, c, prm, grid, st);
+template <int MODE>
+int launch_mode(int epi_kind, const CUtensorMap (&maps)[4], const TcParams& prm, cudaStream_t st) {
+  switch (epi_kind) {
+    case EPI_STORE: return launch_k<EPI_STORE, MODE>(maps, prm, st);
+    case EPI_BCE:   return launch_k<EPI_BCE, MODE>(maps, prm, st);
+    case EPI_KL:    return launch_k<EPI_KL, MODE>(maps, prm, st);
+    case EPI_RANK:  return launch_k<EPI_RANK, MODE>(maps, prm, st);
+  }
+  set_error("bad epilogue kind %d", epi_kind);
+  return B200KGE_ERR_INVALID;
 }
 
 }  // namespace
 
 bool tc_supported(int pair_op, int K, const Rows& cand, int col_off) {
   if (pair_op != PAIR_DOT) return false;
-  if (K < TK) return false;
+  if (K < 32) return false;
   if (cand.ld % 4 != 0 || col_off % 4 != 0) return false;
   if ((reinterpret_cast<uintptr_t>(cand.base) & 15) != 0) return false;
   if (cand.rows >= (1ll << 31)) return false;
@@ -339,35 +320,61 @@ bool tc_supported(int pair_op, int K, const Rows& cand, int col_off) {
 }
 
 int tc_nchunks(int64_t nq, int64_t m) {
-  int qt, et, ec, tn;
-  plan(nq, m, qt, et, ec, tn);
+  int qt, et, ec;
+  plan(nq, m, qt, et, ec);
   return 2 * ec;
 }
 
+// in-kernel split of raw fp32 operands: passes 1 = TF32, 2 = MIXED, 3 = TF32X3
 int launch_pairwise_tc(int epi_kind, int passes, const float* Q, int64_t ldq,
                        int64_t nq, const float* T, int64_t ldt, int64_t m, int K,
                        const EpiParams& P, cudaStream_t st) {
   if (nq == 0 || m == 0) return 0;
-  CUtensorMap mQ, mT;
+  CUtensorMap maps[4];
   int rc;
-  if ((rc = tc::make_map(&mQ, Q, nq, K, ldq, TK, TM))) return rc;
+  if ((rc = tc::make_map(&maps[0], Q, nq, K, ldq, 32, TM))) return rc;
+  if ((rc = tc::make_map(&maps[1], T, m, K, ldt, 32, TN))) return rc;
+  maps[2] = maps[0]; maps[3] = maps[1];
   TcParams prm;
-  prm.nq = nq; prm.m = m; prm.K = K;
-  plan(nq, m, prm.q_tiles, prm.e_tiles, prm.echunks, prm.tn);
-  if ((rc = tc::make_map(&mT, T, m, K, ldt, TK, prm.tn))) return rc;
+  prm.nq = nq; prm.m = m; prm.nk = (K + 31) / 32;
+  plan(nq, m, prm.q_tiles, prm.e_tiles, prm.echunks);
+  prm.ksplit = 1; prm.kseg = prm.nk;
+  prm.q_scale = nullptr; prm.t_scale = nullptr;
   prm.epi = P;
-  prm.epi.nchunks = 2 * prm.echunks;   // two epilogue warps (column halves) per row
-  { const char* e = getenv("B200KGE_DBG"); prm.dbg = e ? atoi(e) : 0; }
-  const int total = prm.q_tiles * prm.echunks;
-  const int grid = total < num_sms() ? total : num_sms();
-  switch (epi_kind) {
-    case EPI_STORE: return launch_e<EPI_STORE>(passes, mQ, mT, prm, grid, st);
-    case EPI_BCE:   return launch_e<EPI_BCE>(passes, mQ, mT, prm, grid, st);
-    case EPI_KL:    return launch_e<EPI_KL>(passes, mQ, mT, prm, grid, st);
-    case EPI_RANK:  return launch_e<EPI_RANK>(passes, mQ, mT, prm, grid, st);
+  prm.epi.nchunks = 2 * prm.echunks;   // two epilogue threads (column halves) per row
+  if (passes == 3) return launch_mode<MODE_TF32X3>(epi_kind, maps, prm, st);
+  if (passes == 2) return launch_mode<MODE_MIXED>(epi_kind, maps, prm, st);
+  return launch_mode<MODE_TF32>(epi_kind, maps, prm, st);
+}
+
+// pre-split fp16 planes (F16X3)
+int launch_pairwise_tc3(int epi_kind, const SplitSet& Q, const SplitSet& T, const EpiParams& P, cudaStream_t st) {
+  const int64_t nq = Q.rows, m = T.rows;
+  if (nq == 0 || m == 0) return 0;
+  if (Q.Kp != T.Kp || Q.Kp % 64 != 0) { set_error("operand planes disagree on the padded reduction length"); return B200KGE_ERR_INVALID; }
+  TcParams prm;
+  prm.nq = nq; prm.m = m; prm.nk = Q.Kp / 64;
+  plan(nq, m, prm.q_tiles, prm.e_tiles, prm.echunks);
+  prm.ksplit = 1; prm.kseg = prm.nk;
+  if (P.accumulate_out) {
+    // split-K GEMM: segments of 8 chunks (512 reduction elements) bound the tensor core's accumulator error, which
+    // grows with the reduction length; segment results are added in fp32 by the epilogue (red.global.add).  One
+    // entity tile per work item.
+    if (epi_kind != EPI_STORE) { set_error("split-K accumulation is a GEMM (store) mode"); return B200KGE_ERR_INVALID; }
+    prm.kseg = 8;
+    prm.ksplit = (prm.nk + prm.kseg - 1) / prm.kseg;
+    prm.echunks = prm.e_tiles;
   }
-  set_error("bad epilogue kind %d", epi_kind);
-  return B200KGE_ERR_INVALID;
+  prm.q_scale = Q.inv_scale; prm.t_scale = T.inv_scale;
+  CUtensorMap maps[4];
+  int rc;
+  if ((rc = tc::make_map_f16(&maps[0], Q.hi, nq, Q.Kp, Q.Kp, TM))) return rc;
+  if ((rc = tc::make_map_f16(&maps[1], T.hi, m, T.Kp, T.Kp, TN))) return rc;
+  if ((rc = tc::make_map_f16(&maps[2], Q.lo, nq, Q.Kp, Q.Kp, TM))) return rc;
+  if ((rc = tc::make_map_f16(&maps[3], T.lo, m, T.Kp, T.Kp, TN))) return rc;
+  prm.epi = P;
+  prm.epi.nchunks = 2 * prm.echunks;
+  return launch_mode<MODE_F16X3>(epi_kind, maps, prm, st);
 }
 
 }  // namespace b200kge

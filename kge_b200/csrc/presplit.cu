@@ -1,4 +1,4 @@
-// presplit.cu — operand split for the pre-split fp16 tensor-core kernels (pairwise_tc3.cu, pairwise_tc4.cu): the
+// presplit.cu — operand split for the pre-split fp16 tensor-core kernel (pairwise_tc.cu, F16X3 mode): the
 // default path of the dot family (B200KGE_PREC_AUTO / F16X3).
 //
 // A fp32 value x of row r is represented as  x = inv_scale[r] * (hi + lo),  hi = fp16_rn(x * 2^s),
@@ -150,8 +150,8 @@ presplit_longrow_kernel(const SplitSet A, const SplitSet B, const int rows_a) {
 //                      (o_b, p_b) for _po (b >= n) into shared memory, row scale, hi/lo planes, inverse scale, and
 //                      the row's label (o_b | s_b); block 0 also zeroes the finalisation ticket
 //   blocks [2n, ...) : table rows, one warp per row (presplit_row)
-// replaces prep_1vsall_kernel + presplit_kernel (one launch and one launch gap less per step: 15.0 us against
-// 5.3 + 11.7 us measured; the folded fp32 query matrix never reaches HBM).
+// replaces prep_1vsall_kernel + presplit_kernel (one launch and one launch gap less per step; the folded fp32 query
+// matrix never reaches HBM).
 constexpr int PQ_THREADS = PS_WARPS * 32;
 
 template <int MODEL>

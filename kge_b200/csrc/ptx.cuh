@@ -1,5 +1,5 @@
-// ptx.cuh — thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05
-// (alloc / mma kind::tf32 / commit / ld), proxy fences.  No CUTLASS dependency.
+// ptx.cuh — thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma),
+// proxy fences.  No CUTLASS dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -36,20 +36,6 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t}"
-      ::"r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-}
-
-// Bounded variants for kernels that have not run on hardware yet (pairwise_tc3 / tc4): a protocol bug shows up
-// as a trap ("unspecified launch failure") after ~2^24 polls instead of a hang that only a timeout ends.
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -59,34 +45,20 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
   return ok != 0;
 }
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  return ok != 0;
-}
+// Bounded wait: a protocol bug shows up as a trap ("unspecified launch failure") after ~2^24 polls instead of a
+// hang that only a timeout ends.
 __device__ __forceinline__ void mbar_wait_bounded(uint64_t* bar, uint32_t parity) {
   for (uint32_t polls = 0; !mbar_try_wait(bar, parity); ++polls)
     if (polls > (1u << 24)) __trap();
 }
-__device__ __forceinline__ void mbar_wait_cluster_bounded(uint64_t* bar, uint32_t parity) {
-  for (uint32_t polls = 0; !mbar_try_wait_cluster(bar, parity); ++polls)
-    if (polls > (1u << 24)) __trap();
-}
 
-// ---- proxy / tcgen05 fences -----------------------------------------------------------------
-// generic-proxy smem writes -> visible to the async proxy (TMA / UMMA operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+// named barrier over `nthreads` threads (a warpgroup: 128)
+__device__ __forceinline__ void bar_sync(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
 // ---- TMA ------------------------------------------------------------------------------------
@@ -104,189 +76,62 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// Same load for CTA pairs: with .cta_group::2 the completion bytes may be signalled on an mbarrier in the PEER
-// CTA (given by its shared::cluster address), so both CTAs' loads complete on the leader's barrier — the form
-// CUTLASS's SM100_TMA_2SM_LOAD uses (cute/arch/copy_sm100_tma.hpp).
-__device__ __forceinline__ void tma_load_2d_cluster_bar(void* smem_dst, const CUtensorMap* m, uint32_t bar_cluster_addr,
-                                                        int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
+// ---- wgmma ----------------------------------------------------------------------------------
+// Shared-memory matrix descriptor of a K-major operand in the 128-byte (rows of 128 B, 8-row groups 1024 B apart)
+// or 64-byte (rows of 64 B, groups 512 B apart) swizzled layout TMA writes.  Fields: start address >> 4 [0,14),
+// leading byte offset >> 4 [16,30) (unused for swizzled K-major), stride byte offset >> 4 [32,46), layout type
+// [62,64) (1 = 128B swizzle, 2 = 64B swizzle).  Stepping along K inside a row adds bytes to the start address.
+__device__ __forceinline__ uint64_t wg_desc_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
+         ((uint64_t)1 << 62);
+}
+__device__ __forceinline__ uint64_t wg_desc_sw64(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(512 >> 4) << 32) |
+         ((uint64_t)2 << 62);
 }
 
-// ---- TMEM -----------------------------------------------------------------------------------
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// 32 lanes x 32 consecutive 32-bit columns: thread t of the warp receives lane (base_lane + t).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+// D[64 x 128] += A[64 x K] * B[128 x K]^T, both operands K-major in shared memory, fp32 accumulator in registers:
+// thread t of the warpgroup holds d[4*j + i] = D[16*(t/32) + (t%32)/4 + 8*(i/2)][8*j + 2*(t%4) + (i%2)].
+#define B2K_WG_D64                                                                                               \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                     \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                            \
+  "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                            \
+  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define B2K_WG_OUT64(d)                                                                                          \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),              \
+  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),        \
+  "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),      \
+  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),      \
+  "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),      \
+  "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),      \
+  "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),      \
+  "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
 
-// ---- UMMA -----------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle: rows of 128 B, 8-row
-// groups 1024 B apart (SBO), version 1 (Blackwell), layout type 2 (SWIZZLE_128B).
-// Field layout: cute/arch/mma_sm100_desc.hpp (UMMA::SmemDescriptor).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);  // start address, bits [0,14)
-  d |= (uint64_t)1 << 16;                        // leading byte offset (unused for SW128 K-major)
-  d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                        // descriptor version
-  d |= (uint64_t)2 << 61;                        // SWIZZLE_128B
-  return d;
+// k = 16, IEEE half operands
+__device__ __forceinline__ void wgmma_f16(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " B2K_WG_D64 ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+               : B2K_WG_OUT64(d) : "l"(adesc), "l"(bdesc) : "memory");
 }
-
-// Instruction descriptor for kind::tf32, fp32 accumulate, both operands K-major.
-// Field layout: UMMA::InstrDescriptor (c_format [4,6), a_format [7,10), b_format [10,13),
-// n_dim [17,23) = N>>3, m_dim [24,29) = M>>4).
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// k = 16, bf16 operands
+__device__ __forceinline__ void wgmma_bf16(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " B2K_WG_D64 ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+               : B2K_WG_OUT64(d) : "l"(adesc), "l"(bdesc) : "memory");
 }
-
-// Instruction descriptor for kind::f16 with bf16 operands, fp32 accumulate, both operands K-major.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// k = 8, tf32 operands (fp32 bit patterns; the low 13 mantissa bits are not used)
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " B2K_WG_D64 ", %64, %65, p, 1, 1;\n\t}"
+               : B2K_WG_OUT64(d) : "l"(adesc), "l"(bdesc) : "memory");
 }
-// Same kind with fp16 (IEEE half) operands: a_format = b_format = 0.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// kind::f16 MMA; the operand type (bf16 / fp16) is carried by the instruction descriptor.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]^T, issued by ONE thread.
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued MMAs of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-
-// ---- clusters / CTA pairs (cta_group::2) ------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `local` (a shared::cta address) in CTA `rank` of this cluster
-__device__ __forceinline__ uint32_t mapa(uint32_t local, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local), "r"(rank));
-  return r;
-}
-// arrive (release at cluster scope) on an mbarrier that may live in the peer CTA
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// wait with acquire at cluster scope (pairs with mbar_arrive_cluster / multicast commits)
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAITC_%=:\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONEC_%=;\n\t"
-      "bra WAITC_%=;\n\t"
-      "DONEC_%=:\n\t}"
-      ::"r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-}
-
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_result) {  // same warp id in both CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-
-// Shared-memory matrix descriptor, K-major, 64-byte swizzle (rows of 64 B, 8-row groups 512 B apart).
-__device__ __forceinline__ uint64_t umma_desc_sw64(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(512 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)4 << 61;                        // SWIZZLE_64B
-  return d;
-}
-
-// D[tmem of both CTAs] (+)= A * B^T over a CTA pair: M = 256 (128 rows from each CTA's smem),
-// N = 256 (128 rows of B from each CTA's smem).  Issued by ONE thread of the leader CTA.
-__device__ __forceinline__ void umma_tf32_2cta(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2cta(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit -> arrive on the mbarrier at this smem offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
+#undef B2K_WG_D64
+#undef B2K_WG_OUT64
 
 }  // namespace ptx
 }  // namespace b200kge

@@ -1,4 +1,4 @@
-// tc_common.cuh — pieces shared by the tcgen05 kernels (pairwise_tc.cu, pairwise_tc3.cu, pairwise_tc4.cu).
+// tc_common.cuh — pieces shared by the tensor-core scorer (pairwise_tc.cu) and its callers.
 #pragma once
 #include <cuda.h>
 #include <cstdlib>
@@ -16,8 +16,11 @@ __device__ __forceinline__ float tf32_rna(float x) {
   return __uint_as_float(u);
 }
 
-// lo = rn_tf32(x - trunc_tf32(x)) for 4 packed floats (hi needs no write: kind::tf32 ignores the low
-// 13 mantissa bits of a raw fp32 operand — truncation, measured on B200).
+__device__ __forceinline__ float4 trunc_tf32_4(const float4 v) {
+  return make_float4(__uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u), __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u),
+                     __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u), __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u));
+}
+// lo = rn_tf32(x - trunc_tf32(x)) for 4 packed floats
 __device__ __forceinline__ float4 split_lo4(const float4 v) {
   float4 l;
   l.x = tf32_rna(v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u));
@@ -39,8 +42,9 @@ __device__ __forceinline__ void sts128(uint32_t addr, const float4 v) {
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
-// lo tile = split_lo(raw tile) for NBYTES bytes, by `nthreads` threads (thread index t); all loads
-// of a thread are issued before its stores so the smem latency is paid once.
+// lo tile = split_lo(raw tile) for NBYTES bytes, by `nthreads` threads (thread index t); the raw tile is
+// rewritten as trunc_tf32(raw), so the tf32 MMA's hi operand is exact whether the tensor core truncates or rounds
+// the low mantissa bits.  All loads of a thread are issued before its stores so the smem latency is paid once.
 template <int NBYTES, int NTHR>
 __device__ __forceinline__ void split_tile(uint32_t src, uint32_t dst, int t) {
   constexpr int PER = NBYTES / 16 / NTHR;   // float4s per thread
@@ -49,13 +53,17 @@ __device__ __forceinline__ void split_tile(uint32_t src, uint32_t dst, int t) {
 #pragma unroll
   for (int i = 0; i < PER; ++i) v[i] = lds128(src + (uint32_t)(t + i * NTHR) * 16u);
 #pragma unroll
-  for (int i = 0; i < PER; ++i) sts128(dst + (uint32_t)(t + i * NTHR) * 16u, split_lo4(v[i]));
+  for (int i = 0; i < PER; ++i) {
+    sts128(dst + (uint32_t)(t + i * NTHR) * 16u, split_lo4(v[i]));
+    sts128(src + (uint32_t)(t + i * NTHR) * 16u, trunc_tf32_4(v[i]));
+  }
 }
 
 // Mixed mode (tf32 hi*hi + bf16 cross terms): from a raw fp32 K-major tile [ROWS][32] in the 128-B
 // swizzled layout, derive two bf16 K-major tiles [ROWS][32] in the 64-B swizzled layout:
 //   hi16 = bf16_rn(x)            (hi operand of the cross terms)
-//   lo16 = bf16_rn(x - trunc_tf32(x))   (remainder w.r.t. what the tf32 MMA uses as hi)
+//   lo16 = bf16_rn(x - trunc_tf32(x))   (remainder w.r.t. the tf32 MMA's hi operand)
+// and rewrite the raw tile as trunc_tf32(x) (the tf32 MMA's hi operand, exact in tf32).
 // One item = (row r, group c of 8 consecutive k): reads fp32 16-B chunks 2c, 2c+1 of row r (physical
 // chunk = logical ^ (r & 7)), writes bf16 16-B chunk c of row r (physical = c ^ ((r >> 1) & 3)).
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
@@ -86,6 +94,9 @@ __device__ __forceinline__ void split_tile_bf16(uint32_t src, uint32_t dst_hi, u
     float lo[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) lo[k] = x[k] - __uint_as_float(__float_as_uint(x[k]) & 0xFFFFE000u);
+    const uint32_t roff = (uint32_t)(i * RSTEP * 128);
+    sts128(s0 + roff, trunc_tf32_4(v0[i]));
+    sts128(s1 + roff, trunc_tf32_4(v1[i]));
     const uint32_t off = doff + (uint32_t)(i * RSTEP * 64);
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst_hi + off), "r"(pack_bf16x2(x[0], x[1])),
                  "r"(pack_bf16x2(x[2], x[3])), "r"(pack_bf16x2(x[4], x[5])), "r"(pack_bf16x2(x[6], x[7])) : "memory");
@@ -94,18 +105,12 @@ __device__ __forceinline__ void split_tile_bf16(uint32_t src, uint32_t dst_hi, u
   }
 }
 
-// Epilogue.  TMEM lane = query row, so one thread owns one row and walks 32-column chunks.
-// The first version fed every element through the generic epi_elem functor: ~43 SASS instructions
-// per element (64-bit bounds/label compares, per-element null checks of optional operands) on ONE
-// warp per SM sub-partition — the whole kernel was epilogue-bound (profiles/r1_notes.md).  Here:
-// warp-uniform fast paths for full chunks, optional operands resolved once per chunk, the one-hot
-// label handled outside the element loop, and TWO epilogue warps per sub-partition (each takes
-// half of the accumulator's columns) so dependent-issue latency is hidden.
+// Epilogue.  The accumulator tile is staged in shared memory with one row per thread, so one thread owns
+// one query row and walks 32-column chunks; every per-row reduction is thread-local.  Warp-uniform fast
+// paths for full chunks, optional operands resolved once per chunk, the one-hot label handled outside the
+// element loop, and two threads per row (each takes half of the tile's columns).
 
 constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
-constexpr int EPI_WARPS = 8;    // warps 4..11: quadrant = warp % 4 (TMEM lanes), half = (warp-4)/4 (columns)
-constexpr int SPLIT_WARPS = 4;  // warps 12..15
-constexpr int NTHREADS = 16 * 32;
 
 __device__ __forceinline__ float fast_ex2(float x) {
   float y;
@@ -207,14 +212,14 @@ __device__ __forceinline__ void epi_chunk32(const EpiParams& P, RowState<EPI>& s
   }
 }
 
-// Epilogue of NCH 32-column chunks of one accumulator for the warp owning TMEM lanes
-// [32*quadrant, +32) and columns [col_first, col_first + 32*NCH) of the tile.
-// SCALED (pre-split fp16 kernel, pairwise_tc3.cu): the accumulator holds the product of row-scaled
+// Epilogue of NCH 32-column chunks of one accumulator tile for the warp owning 32 of its rows and columns
+// [col_first, col_first + 32*NCH); `acc` points at this thread's row, first column of the span.
+// SCALED (pre-split fp16 planes): the accumulator holds the product of row-scaled
 // operands; score = acc * row_scale * col_scale[column] (both exact powers of two).  col_scale must be
 // readable (and 16-byte aligned) for 32 floats from any chunk start < m.
 template <int EPI, int NCH, bool SCALED = false>
 __device__ __forceinline__ void epilogue_tile(const EpiParams& P, RowState<EPI>& st, float aux,
-                                              uint32_t tmem_acc /* base + lane<<16 + first column */,
+                                              const float* acc,
                                               int64_t tile_row0 /* first row of this warp's 32 */,
                                               int64_t e0 /* global column of the first chunk */, int64_t nq,
                                               int64_t m, float* my_stg, int lane, float row_scale = 1.f,
@@ -230,12 +235,12 @@ __device__ __forceinline__ void epilogue_tile(const EpiParams& P, RowState<EPI>&
     const int64_t c0 = e0 + j * 32;
     if (c0 >= m) break;                                   // warp-uniform: chunk entirely out of range
     uint32_t v[32];
-    ptx::tmem_ld_32x32(tmem_acc + (uint32_t)(j * 32), v);
+#pragma unroll
+    for (int c = 0; c < 32; ++c) v[c] = __float_as_uint(acc[j * 32 + c]);
     if constexpr (SCALED) {
       float4 cs[8];
 #pragma unroll
       for (int g = 0; g < 8; ++g) cs[g] = __ldg(reinterpret_cast<const float4*>(col_scale + c0) + g);
-      ptx::tmem_ld_wait();
 #pragma unroll
       for (int g = 0; g < 8; ++g) {
         v[4 * g + 0] = __float_as_uint(__uint_as_float(v[4 * g + 0]) * (row_scale * cs[g].x));
@@ -243,8 +248,6 @@ __device__ __forceinline__ void epilogue_tile(const EpiParams& P, RowState<EPI>&
         v[4 * g + 2] = __float_as_uint(__uint_as_float(v[4 * g + 2]) * (row_scale * cs[g].z));
         v[4 * g + 3] = __float_as_uint(__uint_as_float(v[4 * g + 3]) * (row_scale * cs[g].w));
       }
-    } else {
-      ptx::tmem_ld_wait();
     }
     if (csr_cur < csr_end) {
       // listed columns of this row inside [c0, c0 + 32): emit their scores (losses) or filter them (rank)
@@ -418,15 +421,14 @@ inline int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
 
 }  // namespace tc
 
-// Pre-split fp16 kernels (presplit.cu + pairwise_tc3.cu / pairwise_tc4.cu), experimental: B200KGE_TC_VERSION=3|4.
-// One row set of the operand split: rows of `src` (optionally gathered through idx, starting at column
+// Pre-split fp16 path (presplit.cu + pairwise_tc.cu).  One row set of the operand split: rows of `src` (optionally gathered through idx, starting at column
 // col_off, K columns) -> hi/lo fp16 planes [rows, Kp] (Kp = round_up(K, 64), zero padded) and the
 // per-row power-of-two factor inv_scale[rows_pad] that undoes the row scaling (0 beyond `rows`).
 struct SplitSet {
@@ -440,11 +442,7 @@ int launch_presplit(const SplitSet& A, const SplitSet& B, cudaStream_t st);   //
 int launch_prep_split_1vsall(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n,
                              const SplitSet& Qs, const SplitSet& Ts, int64_t* labels2n, unsigned int* ticket,
                              cudaStream_t st);
-int tc3_nchunks(int64_t nq, int64_t m);
 int launch_pairwise_tc3(int epi_kind, const SplitSet& Q, const SplitSet& T, const EpiParams& P, cudaStream_t st);
-// CTA-pair version on the same planes (pairwise_tc4.cu), experimental: B200KGE_TC_VERSION=4.
-int tc4_nchunks(int64_t nq, int64_t m);
-int launch_pairwise_tc4(int epi_kind, const SplitSet& Q, const SplitSet& T, const EpiParams& P, cudaStream_t st);
 
 // Backward pieces (grad.cu), experimental.
 int launch_transpose(const float* src, int64_t lds, int64_t R, int64_t C, float* dst, int64_t ldd, cudaStream_t st);

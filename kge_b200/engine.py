@@ -1,7 +1,7 @@
 """Tensor-level façade over the C ABI: torch CUDA tensors in, torch CUDA tensors out.
 
 torch is used for device memory (caching allocator), streams and nothing else: every number is
-produced by libb200kge's hand-written sm_100a kernels.  All functions raise on CPU tensors.
+produced by libb200kge's hand-written sm_90a kernels.  All functions raise on CPU tensors.
 """
 from __future__ import annotations
 
@@ -20,7 +20,7 @@ def _require_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
             raise RuntimeError(
-                "kge_b200 runs on CUDA (sm_100) tensors only; there is no CPU path "
+                "kge_b200 runs on CUDA (sm_90) tensors only; there is no CPU path "
                 f"(got a tensor on {t.device})"
             )
 
@@ -380,7 +380,7 @@ def sample_uniform(n: int, K: int, vocab: int, seed: int, offset: int, device) -
     lib = _lib.load()
     out = torch.empty((n, K), dtype=torch.int64, device=device)
     if not out.is_cuda:
-        raise RuntimeError("kge_b200 runs on CUDA (sm_100) tensors only; there is no CPU path")
+        raise RuntimeError("kge_b200 runs on CUDA (sm_90) tensors only; there is no CPU path")
     _lib.check(lib.b200kge_sample_uniform(seed & (2 ** 64 - 1), offset & (2 ** 64 - 1), vocab, n, K, out.data_ptr(),
                                           _stream(out.device)))
     return out
@@ -482,7 +482,7 @@ class HostStep:
         return float(self.loss_host[0])
 
 
-# ---- SURVEY 8f rows (gradients, penalties, CSR labels): validated on a B200 in round 2 -------------------------
+# ---- SURVEY 8f rows (gradients, penalties, CSR labels) ---------------------------------------------------------
 def gemm_nt(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     """C = A @ B^T (fp32 in/out) on the f16 tensor pipe from pre-split hi/lo fp16 planes."""
     _require_cuda(a, b)

@@ -11,7 +11,7 @@ Same names, argument meaning and error behaviour as LibKGE's
                                                                          eval_entity_ranking.py:533-618
 
 but standalone (the reference package is not required) and with every number produced by
-libb200kge's sm_100a kernels.  The LibKGE plugin (kge_b200/plugin) wraps the same engine calls in
+libb200kge's sm_90a kernels.  The LibKGE plugin (kge_b200/plugin) wraps the same engine calls in
 subclasses of the reference's own classes.  Forward only: backward is row (f)1 of SURVEY.md 8.
 """
 from __future__ import annotations

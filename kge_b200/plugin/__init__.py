@@ -43,7 +43,7 @@ from .. import engine
 
 
 class _ScoreEmbFn(torch.autograd.Function):
-    """Forward: sm_100a kernels.  Backward: recompute with the reference's dense expression."""
+    """Forward: sm_90a kernels.  Backward: recompute with the reference's dense expression."""
 
     @staticmethod
     def forward(ctx, scorer, ref_score_emb, combine, s_emb, p_emb, o_emb):
@@ -100,7 +100,7 @@ def _scorer(name, base):
 
 
 class _TableScoreFn(torch.autograd.Function):
-    """Index-level scoring that reads the embedding tables in place.  Forward: sm_100a kernels (gather fused,
+    """Index-level scoring that reads the embedding tables in place.  Forward: sm_90a kernels (gather fused,
     no `embed_all()` copy).  Backward: `model._b200_score_backward` (gradient kernels where validated, else
     recomputation through the reference's dense expression)."""
 

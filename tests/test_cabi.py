@@ -1,4 +1,4 @@
-"""CPU tests of the boundary: the C-ABI library builds for sm_100a, loads, exports every symbol
+"""CPU tests of the boundary: the C-ABI library builds for sm_90a, loads, exports every symbol
 include/b200kge.h declares, and refuses to compute without a GPU (no CPU fallback)."""
 import os
 import re
@@ -30,7 +30,7 @@ def test_header_symbols_all_exported(lib):
     assert lib.b200kge_version() == 100
 
 
-def test_sass_is_blackwell_native():
+def test_sass_is_hopper_native():
     import shutil
     import subprocess
 
@@ -39,8 +39,8 @@ def test_sass_is_blackwell_native():
     from kge_b200._lib import LIB_PATH
 
     sass = subprocess.run(["cuobjdump", "-sass", LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM"):   # tcgen05.mma / TMA / tcgen05.ld
+    assert "sm_90a" in sass
+    for mnemonic in ("HGMMA", "UTMALDG"):   # wgmma / TMA
         assert mnemonic in sass, mnemonic
 
 
@@ -49,7 +49,7 @@ def test_no_cpu_fallback(lib):
     from kge_b200 import KgeModel, engine
 
     assert lib.b200kge_device_ok() != 0
-    assert b"no CPU fallback" in lib.b200kge_last_error() or b"not sm_100" in lib.b200kge_last_error()
+    assert b"no CPU fallback" in lib.b200kge_last_error() or b"not sm_90" in lib.b200kge_last_error()
     m = KgeModel("complex", 10, 2, 8)
     idx = torch.tensor([0, 1])
     with pytest.raises(RuntimeError):

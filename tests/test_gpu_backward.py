@@ -1,4 +1,4 @@
-"""Parity tests of the gradient kernels (SURVEY 8f-1), validated on a B200 in round 2: the pre-split fp16 GEMM with
+"""Parity tests of the gradient kernels (SURVEY 8f-1): the pre-split fp16 GEMM with
 split-K accumulation, the analytic backward of the fused 1vsAll step (dot family, BCE and KL) against gradients
 of the live reference (tests/golden/grads_*.npz) and against the CPU algebra at medium sizes, and the fused
 negative-sampling backward."""

@@ -22,7 +22,7 @@ def eng():
     from kge_b200 import engine
 
     assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    assert engine.device_ok(), "libb200kge needs an sm_100 device"
+    assert engine.device_ok(), "libb200kge needs an sm_90 (H100) device"
     return engine
 
 
@@ -64,7 +64,7 @@ def test_golden_scores(eng, fname):
 
 
 def test_golden_scores_tensor_core(eng):
-    """Forces the tcgen05 3xTF32 kernel on the golden cases it can take (dot family, K >= 32)."""
+    """Forces the 3xTF32 tensor-core kernel on the golden cases it can take (dot family, K >= 32)."""
     for fname, model in (("scores_complex.npz", "complex"), ("scores_distmult.npz", "distmult"),
                          ("scores_simple.npz", "simple"), ("scores_complex_sigma01.npz", "complex")):
         g = _load(fname)
@@ -100,9 +100,8 @@ def test_oracle_medium(eng, model, D, sigma):
 
 @pytest.mark.parametrize("version,tk", [("1", "32"), ("2", "32"), ("2", "16")])
 def test_tensor_core_kernel_variants(eng, monkeypatch, version, tk):
-    """1-CTA kernel and the CTA-pair (cta_group::2) kernel in both K-chunk/swizzle configurations, in the
-    3xTF32 and the mixed split modes: dense scores, fused BCE/KL, fused rank counting; ragged sizes
-    (tiles cut in both dimensions, odd number of query tiles)."""
+    """In-kernel split of raw fp32 operands in the 3xTF32 and the mixed split modes: dense scores, fused BCE/KL,
+    fused rank counting; ragged sizes (tiles cut in both dimensions, odd number of query tiles)."""
     monkeypatch.setenv("B200KGE_TC_VERSION", version)
     monkeypatch.setenv("B200KGE_TC2_TK", tk)
     for model, D, prec in (("complex", 192, "3xtf32"), ("complex", 192, "tf32+bf16x2"), ("distmult", 64, "tf32+bf16x2"),

@@ -1,6 +1,6 @@
 """Parity tests of the default tensor-core path: operands pre-split into row-scaled fp16 hi/lo planes
-(presplit.cu) scored by pairwise_tc3.cu (AUTO / precision "f16x3"), and of its CTA-pair version pairwise_tc4.cu
-(B200KGE_TC_VERSION=4).  Bar: floating point <= 1e-4 * rms, rank/tie counts bit-exact on the kernel's own scores."""
+(presplit.cu) scored by pairwise_tc.cu (AUTO / precision "f16x3").  Bar: floating point <= 1e-4 * rms, rank/tie
+counts bit-exact on the kernel's own scores."""
 import os
 
 import numpy as np
@@ -38,19 +38,16 @@ def _assert_close(got, ref, what, tol=TOL):
     assert err <= tol * rms, f"{what}: max|d|={err:.3e} rms={rms:.3e} ratio={err / rms:.2e}"
 
 
-VARIANTS = [("3", "1", "64"), ("4", "1", "64")]
-# (B200KGE_TC_VERSION, B200KGE_TC4_DIRECT, B200KGE_TC3_TK)
+VARIANTS = ["3"]   # B200KGE_TC_VERSION
 
 
-@pytest.fixture(params=VARIANTS, ids=["tc3", "tc4-pair"])
+@pytest.fixture(params=VARIANTS, ids=["tc3"])
 def variant(request, monkeypatch):
-    """Selects the experimental kernel for the duration of a test (the default path is restored afterwards)."""
-    ver, direct, tk = request.param
+    """Selects the kernel for the duration of a test (the default path is restored afterwards)."""
+    ver = request.param
 
     def select():
         monkeypatch.setenv("B200KGE_TC_VERSION", ver)
-        monkeypatch.setenv("B200KGE_TC4_DIRECT", direct)
-        monkeypatch.setenv("B200KGE_TC3_TK", tk)
     return select
 
 

@@ -1,5 +1,4 @@
-"""Parity tests of the callers and rows either side of the scorer that were validated on a B200 in round 2
-(SURVEY 8f): the evaluation loop on the fused rank kernels, the reference jobs' traces re-derived on the validated
+"""Parity tests of the callers and rows either side of the scorer (SURVEY 8f): the evaluation loop on the fused rank kernels, the reference jobs' traces re-derived on the validated
 entry points, one negative-sampling training batch, the reciprocal-relations model, Lp/N3 penalties + row
 normalisation, and the KvsAll losses with CSR multi-hot labels."""
 import os
@@ -44,7 +43,7 @@ def test_evaluator_on_gpu_matches_reference_job(model):
     """kge_b200.evaluate.EntityRankingEvaluator driving the fused rank kernels reproduces the reference
     EntityRankingJob's trace (host logic is covered on CPU by tests/test_evaluate_cpu.py; this adds the device
     side: chunked subsets, dense filter planes, accumulation into rank/ties).  To be promoted into
-    tests/test_gpu_model.py once it has run green on a B200."""
+    tests/test_gpu_model.py once it has run green on the GPU."""
     from kge_b200 import KgeModel
     from kge_b200.evaluate import EntityRankingEvaluator
 
@@ -67,7 +66,7 @@ def test_evaluator_on_gpu_matches_reference_job(model):
 @pytest.mark.parametrize("model", ["complex", "transe"])
 def test_job_traces_on_gpu(eng, model):
     """Job-level traces of the reference (tests/golden/jobs_*.npz) through validated entry points only: 1vsAll
-    epoch loss, KvsAll epochs with multi-hot / smoothed labels.  Gated until it has run once on a B200."""
+    epoch loss, KvsAll epochs with multi-hot / smoothed labels.  Gated until it has run once on the GPU."""
     g = _load(f"jobs_{model}.npz")
     ent, rel, train = g["ent"].cuda(), g["rel"].cuda(), g["train"].long().cuda()
     E = ent.shape[0]
@@ -114,7 +113,7 @@ def test_ns_job_batch_on_gpu(eng, model):
 @pytest.mark.parametrize("base", ["complex", "transe"])
 def test_reciprocal_model_on_gpu(base):
     """kge_b200.ReciprocalRelationsModel (index arithmetic over validated `sp_` entry points) against the live
-    reference's ReciprocalRelationsModel.  Gated until it has run once on a B200."""
+    reference's ReciprocalRelationsModel.  Gated until it has run once on the GPU."""
     from kge_b200 import ReciprocalRelationsModel
 
     g = _load(f"reciprocal_{base}.npz")

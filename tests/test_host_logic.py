@@ -56,7 +56,7 @@ def test_bench_reference_arm_runs_on_cpu():
     line = json.loads(r.stdout.strip().splitlines()[-1])
     assert line["impl"] == "reference" and line["unit"] == "triples/s" and line["value"] > 0
     from kge_b200 import hostenv
-    # the live reference's own job when it is installed (scripts/install_ref.sh), else the oracle's restatement
+    # the live reference's own job when it is installed (oracle/install_ref.sh), else the oracle's restatement
     assert line["cpu_baseline"]["kind"] == ("reference" if hostenv.available() else "port")
     assert line["cpu_baseline"]["cores"] >= 1 and line["config"]["workload"].startswith("ComplEx d=512 1vsAll+BCE")
     assert line["e2e"]["h2d_bytes_per_step"] == 0 and line["higher_is_better"] is True
