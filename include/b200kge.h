@@ -79,7 +79,13 @@ typedef enum {
 
 typedef enum {
   B200KGE_LOSS_BCE = 1, /* BCEWithLogitsKgeLoss, reduction sum, + offset  loss.py:153-159 */
-  B200KGE_LOSS_KL = 2   /* KLDivWithSoftmaxKgeLoss (CE for index labels)   loss.py:198-213 */
+  B200KGE_LOSS_KL = 2,  /* KLDivWithSoftmaxKgeLoss (CE for index labels)   loss.py:198-213 */
+  /* the kinds below are row-wise losses of a block with ONE positive per row: b200kge_ns_loss only */
+  B200KGE_LOSS_BCE_MEAN = 3,       /* BCEWithLogitsKgeLoss, bce_type "mean"                 loss.py:160-168 */
+  B200KGE_LOSS_BCE_SELF_ADV = 4,   /* BCEWithLogitsKgeLoss, bce_type "self_adversarial"     loss.py:169-187 */
+  B200KGE_LOSS_MARGIN_RANKING = 5, /* MarginRankingKgeLoss, negative-sampling pairing       loss.py:240-252 */
+  B200KGE_LOSS_SOFT_MARGIN = 6,    /* SoftMarginKgeLoss                                     loss.py:216-224 */
+  B200KGE_LOSS_SE = 7              /* SEKgeLoss (MSELoss, reduction sum)                    loss.py:267-274 */
 } b200kge_loss;
 
 typedef struct {
@@ -218,7 +224,8 @@ int b200kge_shard_gather_rows(const b200kge_rows_t* shard, int64_t lo, const int
                               float* out, int64_t ldo, b200kge_stream_t stream);
 
 /* Dense-score epilogues (for callers that already hold a score matrix) ------------------------ */
-/* KgeLoss on a dense [n,m] score matrix: loss.py:153-159 (BCE) / :198-213 (KL). */
+/* KgeLoss on a dense [n,m] score matrix: loss.py:153-159 (BCE) / :198-213 (KL).  The row-wise kinds
+ * (B200KGE_LOSS_BCE_MEAN and after) return B200KGE_ERR_UNSUPPORTED: use b200kge_ns_loss. */
 int b200kge_loss_dense(const float* scores, int64_t lds, int64_t n, int64_t m,
                        const b200kge_labels_t* labels, int loss_kind, float offset,
                        float* loss_out, float* row_loss_out, void* workspace,
@@ -371,6 +378,33 @@ int b200kge_ns_backward(int model, float l_norm, const b200kge_rows_t* ent, cons
                           const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K,
                           float offset, int64_t batch_size, float* d_ent, int64_t lde, float* d_rel,
                           int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+
+/* KgeLoss of a negative-sampling block (kge/job/train_negative_sampling.py:126-156 with kge/util/loss.py:139-274):
+ * scores [n, m] (row stride lds), one positive per row at column label_idx[i] (NULL: column 0, the layout of
+ * b200kge_ns_score with with_positive = 1), every other column a negative (label 0).  Any b200kge_loss kind; `arg` is
+ * the offset of the BCE kinds and the margin of B200KGE_LOSS_MARGIN_RANKING (ignored otherwise), `temperature` that of
+ * B200KGE_LOSS_BCE_SELF_ADV (user.bce_self_adversarial_temperature, loss.py:64-68).  The row-wise kinds need m >= 2.
+ *   *loss_out       = scale * sum_i loss_i  (fixed-order reduction: deterministic)
+ *   row_loss_out[i] = loss_i                (optional)
+ *   grad_out[i*ldg + c] = scale * dL_i/dz_ic  (optional, [n, m]): the margin-ranking hinge passes the gradient at
+ *                     exactly 0 as torch's clamp_min does; the self-adversarial weights are treated as constants
+ *                     (detached, loss.py:179-181).
+ * workspace: b200kge_ns_loss_workspace_bytes(n). */
+size_t b200kge_ns_loss_workspace_bytes(int64_t n);
+int b200kge_ns_loss(const float* scores, int64_t lds, int64_t n, int64_t m, const int64_t* label_idx,
+                    int loss_kind, float arg, float temperature, float scale, float* loss_out,
+                    float* row_loss_out, float* grad_out, int64_t ldg, void* workspace,
+                    size_t workspace_bytes, b200kge_stream_t stream);
+
+/* b200kge_ns_backward with the gradient of the block given: grad_scores [n, 1+K] (row stride ldg; column 0 the positive,
+ * columns 1.. the sampled ids neg [n, K]) holds dL/dz already scaled (e.g. the grad_out of b200kge_ns_loss with
+ * scale = 1 / batch_size).  The fold, per-column walk, scatter and unfold are those of b200kge_ns_backward; only the
+ * per-column gradient is read instead of computed — so every loss of b200kge_ns_loss trains through the same kernel
+ * (loss.backward() at train_negative_sampling.py:164).  ADDS into d_ent / d_rel; same slots, models and workspace. */
+int b200kge_ns_backward_grad(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                             const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K,
+                             const float* grad_scores, int64_t ldg, float* d_ent, int64_t lde, float* d_rel,
+                             int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
 
 /* LookupEmbedder.penalty (kge/model/embedder/lookup_embedder.py:123-177) on the rows view `rows` (the whole
  * table, or the batch's unique rows through rows->idx with their `counts`, NULL = all ones):

@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(_HERE, "libb200kge.so")
 MODELS = {"complex": 0, "distmult": 1, "simple": 2, "cp": 3, "rescal": 4, "transe": 5, "rotate": 6}
 SP_, _PO = 0, 1
 PREC = {"auto": 0, "fp32": 1, "3xtf32": 2, "tf32": 3, "tf32+bf16x2": 4, "f16x3": 5}
-LOSS = {"bce": 1, "kl": 2}
+LOSS = {"bce": 1, "kl": 2, "bce_mean": 3, "bce_self_adversarial": 4, "margin_ranking": 5, "soft_margin": 6, "se": 7}
 ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA, ERR_WORKSPACE, ERR_NO_DEVICE = -1, -2, -3, -4, -5
 
 
@@ -101,6 +101,13 @@ SIGNATURES = {
     "b200kge_ns_backward": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
                                         C.c_int64, C.c_float, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
                                         C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_ns_loss_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "b200kge_ns_loss": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_float, C.c_float,
+                                  C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t,
+                                  C.c_void_p]),
+    "b200kge_ns_backward_grad": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
+                                           C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                           C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_lookup_penalty": (C.c_int, [_RP, C.c_void_p, C.c_float, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
                                            C.c_size_t, C.c_void_p]),
     "b200kge_normalize_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_float, C.c_void_p]),

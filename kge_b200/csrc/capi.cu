@@ -503,6 +503,7 @@ int b200kge_loss_dense(const float* scores, int64_t lds, int64_t n, int64_t m,
                        size_t workspace_bytes, b200kge_stream_t stream) {
   if (!scores || !labels || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if ((!labels->idx) == (!labels->dense)) { set_error("exactly one of labels.idx / labels.dense must be given"); return B200KGE_ERR_INVALID; }
+  if (loss_kind >= B200KGE_LOSS_BCE_MEAN && loss_kind <= B200KGE_LOSS_SE) { set_error("loss kind %d is row-wise with one positive per row: use b200kge_ns_loss", loss_kind); return B200KGE_ERR_UNSUPPORTED; }
   if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
   if (n == 0 || m == 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
@@ -1065,8 +1066,52 @@ int b200kge_ns_backward(int model, float l_norm, const b200kge_rows_t* ent, cons
   Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
   float* dQ = (float*)ws.take((size_t)n * ldq * 4);
   if (!dQ && n > 0) { set_error("workspace too small (need n * round_up(K,32) floats)"); return B200KGE_ERR_WORKSPACE; }
-  return launch_ns_backward(model, l_norm, E, R, triples, slot, neg, n, K, offset, 1.0f / (float)batch_size, d_ent, lde,
+  return launch_ns_backward(model, l_norm, E, R, triples, slot, neg, n, K, offset, 1.0f / (float)batch_size, nullptr, 0,
+                            d_ent, lde, d_rel, ldr, dQ, ldq, (cudaStream_t)stream);
+}
+
+int b200kge_ns_backward_grad(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                             const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K,
+                             const float* grad_scores, int64_t ldg, float* d_ent, int64_t lde, float* d_rel,
+                             int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+  if (!ent || !rel || !triples || (!neg && n * K > 0) || (!grad_scores && n > 0) || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
+  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
+  if ((rc = validate_norm(model, l_norm))) return rc;
+  if (ldg < K + 1) { set_error("grad_scores is narrower than the 1 + K columns of the block"); return B200KGE_ERR_INVALID; }
+  if (lde < ent->dim || ldr < rel->dim) { set_error("gradient leading dimensions are smaller than the table widths"); return B200KGE_ERR_INVALID; }
+  Rows E = to_rows(ent), R = to_rows(rel);
+  Folded f = folded_problem(model, B200KGE_SP_, E.dim, l_norm);
+  const int64_t ldq = round_up(f.K, 32);
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  float* dQ = (float*)ws.take((size_t)n * ldq * 4);
+  if (!dQ && n > 0) { set_error("workspace too small (need n * round_up(K,32) floats)"); return B200KGE_ERR_WORKSPACE; }
+  return launch_ns_backward(model, l_norm, E, R, triples, slot, neg, n, K, 0.f, 1.f, grad_scores, ldg, d_ent, lde,
                             d_rel, ldr, dQ, ldq, (cudaStream_t)stream);
+}
+
+size_t b200kge_ns_loss_workspace_bytes(int64_t n) { return (size_t)n * 2 * 4 + 256 + 1024; }
+
+int b200kge_ns_loss(const float* scores, int64_t lds, int64_t n, int64_t m, const int64_t* label_idx,
+                    int loss_kind, float arg, float temperature, float scale, float* loss_out,
+                    float* row_loss_out, float* grad_out, int64_t ldg, void* workspace,
+                    size_t workspace_bytes, b200kge_stream_t stream) {
+  if ((!scores && n * m > 0) || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (loss_kind < B200KGE_LOSS_BCE || loss_kind > B200KGE_LOSS_SE) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  if (n > 0 && m < (loss_kind >= B200KGE_LOSS_BCE_MEAN && loss_kind <= B200KGE_LOSS_MARGIN_RANKING ? 2 : 1)) {
+    set_error("loss kind %d needs a positive and at least one negative per row (m = %lld)", loss_kind, (long long)m);
+    return B200KGE_ERR_INVALID;
+  }
+  if (lds < m || (grad_out && ldg < m)) { set_error("row stride smaller than the row width"); return B200KGE_ERR_INVALID; }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n == 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  float* part = (float*)ws.take((size_t)n * 2 * 4);
+  void* scratch = ws.take(1024);
+  if (!part || !scratch) { set_error("workspace too small (need b200kge_ns_loss_workspace_bytes(n) = %zu bytes)", b200kge_ns_loss_workspace_bytes(n)); return B200KGE_ERR_WORKSPACE; }
+  int rc = launch_ns_loss(loss_kind, scores, lds, n, m, label_idx, arg, temperature, scale, part, grad_out, ldg, st);
+  if (rc) return rc;
+  return launch_loss_finalize(B200KGE_LOSS_BCE, part, 1, n, loss_out, row_loss_out, scale, 0, scratch, 0, st);
 }
 
 

@@ -382,14 +382,15 @@ normalize_rows_kernel(float* __restrict__ w, int64_t ld, int64_t rows, int dim, 
 // of the row's 1 + K columns (column 0 = the positive, label 1; columns 1..K = sampled ids, label 0): per
 // column it recomputes z = pair(q, t), g = (sigmoid(z + off) - y) / batch, adds g * dpair/dt into the sampled
 // row of d_ent (atomics: the scatter is inherent) and accumulates g * dpair/dq per lane; the block's dq is
-// added into dQ[i, :], which unfold_kernel then pushes through the relation fold.
+// added into dQ[i, :], which unfold_kernel then pushes through the relation fold.  With G given (any other loss:
+// G = dL/dz * scale from ns_loss_kernel) g = G[i, c] replaces the BCE formula; the rest is unchanged.
 constexpr int NSB_WARPS = 4, NSB_PER_BLOCK = 64, NSB_MAXK = 1024;   // lane-local dq: K / 32 <= 32 registers
 
 template <int MODEL>
 __global__ void __launch_bounds__(NSB_WARPS * 32)
 ns_backward_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int sp, const int64_t* __restrict__ neg,
-                   int64_t Kneg, Folded f, float l_norm, float offset, float inv_batch, float* __restrict__ d_ent,
-                   int64_t lde, float* __restrict__ dQ, int64_t ldq) {
+                   int64_t Kneg, Folded f, float l_norm, float offset, float inv_batch, const float* __restrict__ G,
+                   int64_t ldg, float* __restrict__ d_ent, int64_t lde, float* __restrict__ dQ, int64_t ldq) {
   extern __shared__ __align__(16) float sh[];  // q[K] | dq[K] (+ entity row for RESCAL)
   const int64_t i = blockIdx.x;
   const int64_t si = tri[3 * i], pi = tri[3 * i + 1], oi = tri[3 * i + 2];
@@ -439,7 +440,7 @@ ns_backward_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int sp, 
     float z = acc, nrm = 1.f;
     if (f.pair_op == PAIR_L1 || f.pair_op == PAIR_CMOD_L1) z = -acc;
     else if (f.pair_op == PAIR_L2) { nrm = sqrtf(acc); z = -nrm; }
-    const float g = (1.0f / (1.0f + expf(-(z + offset))) - y) * inv_batch;
+    const float g = G ? G[i * ldg + c] : (1.0f / (1.0f + expf(-(z + offset))) - y) * inv_batch;
     if (f.pair_op == PAIR_DOT) {
       for (int k = lane, j = 0; k < K; k += 32, ++j) {
         dq[j] = fmaf(g, t[k], dq[j]);
@@ -525,8 +526,9 @@ unfold_distance_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int6
 }  // namespace
 
 int launch_ns_backward(int model, float l_norm, const Rows& ent, const Rows& rel, const int64_t* triples, int slot,
-                       const int64_t* neg, int64_t n, int64_t K, float offset, float inv_batch, float* d_ent,
-                       int64_t lde, float* d_rel, int64_t ldr, float* dQ, int64_t ldq, cudaStream_t st) {
+                       const int64_t* neg, int64_t n, int64_t K, float offset, float inv_batch, const float* G,
+                       int64_t ldg, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, float* dQ, int64_t ldq,
+                       cudaStream_t st) {
   if (n == 0) return 0;
   if (slot != 0 && slot != 2) { set_error("the fused negative-sampling backward covers the S and O slots"); return B200KGE_ERR_UNSUPPORTED; }
   const int sp = (slot == 2) ? 1 : 0;      // O slot: fold (s,p), candidates are objects
@@ -540,7 +542,7 @@ int launch_ns_backward(int model, float l_norm, const Rows& ent, const Rows& rel
   const int64_t by = (K + 1 + NSB_PER_BLOCK - 1) / NSB_PER_BLOCK;
   if (by > 65535) { set_error("too many negatives per row (%lld)", (long long)K); return B200KGE_ERR_UNSUPPORTED; }
   dim3 grid((unsigned)n, (unsigned)by), block(NSB_WARPS * 32);
-#define B2K_NSB(M) case M: ns_backward_kernel<M><<<grid, block, smem, st>>>(ent, rel, triples, sp, neg, K, f, l_norm, offset, inv_batch, d_ent, lde, dQ, ldq); break;
+#define B2K_NSB(M) case M: ns_backward_kernel<M><<<grid, block, smem, st>>>(ent, rel, triples, sp, neg, K, f, l_norm, offset, inv_batch, G, ldg, d_ent, lde, dQ, ldq); break;
   switch (model) {
     B2K_NSB(B200KGE_COMPLEX) B2K_NSB(B200KGE_DISTMULT) B2K_NSB(B200KGE_SIMPLE) B2K_NSB(B200KGE_CP)
     B2K_NSB(B200KGE_RESCAL) B2K_NSB(B200KGE_TRANSE) B2K_NSB(B200KGE_ROTATE)

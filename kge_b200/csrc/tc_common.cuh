@@ -475,9 +475,14 @@ int launch_csr_rows(int loss_kind, const int64_t* off, const int64_t* col, const
 int launch_rows_sum(const float* rows, int64_t n, float scale, float* out, cudaStream_t st);
 int launch_row_score_sums(const float* Q, int64_t ldq, int64_t n, const float* T, int64_t ldt, int64_t E, int K,
                           float* scratch, float* zsum, cudaStream_t st);
+// G (optional, [n, 1+K], row stride ldg): dL/dz already scaled, read instead of the BCE gradient
 int launch_ns_backward(int model, float l_norm, const Rows& ent, const Rows& rel, const int64_t* triples, int slot,
-                       const int64_t* neg, int64_t n, int64_t K, float offset, float inv_batch, float* d_ent,
-                       int64_t lde, float* d_rel, int64_t ldr, float* dQ, int64_t ldq, cudaStream_t st);
+                       const int64_t* neg, int64_t n, int64_t K, float offset, float inv_batch, const float* G,
+                       int64_t ldg, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, float* dQ, int64_t ldq,
+                       cudaStream_t st);
+// row-wise KgeLoss of a negative-sampling block (ns_loss.cu): part[2 i] = row loss (BCE finaliser layout), G optional
+int launch_ns_loss(int loss_kind, const float* scores, int64_t lds, int64_t n, int64_t m, const int64_t* label_idx,
+                   float arg, float temperature, float scale, float* part, float* G, int64_t ldg, cudaStream_t st);
 int launch_penalty(const Rows& tab, const float* counts, float p, int complex_abs, float scale, float* scratch,
                    size_t scratch_floats, float* out, cudaStream_t st);
 int launch_normalize_rows(float* w, int64_t ld, int64_t rows, int dim, float p, cudaStream_t st);

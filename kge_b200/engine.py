@@ -602,8 +602,12 @@ def normalize_rows_(weight: torch.Tensor, p: float) -> torch.Tensor:
 
 
 def ns_backward(model: str, ent, rel, triples, negatives: dict, offset: float = 0.0, l_norm: float = 1.0,
-                  batch_size: Optional[int] = None):
-    """(d_ent, d_rel) of one negative-sampling batch with BCE; negatives = {slot: [n, K] ids}, slots 0 (S), 2 (O)."""
+                  batch_size: Optional[int] = None, grad_scores: Optional[dict] = None):
+    """(d_ent, d_rel) of one negative-sampling batch; negatives = {slot: [n, K] ids}, slots 0 (S), 2 (O).
+
+    Without grad_scores the loss is BCE with `offset`, divided by batch_size.  With grad_scores = {slot: G}, G [n, 1+K]
+    (positive first) is dL/dscores of each slot's block already scaled — e.g. the G of ns_loss(..., want_grad=True) —
+    and `offset` / `batch_size` are not used: any loss of ns_loss trains through the same kernel."""
     _require_cuda(ent, rel, triples)
     lib, k = _lib.load(), _Keep()
     re_, rr = k.rows(ent), k.rows(rel)
@@ -615,11 +619,55 @@ def ns_backward(model: str, ent, rel, triples, negatives: dict, offset: float = 
     ws = torch.empty(n * (ent.shape[1] + 32) * 4 + 1024, dtype=torch.uint8, device=dev)
     for slot, neg in negatives.items():
         ng = neg if (neg.dtype == torch.int64 and neg.is_contiguous()) else neg.long().contiguous()
-        _lib.check(lib.b200kge_ns_backward(
+        if grad_scores is None:
+            _lib.check(lib.b200kge_ns_backward(
+                MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), int(slot), ng.data_ptr(), n,
+                ng.shape[1], offset, batch_size or n, d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(),
+                d_rel.stride(0), ws.data_ptr(), ws.numel(), _stream(dev)))
+            continue
+        g = grad_scores[slot]
+        _require_cuda(g)
+        if g.shape != (n, ng.shape[1] + 1):
+            raise ValueError(f"grad_scores[{slot}] has shape {tuple(g.shape)}, expected {(n, ng.shape[1] + 1)}")
+        g = g if (g.dtype == torch.float32 and g.stride(1) == 1) else g.float().contiguous()
+        k.refs.append(g)
+        _lib.check(lib.b200kge_ns_backward_grad(
             MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), int(slot), ng.data_ptr(), n, ng.shape[1],
-            offset, batch_size or n, d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0),
+            g.data_ptr(), g.stride(0), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0),
             ws.data_ptr(), ws.numel(), _stream(dev)))
     return d_ent, d_rel
+
+
+def ns_loss(scores, loss: str, arg: float = 0.0, temperature: float = 1.0, label_idx=None,
+            batch_size: Optional[int] = None, want_grad: bool = False, return_rows: bool = False):
+    """KgeLoss of a negative-sampling block (train_negative_sampling.py:126-156): scores [n, m] with one positive per
+    row at label_idx[i] (None: column 0, the ns_score(with_positive=True) layout), label 0 elsewhere.  `loss` is any
+    `train.loss` of the reference but ce; `arg` is the offset (bce, bce_mean, bce_self_adversarial) or the margin
+    (margin_ranking), `temperature` that of bce_self_adversarial.
+
+    Returns (loss, G): loss = sum of the row losses / batch_size (0-d tensor, deterministic); G = dL/dscores [n, m]
+    (fp32) when want_grad, else None.  With return_rows the per-row losses (not divided) follow as a third item."""
+    _require_cuda(scores, label_idx)
+    if loss not in LOSS:
+        raise ValueError(f"unknown loss {loss!r}")
+    lib = _lib.load()
+    x = scores if (scores.dtype == torch.float32 and scores.dim() == 2 and scores.stride(1) == 1) \
+        else scores.float().contiguous()
+    n, m = x.shape
+    dev = x.device
+    li = _i64(label_idx)
+    if li is not None and li.numel() != n:
+        raise ValueError(f"label_idx has {li.numel()} entries for {n} rows")
+    out = torch.empty((), dtype=torch.float32, device=dev)
+    G = torch.empty((n, m), dtype=torch.float32, device=dev) if want_grad else None
+    rows = torch.empty(n, dtype=torch.float32, device=dev) if return_rows else None
+    ws = torch.empty(lib.b200kge_ns_loss_workspace_bytes(n), dtype=torch.uint8, device=dev)
+    scale = 1.0 / float(batch_size) if batch_size else 1.0
+    _lib.check(lib.b200kge_ns_loss(
+        x.data_ptr(), x.stride(0), n, m, li.data_ptr() if li is not None else None, LOSS[loss], float(arg),
+        float(temperature), scale, out.data_ptr(), rows.data_ptr() if rows is not None else None,
+        G.data_ptr() if G is not None else None, m, ws.data_ptr(), ws.numel(), _stream(dev)))
+    return (out, G, rows) if return_rows else (out, G)
 
 
 def score_1vsN_loss_csr(model: str, combine: str, q_tab, rel, cand_tab, csr_offsets, csr_cols, q=None, p=None,

@@ -252,22 +252,50 @@ class ReciprocalRelationsModel(KgeModel):
 
 
 class KgeLoss:
-    """loss.py:20-213 for the two in-scope losses; `__call__(scores, labels)` with labels either a
-    vector of positions or a label matrix; reduction is SUM (the caller divides by batch size)."""
+    """loss.py:20-274: `__call__(scores, labels)` with labels either a vector of positions or a label matrix; reduction
+    is SUM (the caller divides by batch size).  bce / kl take any labels (the dense-loss kernel); bce_mean,
+    bce_self_adversarial, margin_ranking, soft_margin and se take one positive per row — positions, or a 0/1 matrix with
+    exactly one 1 per row such as the negative-sampling labels — on the row-loss kernel (margin_ranking pairs each
+    row's positive with that row's other columns, the negative-sampling form of loss.py:240-252)."""
 
-    def __init__(self, kind: str, offset: float = 0.0):
-        self.kind, self._offset = kind, offset
+    ROW_WISE = ("bce_mean", "bce_self_adversarial", "margin_ranking", "soft_margin", "se")
+
+    def __init__(self, kind: str, offset: float = 0.0, temperature: float = 1.0):
+        self.kind, self._offset, self._temperature = kind, offset, temperature
 
     @staticmethod
     def create(train_loss: str, loss_arg: float = float("nan")) -> "KgeLoss":
+        """The losses of the 1vsAll / KvsAll steps (bce, kl)."""
         if train_loss == "bce":
             return KgeLoss("bce", 0.0 if math.isnan(loss_arg) else loss_arg)   # loss.py:46-52
         if train_loss == "kl":
             return KgeLoss("kl")
         raise ValueError("invalid value train.loss={}".format(train_loss))
 
+    @staticmethod
+    def create_negative_sampling(train_loss: str, loss_arg: float = float("nan"),
+                                 temperature: float = 1.0) -> "KgeLoss":
+        """Every loss a negative-sampling job accepts (loss.py:30-90 without ce), with the reference's loss_arg defaults:
+        offset 0 for the BCE family, margin 1 for margin_ranking; `temperature` is
+        user.bce_self_adversarial_temperature (loss.py:64-68)."""
+        if train_loss in ("bce", "bce_mean", "bce_self_adversarial"):
+            return KgeLoss(train_loss, 0.0 if math.isnan(loss_arg) else loss_arg, temperature)
+        if train_loss == "margin_ranking":
+            return KgeLoss("margin_ranking", 1.0 if math.isnan(loss_arg) else loss_arg)
+        if train_loss in ("kl", "soft_margin", "se"):
+            return KgeLoss(train_loss)
+        raise ValueError("invalid value train.loss={}".format(train_loss))
+
     def __call__(self, scores, labels, **kwargs):
-        return engine.loss_dense(scores, labels, self.kind, self._offset)
+        if self.kind not in self.ROW_WISE:
+            return engine.loss_dense(scores, labels, self.kind, self._offset)
+        if labels.dim() == 2:
+            # _labels_as_indexes (loss.py:119-136): exactly one 1 per row
+            nz = labels.nonzero()
+            if not nz[:, 0].equal(torch.arange(len(labels), device=labels.device)):
+                raise ValueError("exactly one 1 per row required")
+            labels = nz[:, 1]
+        return engine.ns_loss(scores, self.kind, self._offset, self._temperature, label_idx=labels)[0]
 
 
 class BatchNegativeSample:

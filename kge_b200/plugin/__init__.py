@@ -232,25 +232,32 @@ class _KvsAllLossFn(torch.autograd.Function):
 
 
 class _NsSlotLossFn(torch.autograd.Function):
-    """One slot of a negative-sampling batch with BCE: forward = fused gather+score [n, 1+K] and the dense-loss kernel;
-    backward = the fused NS gradient kernel (b200kge_ns_backward: per-row fold, per-column recompute, scatter)."""
+    """One slot of a negative-sampling batch: forward = fused gather+score [n, 1+K] and the loss kernel; backward = the
+    fused NS gradient kernel (b200kge_ns_backward: per-row fold, per-column recompute, scatter).  BCE runs the dense-loss
+    kernel and the kernel's own BCE gradient; every other loss runs the row-loss kernel (b200kge_ns_loss), which also
+    writes G = dL/dscores, and the backward reads G (b200kge_ns_backward_grad)."""
 
     @staticmethod
-    def forward(ctx, ent_w, rel_w, model, triples, negatives, slot, offset, batch_size):
-        ctx.args = (model, slot, offset, batch_size)
-        ctx.save_for_backward(ent_w, rel_w, triples, negatives)
+    def forward(ctx, ent_w, rel_w, model, triples, negatives, slot, offset, batch_size, loss="bce", temperature=1.0):
+        ctx.args = (model, slot, offset, batch_size, loss)
         ln = model._b200_args()[0]
         scores = engine.ns_score(model._b200_name, ent_w.detach(), rel_w.detach(), triples, negatives, slot, True, ln)
-        lab = torch.zeros(triples.shape[0], dtype=torch.int64, device=triples.device)
-        return engine.loss_dense(scores, lab, "bce", offset) / batch_size
+        if loss == "bce":
+            ctx.save_for_backward(ent_w, rel_w, triples, negatives)
+            lab = torch.zeros(triples.shape[0], dtype=torch.int64, device=triples.device)
+            return engine.loss_dense(scores, lab, "bce", offset) / batch_size
+        value, G = engine.ns_loss(scores, loss, offset, temperature, batch_size=batch_size, want_grad=True)
+        ctx.save_for_backward(ent_w, rel_w, triples, negatives, G)
+        return value
 
     @staticmethod
     def backward(ctx, g):
-        ent_w, rel_w, triples, negatives = ctx.saved_tensors
-        model, slot, offset, batch_size = ctx.args
+        model, slot, offset, batch_size, loss = ctx.args
+        ent_w, rel_w, triples, negatives = ctx.saved_tensors[:4]
+        kw = {} if loss == "bce" else {"grad_scores": {slot: ctx.saved_tensors[4]}}
         d_ent, d_rel = engine.ns_backward(model._b200_name, ent_w.detach(), rel_w.detach(), triples, {slot: negatives},
-                                          offset, model._b200_args()[0], batch_size)
-        return d_ent * g, d_rel * g, None, None, None, None, None, None
+                                          offset, model._b200_args()[0], batch_size, **kw)
+        return (d_ent * g, d_rel * g) + (None,) * 8
 
 
 class _B200ModelMixin:
@@ -467,12 +474,17 @@ class _B200ModelMixin:
         ln = self._b200_args()[0]
         return {"transe": ln in (1.0, 2.0), "rotate": ln == 1.0}.get(self._b200_name, True)
 
-    def loss_negatives(self, triples, negatives, slot, offset, batch_size):
-        """BCE of one slot's [n, 1+K] block (positive first) / batch_size, differentiable through the gradient kernel
-        (train_negative_sampling.py:139-164)."""
+    def loss_negatives(self, triples, negatives, slot, offset, batch_size, loss="bce", temperature=1.0):
+        """KgeLoss of one slot's [n, 1+K] block (positive first) / batch_size, differentiable through the gradient
+        kernel (train_negative_sampling.py:139-164).  `loss` is a name of engine.ns_loss; `offset` its argument (the BCE
+        offset, or the margin of margin_ranking), `temperature` that of bce_self_adversarial."""
         ent_w, rel_w = self._b200_weights()
         return _NsSlotLossFn.apply(ent_w, rel_w, self, triples.long().contiguous(), negatives.long().contiguous(),
-                                   int(slot), float(offset), int(batch_size))
+                                   int(slot), float(offset), int(batch_size), loss, float(temperature))
+
+    def loss_negatives_forward(self, scores, loss, arg=0.0, temperature=1.0):
+        """Sum over rows of the KgeLoss of a scored [n, 1+K] block (positive first); forward only."""
+        return engine.ns_loss(scores, loss, arg, temperature)[0]
 
     def score_sp_loss(self, s, p, labels, loss="bce", offset=0.0):
         ent, rel = self._b200_tables()

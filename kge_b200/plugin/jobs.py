@@ -12,7 +12,7 @@ config.modules(), ...)`), i.e. in a LibKGE config:
 
 Everything else of the job (data loading, collate, sub-batching, trace entries, penalties, optimizer, hooks,
 checkpoints) is the reference's code, unchanged.  Whenever a fused form is not available for the configured
-combination (a non-b200 model, a loss other than bce / kl, dropout active, ...) the method falls through to
+combination (a non-b200 model, a loss outside the fused set, dropout active, ...) the method falls through to
 the reference implementation, which then still reaches the kernels through `model.score_*`.
 """
 from __future__ import annotations
@@ -25,7 +25,8 @@ from kge.job.train_1vsAll import TrainingJob1vsAll
 from kge.job.train_KvsAll import TrainingJobKvsAll
 from kge.job.train_negative_sampling import TrainingJobNegativeSampling
 from kge.job import Job
-from kge.util.loss import BCEWithLogitsKgeLoss, KLDivWithSoftmaxKgeLoss
+from kge.util.loss import (BCEWithLogitsKgeLoss, KLDivWithSoftmaxKgeLoss, MarginRankingKgeLoss, SEKgeLoss,
+                           SoftMarginKgeLoss)
 
 S, P, O = 0, 1, 2
 SLOT_STR = ["s", "p", "o"]
@@ -37,6 +38,26 @@ def _fused_loss_kind(loss):
         return "bce", float(loss._offset)
     if type(loss) is KLDivWithSoftmaxKgeLoss:
         return "kl", 0.0
+    return None
+
+
+def _ns_loss_kind(loss):
+    """(name, arg, temperature) of the job's KgeLoss if the negative-sampling kernels cover it, else None: every loss
+    KgeLoss.create builds for a negative-sampling job (loss.py:30-90; "ce" is not one of its names)."""
+    t = type(loss)
+    if t is BCEWithLogitsKgeLoss:
+        name = {None: "bce", "mean": "bce_mean", "self_adversarial": "bce_self_adversarial"}.get(loss._bce_type)
+        if name is None:
+            return None
+        return name, float(loss._offset), float(getattr(loss, "_temperature", 1.0))
+    if t is KLDivWithSoftmaxKgeLoss:
+        return "kl", 0.0, 1.0
+    if t is MarginRankingKgeLoss and loss._loss.reduction == "sum":
+        return "margin_ranking", float(loss._loss.margin), 1.0
+    if t is SoftMarginKgeLoss and loss._loss.reduction == "sum":
+        return "soft_margin", 0.0, 1.0
+    if t is SEKgeLoss and loss._loss.reduction == "sum":
+        return "se", 0.0, 1.0
     return None
 
 
@@ -279,14 +300,14 @@ class B200TrainingJobNegativeSampling(_BatchSplit, TrainingJobNegativeSampling):
         if subbatch_slice is None:
             return
         model = _fused_model(self.model)
-        kind = _fused_loss_kind(self.loss)
+        kind = _ns_loss_kind(self.loss)
         slots = [sl for sl in (S, P, O) if self._sampler.num_samples[sl] > 0]
-        trainable = (model is not None and kind is not None and kind[0] == "bce"
+        trainable = (model is not None and kind is not None
                      and all(model.b200_ns_native_backward_ok(sl) for sl in slots))
         if model is None or (not self.is_forward_only and not trainable):
             if self._device_sampling:
                 raise NotImplementedError("user.b200_device_sampling needs a b200_* model whose slots the fused "
-                                          "gradient kernel covers (S / O slots, bce)")
+                                          "gradient kernel covers (S / O slots)")
             return super()._process_subbatch(batch_index, batch, subbatch_slice, result)
         batch_size = result.size
         result.prepare_time -= time.time()
@@ -314,7 +335,8 @@ class B200TrainingJobNegativeSampling(_BatchSplit, TrainingJobNegativeSampling):
             result.forward_time -= time.time()
             if not self.is_forward_only:
                 # training: forward + the fused NS gradient kernel behind one autograd node
-                loss_value = model.loss_negatives(triples, negatives.to(self.device), slot, kind[1], batch_size)
+                loss_value = model.loss_negatives(triples, negatives.to(self.device), slot, kind[1], batch_size,
+                                                  kind[0], kind[2])
                 result.avg_loss += loss_value.item()
                 result.forward_time += time.time()
                 result.backward_time -= time.time()
@@ -326,6 +348,9 @@ class B200TrainingJobNegativeSampling(_BatchSplit, TrainingJobNegativeSampling):
                 # labels are 1 in column 0 and 0 elsewhere (train_negative_sampling.py:128-137): index labels
                 lab = torch.zeros(subbatch_size, dtype=torch.int64, device=self.device)
                 loss_value = model.loss_dense(scores, lab, "bce", kind[1]) / batch_size
+            elif kind is not None:
+                # the row-loss kernel, positive in column 0 (train_negative_sampling.py:126-156)
+                loss_value = model.loss_negatives_forward(scores, kind[0], kind[1], kind[2]) / batch_size
             else:
                 if labels[slot] is None or labels[slot].shape != (subbatch_size, 1 + num_samples):
                     labels[slot] = torch.zeros((subbatch_size, 1 + num_samples), device=self.device)
