@@ -421,6 +421,76 @@ int b200kge_lookup_penalty(const b200kge_rows_t* rows, const float* counts, floa
 int b200kge_normalize_rows(float* weight, int64_t ld, int64_t rows, int32_t dim, float p,
                              b200kge_stream_t stream);
 
+/* ---- Embedding dropout of the 1vsAll / KvsAll training steps ---------------------------------------------------------
+ * LookupEmbedder._postprocess (lookup_embedder.py:96-105) draws a fresh element-wise Bernoulli mask per embed(idx) /
+ * embed_all() call and scales kept values by 1/(1-p).  One sub-batch of 1vsAll training (train_1vsAll.py:64,75 with
+ * kge_model.py:682-721) makes six independent draws, numbered as mask streams:
+ *   score_sp(s, p): 0 = embed(s), 1 = embed(p), 2 = embed_all()       (entity, relation, entity table)
+ *   score_po(p, o): 3 = embed_all(), 4 = embed(p), 5 = embed(o)       (entity table, relation, entity)
+ * so the two directions use different masks on the candidate table and on p.  KvsAll (train_KvsAll.py:274-285) draws
+ * streams 0-2 for its sp_ queries and 3-5 for its _po queries.
+ *
+ * Mask layout (never stored: the backward regenerates the forward's mask from the same key):
+ *   element (row, k) of a draw over rows of width dim has elem = row * dim + k, where row is the GLOBAL row: the entity
+ *   id for the table draws (2, 3), row_base + i for row i of the sub-batch's queries (0, 1, 4, 5);
+ *   Philox4x32-10 with key = seed (64 bits) and counter = ((stream << 46) | (elem >> 2), call), both 64-bit halves
+ *   little-endian as four 32-bit words; the element takes output word elem & 3;
+ *   kept iff word < floor((1 - p) * 2^32), kept value x * (1 / (1 - p)) in fp32.
+ * Requirements (else B200KGE_ERR_INVALID): 0 <= p < 1; row_base >= 0; elem < 2^48 for every element of every draw. */
+#define B200KGE_DROP_SP_ENT 0
+#define B200KGE_DROP_SP_REL 1
+#define B200KGE_DROP_SP_TABLE 2
+#define B200KGE_DROP_PO_TABLE 3
+#define B200KGE_DROP_PO_REL 4
+#define B200KGE_DROP_PO_ENT 5
+
+typedef struct {
+  float p_ent;      /* entity_embedder.dropout   */
+  float p_rel;      /* relation_embedder.dropout */
+  uint64_t seed;    /* Philox key                */
+  uint64_t call;    /* one value per sub-batch (e.g. from epoch, batch index, sub-batch ordinal) */
+  int64_t row_base; /* global index of the sub-batch's first query row */
+} b200kge_dropout_t;
+
+/* The keep mask of one draw: out[i * dim + k] = 1 if element (row_base + i, k) of stream `mask_stream` is kept, else 0,
+ * for i < rows, k < dim (uint8, device). */
+int b200kge_dropout_mask(float p, uint64_t seed, uint64_t call, int mask_stream, int64_t row_base, int64_t rows,
+                         int32_t dim, uint8_t* out, b200kge_stream_t stream);
+
+/* b200kge_train_1vsall_forward / _backward with dropout: the six draws above, applied to gathered copies of the query
+ * rows, the relation rows and one table copy per direction; each direction then runs the per-direction scorer (forward)
+ * or gradient machinery (backward, same model coverage as b200kge_train_1vsall_backward) on those copies, and the
+ * backward masks the table and row gradients with the same draws before adding them into d_ent / d_rel (OVERWRITTEN).
+ * Workspace (either call): b200kge_train_1vsall_dropout_workspace_bytes. */
+size_t b200kge_train_1vsall_dropout_workspace_bytes(int model, int64_t n, int64_t E, int32_t D);
+int b200kge_train_1vsall_forward_dropout(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                                         const b200kge_rows_t* rel, const int64_t* triples, int64_t n, int loss_kind,
+                                         float offset, const b200kge_dropout_t* drop, float* loss_out, void* workspace,
+                                         size_t workspace_bytes, b200kge_stream_t stream);
+int b200kge_train_1vsall_backward_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                          const int64_t* triples, int64_t n, int loss_kind, float offset,
+                                          const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
+                                          int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+
+/* b200kge_score_1vsN_loss_csr / _backward with dropout for one KvsAll query type: queries ent[q_idx] (stream 0 | 5),
+ * relations rel[p_idx] (1 | 4) and the candidate table ent (2 | 3) for combine sp_ | _po.  The backward covers the dot
+ * family (as b200kge_score_1vsN_loss_csr_backward) and OVERWRITES d_ent / d_rel.
+ * Workspace (either call): b200kge_score_1vsN_loss_csr_dropout_workspace_bytes. */
+size_t b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(int model, int64_t n, int64_t E, int32_t D, int64_t nnz);
+int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, float l_norm, int precision, const b200kge_rows_t* ent,
+                                        const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx, int64_t n,
+                                        const int64_t* csr_off, const int64_t* csr_col, int64_t nnz,
+                                        float label_smoothing, int loss_kind, float offset,
+                                        const b200kge_dropout_t* drop, float* loss_out, float* row_loss_out,
+                                        void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+int b200kge_score_1vsN_loss_csr_backward_dropout(int model, int combine, const b200kge_rows_t* ent,
+                                                 const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx,
+                                                 int64_t n, const int64_t* csr_off, const int64_t* csr_col,
+                                                 float label_smoothing, int loss_kind, float offset, int64_t batch_size,
+                                                 const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
+                                                 int64_t ldr, void* workspace, size_t workspace_bytes,
+                                                 b200kge_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -28,8 +28,15 @@ class Labels(C.Structure):
     _fields_ = [("idx", C.c_void_p), ("dense", C.c_void_p), ("ldl", C.c_int64)]
 
 
+class Dropout(C.Structure):
+    """b200kge_dropout_t: rates and mask key of one sub-batch (layout: include/b200kge.h)."""
+    _fields_ = [("p_ent", C.c_float), ("p_rel", C.c_float), ("seed", C.c_uint64), ("call", C.c_uint64),
+                ("row_base", C.c_int64)]
+
+
 # every symbol include/b200kge.h declares, with its signature
 _RP = C.POINTER(Rows)
+_DP = C.POINTER(Dropout)
 SIGNATURES = {
     "b200kge_version": (C.c_int, []),
     "b200kge_last_error": (C.c_char_p, []),
@@ -111,6 +118,26 @@ SIGNATURES = {
     "b200kge_lookup_penalty": (C.c_int, [_RP, C.c_void_p, C.c_float, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
                                            C.c_size_t, C.c_void_p]),
     "b200kge_normalize_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_float, C.c_void_p]),
+    "b200kge_dropout_mask": (C.c_int, [C.c_float, C.c_uint64, C.c_uint64, C.c_int, C.c_int64, C.c_int64, C.c_int32,
+                                       C.c_void_p, C.c_void_p]),
+    "b200kge_train_1vsall_dropout_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32]),
+    "b200kge_train_1vsall_forward_dropout": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_void_p, C.c_int64,
+                                                       C.c_int, C.c_float, _DP, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                       C.c_void_p]),
+    "b200kge_train_1vsall_backward_dropout": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int64, C.c_int,
+                                                        C.c_float, _DP, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                                        C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_score_1vsN_loss_csr_dropout_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32,
+                                                                         C.c_int64]),
+    "b200kge_score_1vsN_loss_csr_dropout": (C.c_int, [C.c_int, C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_void_p,
+                                                      C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
+                                                      C.c_float, C.c_int, C.c_float, _DP, C.c_void_p, C.c_void_p,
+                                                      C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_score_1vsN_loss_csr_backward_dropout": (C.c_int, [C.c_int, C.c_int, _RP, _RP, C.c_void_p, C.c_void_p,
+                                                               C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.c_int,
+                                                               C.c_float, C.c_int64, _DP, C.c_void_p, C.c_int64,
+                                                               C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t,
+                                                               C.c_void_p]),
 }
 
 _lib = None

@@ -1212,3 +1212,323 @@ int b200kge_score_1vsN_loss_csr(int model, int combine, float l_norm, int precis
 }
 
 }  // extern "C"
+
+// ==================================================================================================
+// Embedding dropout for the 1vsAll and KvsAll training steps (layout: include/b200kge.h, kernels: dropout.cu).  Each
+// direction gathers masked copies of its query rows, relation rows and candidate table into the workspace and runs the
+// existing per-direction machinery on them as plain operands (idx = NULL).  The backward hands the unfold identity
+// triples, so row i's gradient lands in row i of [n, D] buffers, and then adds the masked table gradient and scatters
+// the masked row gradients into d_ent / d_rel: two directions that read the same table columns under different masks
+// contribute the SUM of their masked dT.
+namespace {
+
+int validate_dropout(const b200kge_dropout_t* d, int64_t n, int64_t E, int D, int Dr) {
+  if (!d) { set_error("null dropout key"); return B200KGE_ERR_INVALID; }
+  if (!(d->p_ent >= 0.f && d->p_ent < 1.f) || !(d->p_rel >= 0.f && d->p_rel < 1.f)) {
+    set_error("dropout rates must lie in [0, 1) (got %g, %g)", (double)d->p_ent, (double)d->p_rel);
+    return B200KGE_ERR_INVALID;
+  }
+  const double lim = 281474976710656.0;    // 2^48: elem >> 2 must fit below the stream bits of the counter
+  if (d->row_base < 0 || (double)(d->row_base + n) * D > lim || (double)(d->row_base + n) * Dr > lim ||
+      (double)E * D > lim) {
+    set_error("dropout rows out of range: row_base >= 0 and row * dim + k < 2^48 are required");
+    return B200KGE_ERR_INVALID;
+  }
+  return 0;
+}
+
+DropMask drop_mask(float p, uint64_t seed, uint64_t call, int stream, int64_t row_base) {
+  DropMask m;
+  m.seed = seed; m.call = call; m.stream = stream; m.row_base = row_base;
+  m.thresh = (uint64_t)floor((1.0 - (double)p) * 4294967296.0);
+  m.scale = (float)(1.0 / (1.0 - (double)p));
+  return m;
+}
+
+// the three draws of one direction: query entity rows, relation rows, candidate table
+struct DirMasks { DropMask q, r, t; };
+DirMasks dir_masks(const b200kge_dropout_t& d, int dir) {
+  DirMasks m;
+  m.q = drop_mask(d.p_ent, d.seed, d.call, dir == 0 ? B200KGE_DROP_SP_ENT : B200KGE_DROP_PO_ENT, d.row_base);
+  m.r = drop_mask(d.p_rel, d.seed, d.call, dir == 0 ? B200KGE_DROP_SP_REL : B200KGE_DROP_PO_REL, d.row_base);
+  m.t = drop_mask(d.p_ent, d.seed, d.call, dir == 0 ? B200KGE_DROP_SP_TABLE : B200KGE_DROP_PO_TABLE, 0);
+  return m;
+}
+
+// masked copies of one direction's operands: Qm [n, D], Pm [n, Dr], Tm [E, D] (row strides = widths)
+struct MaskedOps { float *Qm, *Pm, *Tm; };
+bool take_masked(Arena& ws, int64_t n, int64_t E, int D, int Dr, MaskedOps& o) {
+  o.Qm = (float*)ws.take((size_t)n * D * 4);
+  o.Pm = (float*)ws.take((size_t)n * Dr * 4);
+  o.Tm = (float*)ws.take((size_t)E * D * 4);
+  return o.Qm && o.Pm && o.Tm;
+}
+int gather_masked(const DirMasks& m, const Rows& E, const Rows& R, const int64_t* q_idx, const int64_t* p_idx, int64_t n,
+                  const MaskedOps& o, Rows& Qr, Rows& Pr, Rows& Tr, cudaStream_t st) {
+  Rows qs = E; qs.idx = q_idx; qs.rows = n;
+  Rows ps = R; ps.idx = p_idx; ps.rows = n;
+  Rows ts = E; ts.idx = nullptr;
+  int rc;
+  if ((rc = launch_dropout_gather(m.q, qs, o.Qm, E.dim, st))) return rc;
+  if ((rc = launch_dropout_gather(m.r, ps, o.Pm, R.dim, st))) return rc;
+  if ((rc = launch_dropout_gather(m.t, ts, o.Tm, E.dim, st))) return rc;
+  Qr = Rows{o.Qm, nullptr, n, E.dim, E.dim};
+  Pr = Rows{o.Pm, nullptr, n, R.dim, R.dim};
+  Tr = Rows{o.Tm, nullptr, E.rows, E.dim, E.dim};
+  return 0;
+}
+
+size_t masked_bytes(int model, int64_t n, int64_t E, int32_t D) {
+  const int64_t Dr = relation_dim(model, D), ldq = round_up(D, 32);
+  return 2 * ((size_t)E * D * 4 + 256)                       // Tm, dT
+         + 2 * ((size_t)n * D * 4 + (size_t)n * Dr * 4 + 512)  // Qm, Pm, dQe, dPr
+         + 2 * ((size_t)n * ldq * 4 + 256)                     // Q, dQ
+         + (size_t)n * 10 * 8 + 5 * 256                        // s/p/o, labels [2n], identity triples [3n]
+         + (size_t)n * 2 * 4 + 4096;                           // KL row statistics, scalars
+}
+
+// One direction of the masked backward: gather, fold, dT and dQ (tensor-core GEMMs or the distance row-gradient
+// passes), unfold into the per-row buffers, then d_ent[:, cols] += mask_t * dT, d_ent[q] += mask_q * dQe,
+// d_rel[p] += mask_r * dPr.  Labels: lab (one per row, 1vsAll, scaled 1/n) or the CSR of a KvsAll query type.
+struct DirGrad {
+  const int64_t* lab;
+  const int64_t* csr_off; const int64_t* csr_col; float csr_a, csr_b, inv_batch;
+  int loss_kind; float offset;
+};
+int dropout_backward_dir(int model, float l_norm, int dir, const Rows& E, const Rows& R, const int64_t* q_idx,
+                         const int64_t* p_idx, int64_t n, const b200kge_dropout_t& d, const DirGrad& g,
+                         const MaskedOps& o, float* Q, float* dQ, float* dT, float* dQe, float* dPr, const int64_t* tri,
+                         Arena ws, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, cudaStream_t st) {
+  const DirMasks m = dir_masks(d, dir);
+  const Folded f = folded_problem(model, dir, E.dim, l_norm);
+  const int64_t ldq = round_up(f.K, 32), mE = E.rows;
+  const int D = E.dim, Dr = R.dim;
+  Rows Qr, Pr, Tr;
+  int rc = gather_masked(m, E, R, q_idx, p_idx, n, o, Qr, Pr, Tr, st);
+  if (rc) return rc;
+  if ((rc = launch_fold_queries(model, dir, Qr, Pr, n, 0, Q, ldq, st))) return rc;
+  B2K_CUDA(cudaMemsetAsync(dQe, 0, (size_t)n * D * 4, st));
+  B2K_CUDA(cudaMemsetAsync(dPr, 0, (size_t)n * Dr * 4, st));
+  if (f.pair_op == PAIR_DOT) {
+    if ((rc = backward_block(model, Tr, Pr, tri, n, dir, Q, ldq, g.lab, f.col_off, f.K, g.loss_kind, g.offset, dT, D, dQ,
+                             ws, st, nullptr, 0, g.csr_off, g.csr_col, g.csr_a, g.csr_b, g.inv_batch))) return rc;
+    if ((rc = launch_unfold(model, Qr, Pr, tri, n, dir, dQ, ldq, dQe, D, dPr, Dr, st))) return rc;
+  } else {
+    // distance family: scores by the CUDA-core scorer, dense G, the two row-gradient passes (as the stacked step)
+    const int64_t ldz = round_up(mE, 4), ldN = round_up(n, 4);
+    float* z = (float*)ws.take((size_t)n * ldz * 4);
+    float* G = (float*)ws.take((size_t)n * ldz * 4);
+    float* Gt = (float*)ws.take((size_t)mE * ldN * 4);
+    float* row_stat = g.loss_kind == B200KGE_LOSS_KL ? (float*)ws.take((size_t)n * 2 * 4) : nullptr;
+    if (!z || !G || !Gt || (g.loss_kind == B200KGE_LOSS_KL && !row_stat)) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
+    {
+      EpiParams P = empty_epi();
+      P.out = z; P.ldo = ldz;
+      Block B{model, dir, &Qr, nullptr, &Pr, &Tr, n};
+      B.Qpre = Q;
+      if ((rc = run_block(B, l_norm, B200KGE_PREC_AUTO, EPI_STORE, P, ws, st, nullptr))) return rc;
+    }
+    if (row_stat && (rc = launch_row_lse(z, ldz, n, mE, g.lab, row_stat, st))) return rc;
+    if ((rc = launch_grad_dense(z, ldz, n, mE, g.lab, row_stat, g.loss_kind == B200KGE_LOSS_KL ? 0.f : g.offset,
+                                1.0f / (float)n, f.pair_op == PAIR_L2, G, ldz, st))) return rc;
+    if ((rc = launch_transpose(G, ldz, n, mE, Gt, ldN, st))) return rc;
+    if ((rc = launch_pair_rowgrad(f.pair_op, Q, ldq, n, Tr.base, Tr.ld, mE, f.K, Gt, ldN, dQ, ldq, st))) return rc;
+    if ((rc = launch_pair_rowgrad(f.pair_op, Tr.base, Tr.ld, mE, Q, ldq, n, f.K, G, ldz, dT, D, st))) return rc;
+    if ((rc = launch_unfold_distance(model, Qr, Pr, tri, n, dir, dQ, ldq, dQe, D, dPr, Dr, st))) return rc;
+  }
+  if ((rc = launch_dropout_add_cols(m.t, dT, D, mE, D, f.col_off, f.col_off + f.K, d_ent, lde, st))) return rc;
+  if ((rc = launch_dropout_scatter(m.q, dQe, D, n, D, q_idx, d_ent, lde, st))) return rc;
+  return launch_dropout_scatter(m.r, dPr, Dr, n, Dr, p_idx, d_rel, ldr, st);
+}
+
+// the per-direction buffers of the backward
+struct BackBufs { MaskedOps o; float *Q, *dQ, *dT, *dQe, *dPr; int64_t* tri; };
+bool take_back(Arena& ws, int64_t n, int64_t E, int D, int Dr, int64_t ldq, BackBufs& b) {
+  if (!take_masked(ws, n, E, D, Dr, b.o)) return false;
+  b.Q = (float*)ws.take((size_t)n * ldq * 4);
+  b.dQ = (float*)ws.take((size_t)n * ldq * 4);
+  b.dT = (float*)ws.take((size_t)E * D * 4);
+  b.dQe = (float*)ws.take((size_t)n * D * 4);
+  b.dPr = (float*)ws.take((size_t)n * Dr * 4);
+  b.tri = (int64_t*)ws.take((size_t)n * 3 * 8);
+  return b.Q && b.dQ && b.dT && b.dQe && b.dPr && b.tri;
+}
+
+Arena rest_of(const Arena& ws) {
+  const size_t used = (ws.off + 255) & ~size_t(255);
+  return Arena{ws.base + used, used < ws.cap ? ws.cap - used : 0, 0};
+}
+
+}  // namespace
+
+extern "C" {
+
+int b200kge_dropout_mask(float p, uint64_t seed, uint64_t call, int mask_stream, int64_t row_base, int64_t rows,
+                         int32_t dim, uint8_t* out, b200kge_stream_t stream) {
+  if (!out && rows > 0 && dim > 0) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (rows < 0 || dim < 0 || mask_stream < 0 || mask_stream >= (1 << 18)) { set_error("bad mask shape or stream"); return B200KGE_ERR_INVALID; }
+  b200kge_dropout_t d{p, 0.f, seed, call, row_base};
+  int rc = validate_dropout(&d, rows, 0, dim, 0); if (rc) return rc;
+  return launch_dropout_mask(drop_mask(p, seed, call, mask_stream, row_base), rows, dim, out, (cudaStream_t)stream);
+}
+
+size_t b200kge_train_1vsall_dropout_workspace_bytes(int model, int64_t n, int64_t E, int32_t D) {
+  size_t dir = b200kge_score_1vsN_backward_workspace_bytes(model, n, E, D) + (size_t)n * 2 * 4 + 1024;
+  const size_t fwd = b200kge_workspace_bytes(model, n, E, D, 0);
+  return masked_bytes(model, n, E, D) + (dir > fwd ? dir : fwd);
+}
+
+int b200kge_train_1vsall_forward_dropout(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                                         const b200kge_rows_t* rel, const int64_t* triples, int64_t n, int loss_kind,
+                                         float offset, const b200kge_dropout_t* drop, float* loss_out, void* workspace,
+                                         size_t workspace_bytes, b200kge_stream_t stream) {
+  if (!ent || !rel || !triples || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
+  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
+  if ((rc = validate_norm(model, l_norm))) return rc;
+  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n <= 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  Rows E = to_rows(ent), R = to_rows(rel);
+  int64_t* sidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* pidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* oidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
+  float* dir_loss = (float*)ws.take(256);
+  MaskedOps o;
+  if (!sidx || !pidx || !oidx || !lab || !dir_loss || !take_masked(ws, n, E.rows, E.dim, R.dim, o)) {
+    set_error("workspace too small (see b200kge_train_1vsall_dropout_workspace_bytes)");
+    return B200KGE_ERR_WORKSPACE;
+  }
+  unpack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(triples, n, sidx, pidx, oidx, lab);
+  B2K_LAUNCH_CHECK("unpack_triples_kernel");
+  const Arena rest = rest_of(ws);
+  for (int dir = 0; dir < 2; ++dir) {
+    Rows Qr, Pr, Tr;
+    if ((rc = gather_masked(dir_masks(*drop, dir), E, R, dir == 0 ? sidx : oidx, pidx, n, o, Qr, Pr, Tr, st))) return rc;
+    const b200kge_rows_t q{Qr.base, nullptr, n, Qr.ld, Qr.dim}, p{Pr.base, nullptr, n, Pr.ld, Pr.dim},
+        c{Tr.base, nullptr, Tr.rows, Tr.ld, Tr.dim};
+    const b200kge_labels_t labels{lab + dir * n, nullptr, 0};
+    if ((rc = b200kge_score_1vsN_loss(model, dir, l_norm, precision, &q, &p, &c, n, &labels, loss_kind, offset,
+                                      dir_loss + dir, nullptr, rest.base, rest.cap, stream))) return rc;
+  }
+  return launch_rows_sum(dir_loss, 2, 1.0f / (float)n, loss_out, st);    // (loss_sp + loss_po) / n
+}
+
+int b200kge_train_1vsall_backward_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                          const int64_t* triples, int64_t n, int loss_kind, float offset,
+                                          const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
+                                          int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+  if (!ent || !rel || !triples || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
+  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
+  if ((rc = validate_norm(model, l_norm))) return rc;
+  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  if (lde < ent->dim || ldr < rel->dim) { set_error("gradient leading dimensions are smaller than the table widths"); return B200KGE_ERR_INVALID; }
+  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
+  const Folded f = folded_problem(model, B200KGE_SP_, ent->dim, l_norm);
+  if (f.pair_op != PAIR_DOT && f.pair_op != PAIR_L1 && f.pair_op != PAIR_L2 && f.pair_op != PAIR_CMOD_L1) {
+    set_error("the distance-family backward covers l_norm 1 and 2 (TransE) and 1 (RotatE)");
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  Rows E = to_rows(ent), R = to_rows(rel);
+  B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
+  B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st));
+  if (n <= 0) return 0;
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  int64_t* sidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* pidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* oidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
+  BackBufs b;
+  if (!sidx || !pidx || !oidx || !lab || !take_back(ws, n, E.rows, E.dim, R.dim, round_up(f.K, 32), b)) {
+    set_error("workspace too small (see b200kge_train_1vsall_dropout_workspace_bytes)");
+    return B200KGE_ERR_WORKSPACE;
+  }
+  unpack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(triples, n, sidx, pidx, oidx, lab);
+  B2K_LAUNCH_CHECK("unpack_triples_kernel");
+  if ((rc = launch_identity_triples(n, b.tri, st))) return rc;
+  const Arena rest = rest_of(ws);
+  for (int dir = 0; dir < 2; ++dir) {
+    DirGrad g{lab + dir * n, nullptr, nullptr, 1.f, 0.f, 0.f, loss_kind, offset};
+    if ((rc = dropout_backward_dir(model, l_norm, dir, E, R, dir == 0 ? sidx : oidx, pidx, n, *drop, g, b.o, b.Q, b.dQ,
+                                   b.dT, b.dQe, b.dPr, b.tri, rest, d_ent, lde, d_rel, ldr, st))) return rc;
+  }
+  return 0;
+}
+
+size_t b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(int model, int64_t n, int64_t E, int32_t D, int64_t nnz) {
+  const size_t fwd = b200kge_score_1vsN_loss_csr_workspace_bytes(model, n, E, D, nnz);
+  const size_t bwd = b200kge_score_1vsN_backward_workspace_bytes(model, n, E, D) + 1024;
+  return masked_bytes(model, n, E, D) + (fwd > bwd ? fwd : bwd);
+}
+
+int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, float l_norm, int precision, const b200kge_rows_t* ent,
+                                        const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx, int64_t n,
+                                        const int64_t* csr_off, const int64_t* csr_col, int64_t nnz,
+                                        float label_smoothing, int loss_kind, float offset,
+                                        const b200kge_dropout_t* drop, float* loss_out, float* row_loss_out,
+                                        void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+  if (!ent || !rel || (!q_idx && n > 0) || (!p_idx && n > 0) || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
+  if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
+  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
+  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n <= 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  Rows E = to_rows(ent), R = to_rows(rel);
+  MaskedOps o;
+  if (!take_masked(ws, n, E.rows, E.dim, R.dim, o)) {
+    set_error("workspace too small (see b200kge_score_1vsN_loss_csr_dropout_workspace_bytes)");
+    return B200KGE_ERR_WORKSPACE;
+  }
+  Rows Qr, Pr, Tr;
+  if ((rc = gather_masked(dir_masks(*drop, combine), E, R, q_idx, p_idx, n, o, Qr, Pr, Tr, st))) return rc;
+  const b200kge_rows_t q{Qr.base, nullptr, n, Qr.ld, Qr.dim}, p{Pr.base, nullptr, n, Pr.ld, Pr.dim},
+      c{Tr.base, nullptr, Tr.rows, Tr.ld, Tr.dim};
+  const Arena rest = rest_of(ws);
+  return b200kge_score_1vsN_loss_csr(model, combine, l_norm, precision, &q, &p, &c, n, csr_off, csr_col, nnz,
+                                     label_smoothing, loss_kind, offset, loss_out, row_loss_out, rest.base, rest.cap,
+                                     stream);
+}
+
+int b200kge_score_1vsN_loss_csr_backward_dropout(int model, int combine, const b200kge_rows_t* ent,
+                                                 const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx,
+                                                 int64_t n, const int64_t* csr_off, const int64_t* csr_col,
+                                                 float label_smoothing, int loss_kind, float offset, int64_t batch_size,
+                                                 const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
+                                                 int64_t ldr, void* workspace, size_t workspace_bytes,
+                                                 b200kge_stream_t stream) {
+  if (!ent || !rel || !q_idx || !p_idx || !csr_off || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
+  if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
+  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
+  if (model > B200KGE_RESCAL) { set_error("the tensor-core backward covers the dot family only (model %d)", model); return B200KGE_ERR_UNSUPPORTED; }
+  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  if (batch_size <= 0 || !(label_smoothing >= 0.f && label_smoothing < 1.f)) { set_error("bad batch_size / label_smoothing"); return B200KGE_ERR_INVALID; }
+  if (lde < ent->dim || ldr < rel->dim) { set_error("leading dimensions too small"); return B200KGE_ERR_INVALID; }
+  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  Rows E = to_rows(ent), R = to_rows(rel);
+  B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
+  B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st));
+  if (n <= 0) return 0;
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  const Folded f = folded_problem(model, combine, E.dim, 1.0f);
+  BackBufs b;
+  if (!take_back(ws, n, E.rows, E.dim, R.dim, round_up(f.K, 32), b)) {
+    set_error("workspace too small (see b200kge_score_1vsN_loss_csr_dropout_workspace_bytes)");
+    return B200KGE_ERR_WORKSPACE;
+  }
+  if ((rc = launch_identity_triples(n, b.tri, st))) return rc;
+  const float a = 1.0f - label_smoothing, bb = label_smoothing > 0.f ? 1.0f / (float)E.rows : 0.f;
+  DirGrad g{q_idx /* placeholder index vector */, csr_off, csr_col, a, bb, 1.0f / (float)batch_size, loss_kind, offset};
+  return dropout_backward_dir(model, 1.0f, combine, E, R, q_idx, p_idx, n, *drop, g, b.o, b.Q, b.dQ, b.dT, b.dQe, b.dPr,
+                              b.tri, rest_of(ws), d_ent, lde, d_rel, ldr, st);
+}
+
+}  // extern "C"

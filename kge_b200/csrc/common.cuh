@@ -359,4 +359,25 @@ int loss_dense_nchunks(int64_t m);
 int launch_rank_dense(const float* scores, int64_t lds, int64_t n, int64_t m, const EpiParams& P,
                       cudaStream_t st);
 
+// Dropout masks (dropout.cu; layout in include/b200kge.h): one draw = one (stream, key).  Element (r, k) of a draw over
+// rows [row_base, row_base + rows) is kept iff its Philox word is below `thresh`; kept values are scaled by `scale`.
+struct DropMask {
+  uint64_t seed, call;
+  uint64_t thresh;      // floor((1 - p) * 2^32); 2^32 keeps everything
+  float scale;          // 1 / (1 - p)
+  int stream;
+  int64_t row_base;
+};
+int launch_dropout_mask(const DropMask& m, int64_t rows, int dim, uint8_t* out, cudaStream_t st);
+// dst[i, k] = mask(row_base + i, k) * src.row(i)[k]   (i < src.rows, k < src.dim)
+int launch_dropout_gather(const DropMask& m, const Rows& src, float* dst, int64_t ldd, cudaStream_t st);
+// dst[r, k] += mask(row_base + r, k) * src[r, k] for r < rows, k in [c0, c1) (row width `dim` keys the mask)
+int launch_dropout_add_cols(const DropMask& m, const float* src, int64_t lds, int64_t rows, int dim, int c0, int c1,
+                            float* dst, int64_t ldd, cudaStream_t st);
+// dst[idx[i], k] += mask(row_base + i, k) * src[i, k]   (atomic: rows of idx may repeat)
+int launch_dropout_scatter(const DropMask& m, const float* src, int64_t lds, int64_t rows, int dim, const int64_t* idx,
+                           float* dst, int64_t ldd, cudaStream_t st);
+// tri[3 i + j] = i: the triples under which the row-wise unfold writes row i's gradient into row i of [n, D] buffers
+int launch_identity_triples(int64_t n, int64_t* tri, cudaStream_t st);
+
 }  // namespace b200kge

@@ -10,6 +10,7 @@
 //    per-negative dot/distance; nothing of size [n*K, D] is materialised (the reference's `triple`
 //    implementation gathers 3 x [n*K, D]).  The P slot goes through spo_kernel with row divisors.
 #include "fold.cuh"
+#include "philox.cuh"
 
 namespace b200kge {
 
@@ -292,24 +293,12 @@ int launch_ns(int model, float l_norm, const Rows& s, const Rows& p, const Rows&
 // only — reproducible, no generator state.  Each 64-bit draw r maps to floor(r * vocab / 2^64) (bias <= vocab / 2^64).
 namespace {
 
-__device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
-  const uint32_t hi0 = __umulhi(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
-  const uint32_t hi1 = __umulhi(0xCD9E8D57u, c[2]), lo1 = 0xCD9E8D57u * c[2];
-  const uint32_t n0 = hi1 ^ c[1] ^ k0, n1 = lo1, n2 = hi0 ^ c[3] ^ k1, n3 = lo0;
-  c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
-}
-
 __global__ void __launch_bounds__(256)
 sample_uniform_kernel(uint64_t seed, uint64_t offset, uint64_t vocab, int64_t total, int64_t* __restrict__ out) {
   const int64_t pair = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;      // two ids per Philox block
   if (2 * pair >= total) return;
   uint32_t c[4] = {(uint32_t)pair, (uint32_t)((uint64_t)pair >> 32), (uint32_t)offset, (uint32_t)(offset >> 32)};
-  uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    philox_round(c, k0, k1);
-    k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-  }
+  philox4x32_10(c, seed);
   const uint64_t r0 = ((uint64_t)c[1] << 32) | c[0], r1 = ((uint64_t)c[3] << 32) | c[2];
   out[2 * pair] = (int64_t)__umul64hi(r0, vocab);
   if (2 * pair + 1 < total) out[2 * pair + 1] = (int64_t)__umul64hi(r1, vocab);

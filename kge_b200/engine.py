@@ -6,12 +6,12 @@ produced by libb200kge's hand-written sm_90a kernels.  All functions raise on CP
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import torch
 
 from . import _lib
-from ._lib import LOSS, MODELS, PREC, Labels, Rows, SP_, _PO
+from ._lib import LOSS, MODELS, PREC, Dropout, Labels, Rows, SP_, _PO
 
 S, P, O = 0, 1, 2
 
@@ -78,6 +78,33 @@ def _workspace(model_id: int, n: int, m: int, D: int, has_idx: bool, dev) -> tor
     nbytes = _lib.load().b200kge_workspace_bytes(model_id, n, m, D, 1 if has_idx else 0)
     # torch's caching allocator raises torch.cuda.OutOfMemoryError ("CUDA out of memory") on failure
     return torch.empty(nbytes, dtype=torch.uint8, device=dev)
+
+
+class DropoutKey(NamedTuple):
+    """Embedding dropout of one training sub-batch (b200kge_dropout_t): the rates of the entity and relation embedders
+    and the mask key.  Every mask element is a pure function of (seed, call, stream, global row, column), so the
+    backward, given the same key, regenerates the forward's masks."""
+    p_ent: float
+    p_rel: float
+    seed: int
+    call: int
+    row_base: int = 0
+
+    def struct(self) -> Dropout:
+        return Dropout(float(self.p_ent), float(self.p_rel), int(self.seed) & (2 ** 64 - 1),
+                       int(self.call) & (2 ** 64 - 1), int(self.row_base))
+
+
+def dropout_mask(p: float, seed: int, call: int, stream: int, rows: int, dim: int, row_base: int = 0,
+                 device="cuda") -> torch.Tensor:
+    """The keep mask [rows, dim] (uint8) of draw `stream` (0-5, include/b200kge.h) over global rows
+    [row_base, row_base + rows)."""
+    out = torch.empty((rows, dim), dtype=torch.uint8, device=device)
+    _require_cuda(out)
+    _lib.check(_lib.load().b200kge_dropout_mask(float(p), int(seed) & (2 ** 64 - 1), int(call) & (2 ** 64 - 1),
+                                                int(stream), int(row_base), rows, dim, out.data_ptr(),
+                                                _stream(out.device)))
+    return out
 
 
 def device_ok() -> bool:
@@ -387,9 +414,11 @@ def sample_uniform(n: int, K: int, vocab: int, seed: int, offset: int, device) -
 
 
 def train_1vsall_forward(model: str, ent, rel, triples, loss: str = "bce", offset: float = 0.0,
-                         l_norm: float = 1.0, precision: str = "auto", out=None, workspace=None):
+                         l_norm: float = 1.0, precision: str = "auto", out=None, workspace=None,
+                         dropout: Optional["DropoutKey"] = None):
     """One fused 1vsAll forward step for device-resident triples [n,3]; returns the 0-d loss
-    (loss(score_sp,o) + loss(score_po,s)) / n  (train_1vsAll.py:48-82)."""
+    (loss(score_sp,o) + loss(score_po,s)) / n  (train_1vsAll.py:48-82).  With `dropout` the six embedding-dropout draws
+    of the step are applied (b200kge_train_1vsall_forward_dropout; `workspace` is not used)."""
     _require_cuda(ent, rel, triples)
     lib, k = _lib.load(), _Keep()
     re_, rr = k.rows(ent), k.rows(rel)
@@ -398,6 +427,13 @@ def train_1vsall_forward(model: str, ent, rel, triples, loss: str = "bce", offse
     dev = ent.device
     if out is None:
         out = torch.empty((), dtype=torch.float32, device=dev)
+    if dropout is not None:
+        ws = torch.empty(lib.b200kge_train_1vsall_dropout_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1]),
+                         dtype=torch.uint8, device=dev)
+        _lib.check(lib.b200kge_train_1vsall_forward_dropout(
+            MODELS[model], l_norm, PREC[precision], C.byref(re_), C.byref(rr), tri.data_ptr(), n, LOSS[loss], offset,
+            C.byref(dropout.struct()), out.data_ptr(), ws.data_ptr(), ws.numel(), _stream(dev)))
+        return out
     ws = workspace if workspace is not None else _workspace(MODELS[model], n, ent.shape[0], ent.shape[1], False, dev)
     _lib.check(lib.b200kge_train_1vsall_forward(
         MODELS[model], l_norm, PREC[precision], C.byref(re_), C.byref(rr), tri.data_ptr(), n, LOSS[loss],
@@ -497,8 +533,10 @@ def gemm_nt(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     return out
 
 
-def train_1vsall_backward(model: str, ent, rel, triples, loss: str = "bce", offset: float = 0.0, l_norm: float = 1.0):
-    """(d_ent, d_rel): dense table gradients of train_1vsall_forward's loss (dot family; TransE L1/L2; RotatE L1)."""
+def train_1vsall_backward(model: str, ent, rel, triples, loss: str = "bce", offset: float = 0.0, l_norm: float = 1.0,
+                          dropout: Optional["DropoutKey"] = None):
+    """(d_ent, d_rel): dense table gradients of train_1vsall_forward's loss (dot family; TransE L1/L2; RotatE L1), with
+    the forward's dropout masks when `dropout` is the forward's key."""
     _require_cuda(ent, rel, triples)
     lib, k = _lib.load(), _Keep()
     re_, rr = k.rows(ent), k.rows(rel)
@@ -507,6 +545,14 @@ def train_1vsall_backward(model: str, ent, rel, triples, loss: str = "bce", offs
     dev = ent.device
     d_ent = torch.empty_like(_f32(ent))
     d_rel = torch.empty_like(_f32(rel))
+    if dropout is not None:
+        ws = torch.empty(lib.b200kge_train_1vsall_dropout_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1]),
+                         dtype=torch.uint8, device=dev)
+        _lib.check(lib.b200kge_train_1vsall_backward_dropout(
+            MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), n, LOSS[loss], offset,
+            C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0),
+            ws.data_ptr(), ws.numel(), _stream(dev)))
+        return d_ent, d_rel
     nbytes = lib.b200kge_train_1vsall_backward_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1])
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     _lib.check(lib.b200kge_train_1vsall_backward(
@@ -537,8 +583,10 @@ def score_1vsN_backward(model: str, combine: str, ent, rel, q, p, grad_scores, l
 
 
 def score_1vsN_loss_csr_backward(model: str, combine: str, ent, rel, q, p, csr_offsets, csr_cols, loss: str = "kl",
-                                 offset: float = 0.0, label_smoothing: float = 0.0, batch_size: Optional[int] = None):
-    """(d_ent, d_rel) of score_1vsN_loss_csr(...) / batch_size over the whole entity table (dot family)."""
+                                 offset: float = 0.0, label_smoothing: float = 0.0, batch_size: Optional[int] = None,
+                                 dropout: Optional["DropoutKey"] = None):
+    """(d_ent, d_rel) of score_1vsN_loss_csr(...) / batch_size over the whole entity table (dot family), with the
+    forward's dropout masks when `dropout` is the forward's key."""
     _require_cuda(ent, rel, csr_offsets, csr_cols)
     lib, k = _lib.load(), _Keep()
     re_, rr = k.rows(ent), k.rows(rel)
@@ -547,6 +595,15 @@ def score_1vsN_loss_csr_backward(model: str, combine: str, ent, rel, q, p, csr_o
     dev = ent.device
     d_ent = torch.empty_like(_f32(ent))
     d_rel = torch.empty_like(_f32(rel))
+    if dropout is not None:
+        ws = torch.empty(lib.b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(
+            MODELS[model], n, ent.shape[0], ent.shape[1], int(cols.numel())), dtype=torch.uint8, device=dev)
+        _lib.check(lib.b200kge_score_1vsN_loss_csr_backward_dropout(
+            MODELS[model], SP_ if combine == "sp_" else _PO, C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n,
+            offs.data_ptr(), cols.data_ptr() if cols.numel() else None, label_smoothing, LOSS[loss], offset,
+            batch_size or n, C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(),
+            d_rel.stride(0), ws.data_ptr(), ws.numel(), _stream(dev)))
+        return d_ent, d_rel
     ws = torch.empty(lib.b200kge_score_1vsN_backward_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1]),
                      dtype=torch.uint8, device=dev)
     _lib.check(lib.b200kge_score_1vsN_loss_csr_backward(
@@ -672,8 +729,10 @@ def ns_loss(scores, loss: str, arg: float = 0.0, temperature: float = 1.0, label
 
 def score_1vsN_loss_csr(model: str, combine: str, q_tab, rel, cand_tab, csr_offsets, csr_cols, q=None, p=None,
                           loss: str = "kl", offset: float = 0.0, label_smoothing: float = 0.0, l_norm: float = 1.0,
-                          precision: str = "auto", return_rows: bool = False):
-    """KvsAll loss (sum over rows) with CSR multi-hot labels — see b200kge_score_1vsN_loss_csr."""
+                          precision: str = "auto", return_rows: bool = False, dropout: Optional["DropoutKey"] = None):
+    """KvsAll loss (sum over rows) with CSR multi-hot labels — see b200kge_score_1vsN_loss_csr.  With `dropout` the three
+    embedding-dropout draws of the query type are applied (b200kge_score_1vsN_loss_csr_dropout): the queries are rows
+    q of the entity table q_tab, which must also be the candidate table."""
     _require_cuda(q_tab, rel, cand_tab, csr_offsets, csr_cols)
     lib, k = _lib.load(), _Keep()
     rq, rp, rc = k.rows(q_tab, q), k.rows(rel, p), k.rows(cand_tab)
@@ -683,6 +742,20 @@ def score_1vsN_loss_csr(model: str, combine: str, q_tab, rel, cand_tab, csr_offs
     nnz = int(cols.numel())
     out = torch.empty((), dtype=torch.float32, device=dev)
     rows = torch.empty(n, dtype=torch.float32, device=dev) if return_rows else None
+    if dropout is not None:
+        if q is None or p is None or q_tab.data_ptr() != cand_tab.data_ptr():
+            raise ValueError("dropout needs query indexes into the candidate table (q_tab is cand_tab) and relation indexes")
+        re_, rr = k.rows(cand_tab), k.rows(rel)
+        qi, pi = _i64(q), _i64(p)
+        k.refs += [qi, pi]
+        ws = torch.empty(lib.b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(MODELS[model], n, m, rq.dim, nnz),
+                         dtype=torch.uint8, device=dev)
+        _lib.check(lib.b200kge_score_1vsN_loss_csr_dropout(
+            MODELS[model], SP_ if combine == "sp_" else _PO, l_norm, PREC[precision], C.byref(re_), C.byref(rr),
+            qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(), cols.data_ptr() if nnz else None, nnz, label_smoothing,
+            LOSS[loss], offset, C.byref(dropout.struct()), out.data_ptr(), rows.data_ptr() if rows is not None else None,
+            ws.data_ptr(), ws.numel(), _stream(dev)))
+        return (out, rows) if return_rows else out
     nbytes = lib.b200kge_score_1vsN_loss_csr_workspace_bytes(MODELS[model], n, m, rq.dim, nnz)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     _lib.check(lib.b200kge_score_1vsN_loss_csr(

@@ -17,6 +17,9 @@ The classes subclass the reference's `KgeModel` / `RelationalScorer` (kge_model.
    the embedding tables in place (the LookupEmbedder gather is fused, no `embed_all()` table copy)
    whenever both embedders are plain LookupEmbedders with dropout inactive; otherwise the
    reference's embedders run and the scorer-level path takes over.
+ * with embedding dropout active in training, the 1vsAll / KvsAll job plugins take the dropout entry points
+   (`loss_1vsall` / `loss_kvsall*` with an engine.DropoutKey: masks drawn on the device with the distribution of the
+   reference's draws); the unmodified jobs' score_sp / score_po and score_sp_po keep the routes above.
  * extra fused methods `score_sp_loss / score_po_loss / rank_sp / rank_po` for job plugins.
 
 CUDA only: CPU tensors raise (no fallback).  Backward (SURVEY 8f-1, "next") is provided by
@@ -120,21 +123,23 @@ class _TableScoreFn(torch.autograd.Function):
 
 
 class _Loss1vsAllFn(torch.autograd.Function):
-    """Fused 1vsAll step: (loss(score_sp, o) + loss(score_po, s)) / n as ONE launch sequence."""
+    """Fused 1vsAll step: (loss(score_sp, o) + loss(score_po, s)) / n as ONE launch sequence.  With a dropout key
+    (engine.DropoutKey) the step applies embedding dropout and the backward regenerates the same masks from the key."""
 
     @staticmethod
-    def forward(ctx, ent_w, rel_w, model, triples, loss, offset):
-        ctx.model, ctx.loss, ctx.offset = model, loss, offset
+    def forward(ctx, ent_w, rel_w, model, triples, loss, offset, dropout=None):
+        ctx.model, ctx.loss, ctx.offset, ctx.dropout = model, loss, offset, dropout
         ctx.save_for_backward(ent_w, rel_w, triples)
         ln, prec = model._b200_args()
+        kw = {} if dropout is None else {"dropout": dropout}
         return engine.train_1vsall_forward(model._b200_name, ent_w.detach(), rel_w.detach(), triples, loss, offset,
-                                           ln, prec)
+                                           ln, prec, **kw)
 
     @staticmethod
     def backward(ctx, g):
         ent_w, rel_w, triples = ctx.saved_tensors
-        d_ent, d_rel = ctx.model._b200_loss_1vsall_backward(ent_w, rel_w, triples, ctx.loss, ctx.offset)
-        return d_ent * g, d_rel * g, None, None, None, None
+        d_ent, d_rel = ctx.model._b200_loss_1vsall_backward(ent_w, rel_w, triples, ctx.loss, ctx.offset, ctx.dropout)
+        return d_ent * g, d_rel * g, None, None, None, None, None
 
 
 def _penalty_torch(emb, w, regularize, rw, p, weighted, indexes):
@@ -181,8 +186,8 @@ def _install_embedder_kernels(emb):
 
     def penalty(**kwargs):
         w = emb._embeddings.weight
-        if (not w.is_cuda or emb.regularize not in ("lp", "n3") or emb.get_option("regularize_weight") == 0.0
-                or (emb.dropout.p > 0 and emb.training)):
+        # the reference's penalty reads _embeddings directly, so dropout never enters it (lookup_embedder.py:139,153)
+        if not w.is_cuda or emb.regularize not in ("lp", "n3") or emb.get_option("regularize_weight") == 0.0:
             return cls.penalty(emb, **kwargs)
         if emb.regularize == "n3":
             p = 3
@@ -212,23 +217,26 @@ def _install_embedder_kernels(emb):
 
 class _KvsAllLossFn(torch.autograd.Function):
     """KvsAll loss of one query type with CSR labels / batch_size: forward = fused score + loss with the CSR consumed in
-    the epilogue; backward = the gradient kernels (b200kge_score_1vsN_loss_csr_backward)."""
+    the epilogue; backward = the gradient kernels (b200kge_score_1vsN_loss_csr_backward).  With a dropout key both run
+    the dropout entry points under the same masks."""
 
     @staticmethod
-    def forward(ctx, ent_w, rel_w, model, combine, a, p, offs, cols, loss, offset, smoothing, batch_size):
-        ctx.args = (model, combine, loss, offset, smoothing, batch_size)
+    def forward(ctx, ent_w, rel_w, model, combine, a, p, offs, cols, loss, offset, smoothing, batch_size, dropout=None):
+        ctx.args = (model, combine, loss, offset, smoothing, batch_size, dropout)
         ctx.save_for_backward(ent_w, rel_w, a, p, offs, cols)
         ln, prec = model._b200_args()
+        kw = {} if dropout is None else {"dropout": dropout}
         return engine.score_1vsN_loss_csr(model._b200_name, combine, ent_w.detach(), rel_w.detach(), ent_w.detach(), offs,
-                                          cols, a, p, loss, offset, smoothing, ln, prec) / batch_size
+                                          cols, a, p, loss, offset, smoothing, ln, prec, **kw) / batch_size
 
     @staticmethod
     def backward(ctx, g):
         ent_w, rel_w, a, p, offs, cols = ctx.saved_tensors
-        model, combine, loss, offset, smoothing, batch_size = ctx.args
+        model, combine, loss, offset, smoothing, batch_size, dropout = ctx.args
+        kw = {} if dropout is None else {"dropout": dropout}
         d_ent, d_rel = engine.score_1vsN_loss_csr_backward(model._b200_name, combine, ent_w.detach(), rel_w.detach(), a, p,
-                                                           offs, cols, loss, offset, smoothing, batch_size)
-        return (d_ent * g, d_rel * g) + (None,) * 10
+                                                           offs, cols, loss, offset, smoothing, batch_size, **kw)
+        return (d_ent * g, d_rel * g) + (None,) * 11
 
 
 class _NsSlotLossFn(torch.autograd.Function):
@@ -300,6 +308,15 @@ class _B200ModelMixin:
                 return False
         return es is eo
 
+    def b200_dropout_rates(self):
+        """(p_ent, p_rel) when embedding dropout is active (training mode, a rate > 0) on plain LookupEmbedders that
+        share one entity table — the case the dropout entry points of the 1vsAll / KvsAll steps serve — else None.
+        Independent of b200_fusable(), which stays False while dropout is active."""
+        es, ep, eo = self.get_s_embedder(), self.get_p_embedder(), self.get_o_embedder()
+        if es is not eo or type(es) is not LookupEmbedder or type(ep) is not LookupEmbedder:
+            return None
+        rates = tuple(float(e.dropout.p) if e.training else 0.0 for e in (es, ep))
+        return rates if max(rates) > 0 else None
 
     def b200_csr_labels_ok(self, label_smoothing):
         return label_smoothing == 0.0 or self._b200_name in ("complex", "distmult", "simple", "cp", "rescal")
@@ -370,10 +387,16 @@ class _B200ModelMixin:
             out = self._b200_ref_scores(e, r, kind, a, p, b)
             return torch.autograd.grad(out, (e, r), grad_out.reshape(out.shape), allow_unused=False)
 
-    def _b200_loss_1vsall_backward(self, ent_w, rel_w, triples, loss, offset):
+    def b200_1vsall_native_backward_ok(self):
+        return self.b200_backward == "native" and self._b200_native_family()
+
+    def _b200_loss_1vsall_backward(self, ent_w, rel_w, triples, loss, offset, dropout=None):
         name = self._b200_name
         ln = self._b200_args()[0]
-        if self.b200_backward == "native" and self._b200_native_family():
+        if dropout is not None:       # no recompute form: the engine refuses what its kernels do not cover
+            return engine.train_1vsall_backward(name, ent_w.detach(), rel_w.detach(), triples, loss, offset, ln,
+                                                dropout=dropout)
+        if self.b200_1vsall_native_backward_ok():
             return engine.train_1vsall_backward(name, ent_w.detach(), rel_w.detach(), triples, loss, offset, ln)
         e, r = ent_w.detach().requires_grad_(True), rel_w.detach().requires_grad_(True)
         n = triples.shape[0]
@@ -417,13 +440,18 @@ class _B200ModelMixin:
         return self._b200_call("sp_po", torch.cat((s.reshape(-1), o.reshape(-1))), p, entity_subset)
 
     # -- fused forms for the job plugins (kge_b200/plugin/jobs.py): scores never reach HBM
-    def loss_1vsall(self, triples, loss="bce", offset=0.0, need_grad=None):
-        """(loss(score_sp, o) + loss(score_po, s)) / n for a [n,3] batch (train_1vsAll.py:48-82)."""
+    def loss_1vsall(self, triples, loss="bce", offset=0.0, need_grad=None, dropout=None):
+        """(loss(score_sp, o) + loss(score_po, s)) / n for a [n,3] batch (train_1vsAll.py:48-82); `dropout` (an
+        engine.DropoutKey) applies embedding dropout with the masks of that key."""
         ent_w, rel_w = self._b200_weights()
         if need_grad is None:
             need_grad = self._b200_needs_grad()
         if need_grad and self._b200_needs_grad():
-            return _Loss1vsAllFn.apply(ent_w, rel_w, self, triples, loss, offset)
+            return _Loss1vsAllFn.apply(ent_w, rel_w, self, triples, loss, offset, dropout)
+        if dropout is not None:
+            ln, prec = self._b200_args()
+            return engine.train_1vsall_forward(self._b200_name, ent_w.detach(), rel_w.detach(), triples, loss, offset,
+                                               ln, prec, dropout=dropout)
         return self._b200_prepared_step(ent_w, rel_w, triples.shape[0], loss, offset)(triples)
 
     def _b200_prepared_step(self, ent_w, rel_w, n, loss, offset):
@@ -442,21 +470,26 @@ class _B200ModelMixin:
         ent_w, rel_w = self._b200_weights()
         return self._b200_prepared_step(ent_w, rel_w, triples_host.shape[0], loss, offset).call_host(triples_host)
 
-    def loss_kvsall(self, combine, a, p, csr_offsets, csr_cols, loss="kl", offset=0.0, label_smoothing=0.0):
-        """Sum over rows of the KvsAll loss with CSR multi-hot labels (train_KvsAll.py:242-294); forward only."""
+    def loss_kvsall(self, combine, a, p, csr_offsets, csr_cols, loss="kl", offset=0.0, label_smoothing=0.0,
+                    dropout=None):
+        """Sum over rows of the KvsAll loss with CSR multi-hot labels (train_KvsAll.py:242-294); forward only.
+        `dropout` (an engine.DropoutKey) applies embedding dropout with the masks of that key."""
         ent, rel = self._b200_tables()
         ln, prec = self._b200_args()
+        kw = {} if dropout is None else {"dropout": dropout}
         return engine.score_1vsN_loss_csr(self._b200_name, combine, ent, rel, ent, csr_offsets, csr_cols, a, p,
-                                          loss, offset, label_smoothing, ln, prec)
+                                          loss, offset, label_smoothing, ln, prec, **kw)
 
     def b200_kvsall_native_backward_ok(self):
         return self.b200_backward == "native" and self._b200_name in ("complex", "distmult", "simple", "cp", "rescal")
 
-    def loss_kvsall_train(self, combine, a, p, csr_offsets, csr_cols, loss, offset, label_smoothing, batch_size):
+    def loss_kvsall_train(self, combine, a, p, csr_offsets, csr_cols, loss, offset, label_smoothing, batch_size,
+                          dropout=None):
         """loss_kvsall / batch_size as a differentiable scalar (train_KvsAll.py:286-294)."""
         ent_w, rel_w = self._b200_weights()
         return _KvsAllLossFn.apply(ent_w, rel_w, self, combine, a.long().contiguous(), p.long().contiguous(),
-                                   csr_offsets, csr_cols, loss, float(offset), float(label_smoothing), int(batch_size))
+                                   csr_offsets, csr_cols, loss, float(offset), float(label_smoothing), int(batch_size),
+                                   dropout)
 
     def score_negatives(self, triples, negatives, slot):
         """[n, 1+K]: the positive triple's score in column 0, its K corrupted versions after it

@@ -12,8 +12,10 @@ config.modules(), ...)`), i.e. in a LibKGE config:
 
 Everything else of the job (data loading, collate, sub-batching, trace entries, penalties, optimizer, hooks,
 checkpoints) is the reference's code, unchanged.  Whenever a fused form is not available for the configured
-combination (a non-b200 model, a loss outside the fused set, dropout active, ...) the method falls through to
-the reference implementation, which then still reaches the kernels through `model.score_*`.
+combination (a non-b200 model, a loss outside the fused set, ...) the method falls through to the reference
+implementation, which then still reaches the kernels through `model.score_*`.  Embedding dropout in training takes the
+dropout entry points in the 1vsAll and KvsAll jobs (masks drawn on the device, keyed per sub-batch); the
+negative-sampling job with dropout keeps the reference step.
 """
 from __future__ import annotations
 
@@ -27,6 +29,8 @@ from kge.job.train_negative_sampling import TrainingJobNegativeSampling
 from kge.job import Job
 from kge.util.loss import (BCEWithLogitsKgeLoss, KLDivWithSoftmaxKgeLoss, MarginRankingKgeLoss, SEKgeLoss,
                            SoftMarginKgeLoss)
+
+from .. import engine
 
 S, P, O = 0, 1, 2
 SLOT_STR = ["s", "p", "o"]
@@ -66,6 +70,33 @@ def _fused_model(model):
     if getattr(model, "_b200_name", None) is None or not hasattr(model, "b200_fusable"):
         return None
     return model if model.b200_fusable() else None
+
+
+def _dropout_model(model):
+    """(b200 model, (p_ent, p_rel)) if embedding dropout is active and the dropout entry points can serve the model's
+    tables, else (None, None)."""
+    if getattr(model, "_b200_name", None) is None or not hasattr(model, "b200_dropout_rates"):
+        return None, None
+    rates = model.b200_dropout_rates()
+    return (model, rates) if rates is not None else (None, None)
+
+
+def dropout_call(epoch, batch_index, ordinal):
+    """The `call` word of a sub-batch's dropout key: a pure function of (epoch, batch index, sub-batch ordinal within
+    the batch), so a resumed run draws the same masks."""
+    return ((int(epoch) << 40) | (int(batch_index) << 16) | int(ordinal)) & (2 ** 64 - 1)
+
+
+class _DropoutKeys:
+    """One engine.DropoutKey per sub-batch: seed = torch.initial_seed() (as the device sampler), call from
+    (epoch, batch index, sub-batch ordinal), row_base = the sub-batch's first row in the batch."""
+
+    def _b200_dropout_key(self, rates, batch_index, subbatch_slice):
+        pos = (self.epoch, batch_index)
+        ordinal = self._b200_drop_ordinal + 1 if getattr(self, "_b200_drop_pos", None) == pos else 0
+        self._b200_drop_pos, self._b200_drop_ordinal = pos, ordinal
+        return engine.DropoutKey(rates[0], rates[1], torch.initial_seed(), dropout_call(self.epoch, batch_index, ordinal),
+                                 subbatch_slice.start or 0)
 
 
 def _user_option(config, key, default=None):
@@ -131,7 +162,7 @@ class _BatchSplit:
         return result
 
 
-class B200TrainingJob1vsAll(_BatchSplit, TrainingJob1vsAll):
+class B200TrainingJob1vsAll(_DropoutKeys, _BatchSplit, TrainingJob1vsAll):
     """`TrainingJob1vsAll` (train_1vsAll.py:10-82) with the sub-batch step as ONE fused call:
     (loss(score_sp, o) + loss(score_po, s)) / batch_size, both directions stacked into one problem."""
 
@@ -146,12 +177,18 @@ class B200TrainingJob1vsAll(_BatchSplit, TrainingJob1vsAll):
         if subbatch_slice is None:
             return
         model, kind = _fused_model(self.model), _fused_loss_kind(self.loss)
+        rates = None
+        if model is None:
+            model, rates = _dropout_model(self.model)
+            if model is not None and not self.is_forward_only and not model.b200_1vsall_native_backward_ok():
+                model = None
         if model is None or kind is None:
             return super()._process_subbatch(batch_index, batch, subbatch_slice, result)
         batch_size = result.size
+        drop = None if rates is None else self._b200_dropout_key(rates, batch_index, subbatch_slice)
 
         host = batch["triples"][subbatch_slice]
-        if (self.is_forward_only and not host.is_cuda and host.dtype == torch.int64 and host.is_contiguous()
+        if (drop is None and self.is_forward_only and not host.is_cuda and host.dtype == torch.int64 and host.is_contiguous()
                 and len(host) > 0):
             # forward only: batch copy, kernels and the scalar read-back in ONE library call (no torch ops in between)
             result.forward_time -= time.time()
@@ -169,7 +206,8 @@ class B200TrainingJob1vsAll(_BatchSplit, TrainingJob1vsAll):
         result.forward_time -= time.time()
         # sum over both directions and all rows of the sub-batch, divided by the sub-batch size by the kernel's
         # finaliser; the reference divides by the size of the whole batch (train_1vsAll.py:65,76)
-        loss_value = model.loss_1vsall(triples, kind[0], kind[1], need_grad=not self.is_forward_only)
+        kw = {} if drop is None else {"dropout": drop}
+        loss_value = model.loss_1vsall(triples, kind[0], kind[1], need_grad=not self.is_forward_only, **kw)
         if len(triples) != batch_size:
             loss_value = loss_value * (len(triples) / batch_size)
         result.avg_loss += loss_value.item()
@@ -181,7 +219,7 @@ class B200TrainingJob1vsAll(_BatchSplit, TrainingJob1vsAll):
         result.backward_time += time.time()
 
 
-class B200TrainingJobKvsAll(_BatchSplit, TrainingJobKvsAll):
+class B200TrainingJobKvsAll(_DropoutKeys, _BatchSplit, TrainingJobKvsAll):
     """`TrainingJobKvsAll` (train_KvsAll.py:205-294): per query type one fused score+loss call that consumes the
     batch's label coordinates as CSR (no dense [n, E] label matrix: job/util.py:32-60 + `.to_dense()`,
     train_KvsAll.py:242-266 are not executed)."""
@@ -197,11 +235,16 @@ class B200TrainingJobKvsAll(_BatchSplit, TrainingJobKvsAll):
         if subbatch_slice is None:
             return
         model, kind = _fused_model(self.model), _fused_loss_kind(self.loss)
+        rates = None
+        if model is None:
+            model, rates = _dropout_model(self.model)
         qtypes = [q for q in self.query_types]
         if (model is None or kind is None or "s_o" in qtypes or not model.b200_csr_labels_ok(self.label_smoothing)
                 or (not self.is_forward_only and not model.b200_kvsall_native_backward_ok())):
             return super()._process_subbatch(batch_index, batch, subbatch_slice, result)
         batch_size = result.size
+        # one key per sub-batch: the sp_ and _po query types draw disjoint mask streams under it
+        kw = {} if rates is None else {"dropout": self._b200_dropout_key(rates, batch_index, subbatch_slice)}
 
         result.prepare_time -= time.time()
         queries = batch["queries"][subbatch_slice].to(self.device)
@@ -241,10 +284,10 @@ class B200TrainingJobKvsAll(_BatchSplit, TrainingJobKvsAll):
                 combine, ent_idx, rel_idx = "_po", queries[examples, 1], queries[examples, 0]
             if self.is_forward_only:
                 loss_value = model.loss_kvsall(combine, ent_idx, rel_idx, offsets, ccols, kind[0], kind[1],
-                                               self.label_smoothing) / batch_size
+                                               self.label_smoothing, **kw) / batch_size
             else:
                 loss_value = model.loss_kvsall_train(combine, ent_idx, rel_idx, offsets, ccols, kind[0], kind[1],
-                                                     self.label_smoothing, batch_size)
+                                                     self.label_smoothing, batch_size, **kw)
             result.avg_loss += loss_value.item()
             result.forward_time += time.time()
             result.backward_time -= time.time()
