@@ -491,6 +491,46 @@ int b200kge_score_1vsN_loss_csr_backward_dropout(int model, int combine, const b
                                                  int64_t ldr, void* workspace, size_t workspace_bytes,
                                                  b200kge_stream_t stream);
 
+/* ---- Embedding dropout of the negative-sampling training step ------------------------------------------------------
+ * Per slot (0 = S or 2 = O; the P slot is not served) and sub-batch, train_negative_sampling.py:139-148 makes six draws,
+ * numbered as mask streams 6 + 6 * slot + j (streams 12-17, the P slot's, are reserved):
+ *   j = 0, 1, 2  score_spo(s, p, o) of the positive column: the s, p and o rows, mask row = row_base + i
+ *   j = 3, 4, 5  the negatives' s, p and o draws:
+ *     B200KGE_NS_TRIPLE (score_spo over the n K corrupted triples, sampler.py:291-306): mask row = (row_base + i) K + j'
+ *                       for all three operands of triple (i, j'), the sampled entity included;
+ *     B200KGE_NS_BATCH  (score_sp / score_po against the unique sampled ids, sampler.py:307-356; `all` draws the same
+ *                       distribution): mask row = row_base + i for the two fixed operands, the ENTITY ID for the open
+ *                       slot, so every row and repeat that samples an id shares its mask.
+ * Everything else is the layout above (key, counter, threshold, scale).  Rows are global within the batch, so the masks
+ * do not depend on the sub-batch size.  Requirements (else B200KGE_ERR_INVALID): those of b200kge_dropout_mask for every
+ * element of every draw, i.e. (mask row + 1) * width <= 2^48 with width D for entities and the relation width (D^2 for
+ * RESCAL) for relations. */
+#define B200KGE_NS_TRIPLE 0
+#define B200KGE_NS_BATCH 1
+
+/* b200kge_ns_score of one slot with dropout: out [n, 1 + K] (row stride ldo) receives the masked positive in column 0 and
+ * the masked negatives neg [n, K] after it.  `ent` / `rel` are the plain tables, `triples` [n, 3] the sub-batch.
+ * Coverage: slots S and O; the dot family (RESCAL included), TransE l_norm 1 / 2, RotatE l_norm 1; every row width a
+ * multiple of 4 (D % 8 == 0 for ComplEx, SimplE, CP and RotatE).  Anything else returns B200KGE_ERR_UNSUPPORTED before
+ * a launch.  TransE adds pairwise_distance's eps to the positive and `triple` scores, not to `batch` ones (cdist). */
+int b200kge_ns_score_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                             const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
+                             const b200kge_dropout_t* drop, float* out, int64_t ldo, b200kge_stream_t stream);
+
+/* Backward of b200kge_ns_score_dropout under the same key: grad_scores [n, 1 + K] (row stride ldg) holds dL/dz already
+ * scaled (the grad_out of b200kge_ns_loss), so every loss trains through it.  The masks are regenerated, the gradients of
+ * the masked operands are masked and scaled again and ADDED into d_ent [E, lde] / d_rel [R, ldr].  Same coverage as the
+ * forward; B200KGE_NS_BATCH (not RESCAL) also needs D <= 1024.  The positive column and `triple` run row-wise (one warp
+ * per triple); the `batch` negatives run ns_kernel / ns_backward_kernel with a mask policy (q folded once per row from
+ * the masked fixed rows, sampled rows masked by id, the fixed rows' gradient reduced per row).
+ * workspace: b200kge_ns_dropout_workspace_bytes(model, n, K, D) bytes (K is not used). */
+size_t b200kge_ns_dropout_workspace_bytes(int model, int64_t n, int64_t K, int32_t D);
+int b200kge_ns_backward_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
+                                const b200kge_dropout_t* drop, const float* grad_scores, int64_t ldg, float* d_ent,
+                                int64_t lde, float* d_rel, int64_t ldr, void* workspace, size_t workspace_bytes,
+                                b200kge_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

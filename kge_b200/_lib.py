@@ -138,7 +138,16 @@ SIGNATURES = {
                                                                C.c_float, C.c_int64, _DP, C.c_void_p, C.c_int64,
                                                                C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t,
                                                                C.c_void_p]),
+    "b200kge_ns_score_dropout": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
+                                           C.c_int64, C.c_int, _DP, C.c_void_p, C.c_int64, C.c_void_p]),
+    "b200kge_ns_dropout_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32]),
+    "b200kge_ns_backward_dropout": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
+                                              C.c_int64, C.c_int, _DP, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                              C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
+
+#: negative-sampling scoring implementations of the dropout entry points (B200KGE_NS_*); "all" draws like "batch"
+NS_IMPL = {"triple": 0, "batch": 1, "all": 1}
 
 _lib = None
 

@@ -1532,3 +1532,88 @@ int b200kge_score_1vsN_loss_csr_backward_dropout(int model, int combine, const b
 }
 
 }  // extern "C"
+
+// ==================================================================================================
+// Embedding dropout of one negative-sampling slot (layout: include/b200kge.h, kernels: ns_dropout.cu).
+namespace {
+
+int validate_ns_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                        const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
+                        const b200kge_dropout_t* drop) {
+  if (!ent || !rel || (!triples && n > 0) || (!neg && n * K > 0)) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (n < 0 || K < 0) { set_error("negative sizes"); return B200KGE_ERR_INVALID; }
+  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
+  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
+  if ((rc = validate_norm(model, l_norm))) return rc;
+  if (impl != B200KGE_NS_TRIPLE && impl != B200KGE_NS_BATCH) { set_error("impl must be B200KGE_NS_TRIPLE or B200KGE_NS_BATCH"); return B200KGE_ERR_INVALID; }
+  if (slot != 0 && slot != 2) { set_error("negative-sampling dropout covers the S and O slots"); return B200KGE_ERR_UNSUPPORTED; }
+  if ((model == B200KGE_TRANSE && l_norm != 1.0f && l_norm != 2.0f) || (model == B200KGE_ROTATE && l_norm != 1.0f)) {
+    set_error("negative-sampling dropout covers l_norm 1 and 2 (TransE) / 1 (RotatE)");
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  const int D = ent->dim;
+  const bool halves = model == B200KGE_COMPLEX || model == B200KGE_SIMPLE || model == B200KGE_CP || model == B200KGE_ROTATE;
+  if (D % (halves ? 8 : 4) != 0) {
+    set_error("negative-sampling dropout needs D %% %d == 0 (got %d)", halves ? 8 : 4, D);
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  if (!drop) { set_error("null dropout key"); return B200KGE_ERR_INVALID; }
+  if (impl == B200KGE_NS_BATCH && model != B200KGE_RESCAL && D > 1024) {
+    set_error("negative-sampling dropout with `batch` covers D <= 1024 (got %d)", D);
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  if ((rc = validate_dropout(drop, n, ent->rows, D, rel->dim))) return rc;
+  // `triple` mask rows reach (row_base + n) K - 1: bound them in double, before any int64 product can overflow
+  const double lim = 281474976710656.0;    // 2^48
+  const double top = ((double)drop->row_base + (double)n) * (double)(K > 0 ? K : 1);
+  if (impl == B200KGE_NS_TRIPLE && (top * ent->dim > lim || top * rel->dim > lim)) {
+    set_error("dropout rows out of range: row * dim + k < 2^48 is required");
+    return B200KGE_ERR_INVALID;
+  }
+  return 0;
+}
+
+NsDropKeys ns_drop_keys(const b200kge_dropout_t& d) {
+  NsDropKeys k;
+  k.ent = drop_mask(d.p_ent, d.seed, d.call, 0, 0);
+  k.rel = drop_mask(d.p_rel, d.seed, d.call, 0, 0);
+  k.row_base = d.row_base;
+  return k;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b200kge_ns_score_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                             const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
+                             const b200kge_dropout_t* drop, float* out, int64_t ldo, b200kge_stream_t stream) {
+  int rc = validate_ns_dropout(model, l_norm, ent, rel, triples, slot, neg, n, K, impl, drop); if (rc) return rc;
+  if (n == 0) return 0;
+  if (!out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (ldo < K + 1) { set_error("out is narrower than the 1 + K columns of the block"); return B200KGE_ERR_INVALID; }
+  return launch_ns_dropout(model, l_norm, to_rows(ent), to_rows(rel), triples, slot, neg, n, K, impl, ns_drop_keys(*drop),
+                           nullptr, 0, out, ldo, nullptr, 0, nullptr, 0, nullptr, 0, (cudaStream_t)stream);
+}
+
+size_t b200kge_ns_dropout_workspace_bytes(int model, int64_t n, int64_t K, int32_t D) {
+  (void)K;
+  return (n > 0 && D > 0) ? ns_dropout_workspace_bytes(model, n, D) : 0;
+}
+
+int b200kge_ns_backward_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
+                                const b200kge_dropout_t* drop, const float* grad_scores, int64_t ldg, float* d_ent,
+                                int64_t lde, float* d_rel, int64_t ldr, void* workspace, size_t workspace_bytes,
+                                b200kge_stream_t stream) {
+  int rc = validate_ns_dropout(model, l_norm, ent, rel, triples, slot, neg, n, K, impl, drop); if (rc) return rc;
+  if (n == 0) return 0;
+  if (!grad_scores || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (ldg < K + 1) { set_error("grad_scores is narrower than the 1 + K columns of the block"); return B200KGE_ERR_INVALID; }
+  if (lde < ent->dim || ldr < rel->dim) { set_error("gradient leading dimensions are smaller than the table widths"); return B200KGE_ERR_INVALID; }
+  return launch_ns_dropout(model, l_norm, to_rows(ent), to_rows(rel), triples, slot, neg, n, K, impl, ns_drop_keys(*drop),
+                           grad_scores, ldg, nullptr, 0, d_ent, lde, d_rel, ldr, workspace, workspace_bytes,
+                           (cudaStream_t)stream);
+}
+
+}  // extern "C"

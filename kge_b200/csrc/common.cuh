@@ -380,4 +380,32 @@ int launch_dropout_scatter(const DropMask& m, const float* src, int64_t lds, int
 // tri[3 i + j] = i: the triples under which the row-wise unfold writes row i's gradient into row i of [n, D] buffers
 int launch_identity_triples(int64_t n, int64_t* tri, cudaStream_t st);
 
+// ns_kernel with dropout on the `batch` negatives (rowwise.cu): the fixed rows of triples [n, 3] (entity, draw ma;
+// relation, draw mp) masked at mask row row_base + i, each sampled row by its entity id (draw mt); scores into
+// out[i * ldo + col0 + k].  ent / rel are the plain tables.
+int launch_ns_masked(int model, float l_norm, const Rows& ent, const Rows& rel, const int64_t* triples, int slot,
+                     const int64_t* neg, int64_t n, int64_t K, const DropMask& ma, const DropMask& mp, const DropMask& mt,
+                     float* out, int64_t ldo, int col0, cudaStream_t st);
+// ns_backward_kernel with the same masks (grad.cu): a and p are [n, D] / [n, Dr] masked copies of the fixed rows (plain
+// rows, row i of the sub-batch), so the fold and the unfold run unchanged and the row gradients land in dA / dP
+// (OVERWRITTEN); the sampled rows' gradients are masked and scattered into d_ent.  Columns 1..K of G only.
+int launch_ns_backward_masked(int model, float l_norm, const Rows& a, const Rows& p, const Rows& table, int slot,
+                              const int64_t* neg, int64_t n, int64_t K, const DropMask& mt, const float* G, int64_t ldg,
+                              float* d_ent, int64_t lde, float* dQ, int64_t ldq, int64_t* tri_ws, float* dA, float* dP,
+                              cudaStream_t st);
+// Dropout of one negative-sampling slot (ns_dropout.cu): the entity and relation draws' key and rate (stream and
+// row_base are set per draw) and the sub-batch's first global row.
+struct NsDropKeys {
+  DropMask ent, rel;
+  int64_t row_base;
+};
+// G == NULL: scores of the [n, 1+K] block into out (positive in column 0); else the backward of that block with
+// grad_scores G, ADDED into d_ent / d_rel.  impl: B200KGE_NS_TRIPLE | B200KGE_NS_BATCH.
+// workspace: ns_dropout_workspace_bytes (the backward of the `batch` negatives only; the rest needs none)
+size_t ns_dropout_workspace_bytes(int model, int64_t n, int32_t D);
+int launch_ns_dropout(int model, float l_norm, const Rows& ent, const Rows& rel, const int64_t* triples, int slot,
+                      const int64_t* neg, int64_t n, int64_t K, int impl, const NsDropKeys& keys, const float* G,
+                      int64_t ldg, float* out, int64_t ldo, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
+                      void* workspace, size_t workspace_bytes, cudaStream_t st);
+
 }  // namespace b200kge

@@ -15,6 +15,7 @@
 // transposed through HBM).  Both GEMMs run split-K (512-element segments added in fp32, pairwise_tc.cu): the
 // tensor core's fp32 accumulator error grows with the reduction length, and dQ = G T reduces over all E entities.
 #include <cuda_fp16.h>
+#include "dropmask.cuh"
 #include "fold.cuh"
 #include "tc_common.cuh"
 
@@ -386,16 +387,20 @@ normalize_rows_kernel(float* __restrict__ w, int64_t ld, int64_t rows, int dim, 
 // G = dL/dz * scale from ns_loss_kernel) g = G[i, c] replaces the BCE formula; the rest is unchanged.
 constexpr int NSB_WARPS = 4, NSB_PER_BLOCK = 64, NSB_MAXK = 1024;   // lane-local dq: K / 32 <= 32 registers
 
-template <int MODEL>
-__global__ void __launch_bounds__(NSB_WARPS * 32)
-ns_backward_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int sp, const int64_t* __restrict__ neg,
-                   int64_t Kneg, Folded f, float l_norm, float offset, float inv_batch, const float* __restrict__ G,
-                   int64_t ldg, float* __restrict__ d_ent, int64_t lde, float* __restrict__ dQ, int64_t ldq) {
+// MASK (ns_backward_kernel_masked, the `batch` negatives with dropout): `fa` / `rel` hold masked copies of the fixed rows
+// under identity triples, column 0 (the positive, drawn on other streams) is skipped, and every sampled row is masked
+// by its entity id (draw tm) where it is loaded and where its gradient is scattered.
+template <int MODEL, bool MASK>
+__device__ __forceinline__ void ns_backward_body(const Rows& fa, const Rows& ent, const Rows& rel, const int64_t* __restrict__ tri,
+                                                 int sp, const int64_t* __restrict__ neg, int64_t Kneg, const Folded& f,
+                                                 float l_norm, float offset, float inv_batch, const float* __restrict__ G,
+                                                 int64_t ldg, float* __restrict__ d_ent, int64_t lde, float* __restrict__ dQ,
+                                                 int64_t ldq, const DropMask& tm) {
   extern __shared__ __align__(16) float sh[];  // q[K] | dq[K] (+ entity row for RESCAL)
   const int64_t i = blockIdx.x;
   const int64_t si = tri[3 * i], pi = tri[3 * i + 1], oi = tri[3 * i + 2];
   const int D = ent.dim, h = D >> 1, K = f.K;
-  const float* __restrict__ a = ent.base + (sp ? si : oi) * ent.ld;
+  const float* __restrict__ a = fa.base + (sp ? si : oi) * fa.ld;
   const float* __restrict__ p = rel.base + pi * rel.ld;
   float* q = sh;
   float* sdq = sh + K;
@@ -417,21 +422,33 @@ ns_backward_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int sp, 
 #pragma unroll
   for (int j = 0; j < NSB_MAXK / 32; ++j) dq[j] = 0.f;
   for (int64_t c = c0 + warp; c < c0 + NSB_PER_BLOCK && c <= Kneg; c += NSB_WARPS) {
+    if constexpr (MASK) { if (c == 0) continue; }
     // column 0 is the positive triple (its open slot holds the true entity), columns 1..K the samples
     const int64_t e = (c == 0) ? (sp ? oi : si) : neg[i * Kneg + (c - 1)];
     const float y = (c == 0) ? 1.f : 0.f;
     const float* __restrict__ t = ent.base + e * ent.ld + f.col_off;
     float* __restrict__ dt = d_ent + e * lde + f.col_off;
+    // T(k): element k of the sampled row, DT_ADD(k, v): its gradient — through the entity's mask under MASK
+#define T(k) (MASK ? t[k] * drop_mask1(tm, (uint64_t)e, D, f.col_off + (k)) : t[k])
+#define DT_ADD(k, v)                                                                   \
+    do {                                                                               \
+      if constexpr (MASK) {                                                            \
+        const float m_ = drop_mask1(tm, (uint64_t)e, D, f.col_off + (k));              \
+        if (m_ != 0.f) atomicAdd(dt + (k), (v) * m_);                                  \
+      } else {                                                                         \
+        atomicAdd(dt + (k), (v));                                                      \
+      }                                                                                \
+    } while (0)
     float acc = 0.f;
     if (f.pair_op == PAIR_DOT) {
-      for (int k = lane; k < K; k += 32) acc = fmaf(q[k], t[k], acc);
+      for (int k = lane; k < K; k += 32) acc = fmaf(q[k], T(k), acc);
     } else if (f.pair_op == PAIR_L1) {
-      for (int k = lane; k < K; k += 32) acc += fabsf(q[k] - t[k]);
+      for (int k = lane; k < K; k += 32) acc += fabsf(q[k] - T(k));
     } else if (f.pair_op == PAIR_L2) {
-      for (int k = lane; k < K; k += 32) { const float d = q[k] - t[k]; acc = fmaf(d, d, acc); }
+      for (int k = lane; k < K; k += 32) { const float d = q[k] - T(k); acc = fmaf(d, d, acc); }
     } else {   // PAIR_CMOD_L1
       for (int k = lane; k < hk; k += 32) {
-        const float d_re = q[k] - t[k], d_im = q[k + hk] - t[k + hk];
+        const float d_re = q[k] - T(k), d_im = q[k + hk] - T(k + hk);
         acc += sqrtf(fmaf(d_im, d_im, d_re * d_re));
       }
     }
@@ -443,36 +460,38 @@ ns_backward_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int sp, 
     const float g = G ? G[i * ldg + c] : (1.0f / (1.0f + expf(-(z + offset))) - y) * inv_batch;
     if (f.pair_op == PAIR_DOT) {
       for (int k = lane, j = 0; k < K; k += 32, ++j) {
-        dq[j] = fmaf(g, t[k], dq[j]);
-        atomicAdd(dt + k, g * q[k]);
+        dq[j] = fmaf(g, T(k), dq[j]);
+        DT_ADD(k, g * q[k]);
       }
     } else if (f.pair_op == PAIR_L1) {          // z = -sum |q - t|
       for (int k = lane, j = 0; k < K; k += 32, ++j) {
-        const float d = q[k] - t[k];
+        const float d = q[k] - T(k);
         const float w = (d > 0.f) ? -g : (d < 0.f ? g : 0.f);
         dq[j] += w;
-        atomicAdd(dt + k, -w);
+        DT_ADD(k, -w);
       }
     } else if (f.pair_op == PAIR_L2) {          // z = -||q - t||_2
       const float inv = (nrm > 0.f) ? g / nrm : 0.f;
       for (int k = lane, j = 0; k < K; k += 32, ++j) {
-        const float w = -(q[k] - t[k]) * inv;
+        const float w = -(q[k] - T(k)) * inv;
         dq[j] += w;
-        atomicAdd(dt + k, -w);
+        DT_ADD(k, -w);
       }
     } else {                                     // z = -sum_k |q_k - t_k| (complex modulus)
       for (int k = lane, j = 0; k < hk; k += 32, j += 2) {
-        const float d_re = q[k] - t[k], d_im = q[k + hk] - t[k + hk];
+        const float d_re = q[k] - T(k), d_im = q[k + hk] - T(k + hk);
         const float m = sqrtf(fmaf(d_im, d_im, d_re * d_re));
         const float inv = (m > 0.f) ? g / m : 0.f;
         const float w_re = -d_re * inv, w_im = -d_im * inv;
         dq[j] += w_re;
         dq[j + 1] += w_im;
-        atomicAdd(dt + k, -w_re);
-        atomicAdd(dt + k + hk, -w_im);
+        DT_ADD(k, -w_re);
+        DT_ADD(k + hk, -w_im);
       }
     }
   }
+#undef T
+#undef DT_ADD
   // block-level dq: lanes own disjoint columns, warps add up through shared memory
   if (f.pair_op == PAIR_CMOD_L1) {
     for (int k = lane, j = 0; k < hk; k += 32, j += 2) { atomicAdd(sdq + k, dq[j]); atomicAdd(sdq + k + hk, dq[j + 1]); }
@@ -481,6 +500,24 @@ ns_backward_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int sp, 
   }
   __syncthreads();
   for (int k = threadIdx.x; k < K; k += blockDim.x) atomicAdd(dQ + i * ldq + k, sdq[k]);
+}
+
+template <int MODEL>
+__global__ void __launch_bounds__(NSB_WARPS * 32)
+ns_backward_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int sp, const int64_t* __restrict__ neg,
+                   int64_t Kneg, Folded f, float l_norm, float offset, float inv_batch, const float* __restrict__ G,
+                   int64_t ldg, float* __restrict__ d_ent, int64_t lde, float* __restrict__ dQ, int64_t ldq) {
+  ns_backward_body<MODEL, false>(ent, ent, rel, tri, sp, neg, Kneg, f, l_norm, offset, inv_batch, G, ldg, d_ent, lde, dQ,
+                                 ldq, DropMask{});
+}
+
+template <int MODEL>
+__global__ void __launch_bounds__(NSB_WARPS * 32)
+ns_backward_kernel_masked(Rows fa, Rows ent, Rows rel, const int64_t* __restrict__ tri, int sp,
+                          const int64_t* __restrict__ neg, int64_t Kneg, Folded f, float l_norm,
+                          const float* __restrict__ G, int64_t ldg, float* __restrict__ d_ent, int64_t lde,
+                          float* __restrict__ dQ, int64_t ldq, DropMask tm) {
+  ns_backward_body<MODEL, true>(fa, ent, rel, tri, sp, neg, Kneg, f, l_norm, 0.f, 1.f, G, ldg, d_ent, lde, dQ, ldq, tm);
 }
 
 // unfold for the distance family (TransE: Q = a +- p; RotatE: rotation) — appended to the dot-family unfold
@@ -561,6 +598,44 @@ int launch_ns_backward(int model, float l_norm, const Rows& ent, const Rows& rel
     return 0;
   }
   return launch_unfold(model, ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, st);
+}
+
+int launch_ns_backward_masked(int model, float l_norm, const Rows& a, const Rows& p, const Rows& table, int slot,
+                              const int64_t* neg, int64_t n, int64_t K, const DropMask& mt, const float* G, int64_t ldg,
+                              float* d_ent, int64_t lde, float* dQ, int64_t ldq, int64_t* tri_ws, float* dA, float* dP,
+                              cudaStream_t st) {
+  if (n == 0) return 0;
+  if (slot != 0 && slot != 2) { set_error("the masked negative-sampling backward covers the S and O slots"); return B200KGE_ERR_UNSUPPORTED; }
+  const int sp = (slot == 2) ? 1 : 0;
+  Folded f = folded_problem(model, sp ? B200KGE_SP_ : B200KGE__PO, table.dim, l_norm);
+  if (model == B200KGE_RESCAL || f.pair_op == PAIR_LP || f.pair_op == PAIR_CMOD_LP || f.K > NSB_MAXK) {
+    set_error("the masked negative-sampling backward covers the non-RESCAL models with l_norm 1 / 2 and K <= %d", NSB_MAXK);
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  int rc;
+  if ((rc = launch_identity_triples(n, tri_ws, st))) return rc;
+  B2K_CUDA(cudaMemsetAsync(dQ, 0, (size_t)n * ldq * 4, st));
+  B2K_CUDA(cudaMemsetAsync(dA, 0, (size_t)n * a.dim * 4, st));
+  B2K_CUDA(cudaMemsetAsync(dP, 0, (size_t)n * p.dim * 4, st));
+  if (K > 0) {
+    const size_t smem = (size_t)2 * f.K * sizeof(float);
+    const int64_t by = (K + 1 + NSB_PER_BLOCK - 1) / NSB_PER_BLOCK;
+    if (by > 65535) { set_error("too many negatives per row (%lld)", (long long)K); return B200KGE_ERR_UNSUPPORTED; }
+    dim3 grid((unsigned)n, (unsigned)by), block(NSB_WARPS * 32);
+#define B2K_NSBM(M) case M: ns_backward_kernel_masked<M><<<grid, block, smem, st>>>(a, table, p, tri_ws, sp, neg, K, f, l_norm, G, ldg, d_ent, lde, dQ, ldq, mt); break;
+    switch (model) {
+      B2K_NSBM(B200KGE_COMPLEX) B2K_NSBM(B200KGE_DISTMULT) B2K_NSBM(B200KGE_SIMPLE) B2K_NSBM(B200KGE_CP)
+      B2K_NSBM(B200KGE_TRANSE) B2K_NSBM(B200KGE_ROTATE)
+      default: set_error("unknown model %d", model); return B200KGE_ERR_INVALID;
+    }
+#undef B2K_NSBM
+    B2K_LAUNCH_CHECK("ns_backward_kernel_masked");
+  }
+  // the row gradients of the masked copies: the unfold on identity triples writes row i's into row i of dA / dP
+  const int dir = sp ? 0 : 1;
+  if (model == B200KGE_TRANSE || model == B200KGE_ROTATE)
+    return launch_unfold_distance(model, a, p, tri_ws, n, dir, dQ, ldq, dA, a.dim, dP, p.dim, st);
+  return launch_unfold(model, a, p, tri_ws, n, dir, dQ, ldq, dA, a.dim, dP, p.dim, st);
 }
 
 int launch_unfold_distance(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n, int dir,

@@ -9,8 +9,8 @@
 //    rows and reduces pair(q, row) — the gather of the sampled indexes is fused with the
 //    per-negative dot/distance; nothing of size [n*K, D] is materialised (the reference's `triple`
 //    implementation gathers 3 x [n*K, D]).  The P slot goes through spo_kernel with row divisors.
+#include "dropmask.cuh"
 #include "fold.cuh"
-#include "philox.cuh"
 
 namespace b200kge {
 
@@ -120,13 +120,25 @@ __device__ __forceinline__ float sqrt_approx(float x) {
 
 // pair(q, t) partial sum of one lane over a row, 16-byte loads: lane handles float4 groups lane, lane + 32, ...
 // (complex pair ops: the re group at k4 pairs with the im group at k4 + hk/4)
-template <int PAIR>
-__device__ __forceinline__ float ns_row_partial(const float4* __restrict__ q4, const float4* __restrict__ t4, int n4, int lane) {
+// MASK: the sampled row is entity `e` of a dropout draw `tm` over rows of width `tw`, its group k starting at column
+// col_off + 4 k (the `batch` negatives of b200kge_ns_score_dropout: one mask per entity id)
+__device__ __forceinline__ float4 ns_masked(float4 t, const DropMask& tm, int64_t e, int tw, int col) {
+  float mk[4];
+  drop_mask4(tm, (uint64_t)e, tw, col, mk);
+  t.x *= mk[0]; t.y *= mk[1]; t.z *= mk[2]; t.w *= mk[3];
+  return t;
+}
+
+template <int PAIR, bool MASK = false>
+__device__ __forceinline__ float ns_row_partial(const float4* __restrict__ q4, const float4* __restrict__ t4, int n4, int lane,
+                                                const DropMask& tm = DropMask{}, int64_t e = 0, int tw = 0, int col_off = 0) {
   float acc = 0.f;
   if constexpr (PAIR == PAIR_CMOD_L1) {
     const int h4 = n4 >> 1;
     for (int k = lane; k < h4; k += 32) {
-      const float4 tr = __ldg(t4 + k), ti = __ldg(t4 + k + h4), qr = q4[k], qi = q4[k + h4];
+      float4 tr = __ldg(t4 + k), ti = __ldg(t4 + k + h4);
+      if constexpr (MASK) { tr = ns_masked(tr, tm, e, tw, col_off + 4 * k); ti = ns_masked(ti, tm, e, tw, col_off + 4 * (k + h4)); }
+      const float4 qr = q4[k], qi = q4[k + h4];
       float dr, di;
       dr = qr.x - tr.x; di = qi.x - ti.x; acc += sqrt_approx(fmaf(di, di, dr * dr));
       dr = qr.y - tr.y; di = qi.y - ti.y; acc += sqrt_approx(fmaf(di, di, dr * dr));
@@ -135,7 +147,9 @@ __device__ __forceinline__ float ns_row_partial(const float4* __restrict__ q4, c
     }
   } else {
     for (int k = lane; k < n4; k += 32) {
-      const float4 t = __ldg(t4 + k), q = q4[k];
+      float4 t = __ldg(t4 + k);
+      if constexpr (MASK) t = ns_masked(t, tm, e, tw, col_off + 4 * k);
+      const float4 q = q4[k];
       if constexpr (PAIR == PAIR_DOT) {
         acc = fmaf(q.x, t.x, acc); acc = fmaf(q.y, t.y, acc); acc = fmaf(q.z, t.z, acc); acc = fmaf(q.w, t.w, acc);
       } else if constexpr (PAIR == PAIR_L1) {
@@ -151,9 +165,10 @@ __device__ __forceinline__ float ns_row_partial(const float4* __restrict__ q4, c
 }
 
 // the warp's rows kk, kk + NS_WARPS, ... of this CTA's range, TWO at a time (both rows' loads are in flight together)
-template <int PAIR>
+template <int PAIR, bool MASK = false>
 __device__ __forceinline__ void ns_rows_vec(const float* q, const Rows& table, int col_off, int K, const int64_t* __restrict__ neg_row,
-                                            int64_t k0, int64_t kend, int warp, int lane, float* __restrict__ out_row) {
+                                            int64_t k0, int64_t kend, int warp, int lane, float* __restrict__ out_row,
+                                            const DropMask& tm = DropMask{}) {
   const float4* q4 = reinterpret_cast<const float4*>(q);
   const int n4 = K >> 2;
   for (int64_t kk = k0 + warp; kk < kend; kk += 2 * NS_WARPS) {
@@ -162,8 +177,8 @@ __device__ __forceinline__ void ns_rows_vec(const float* q, const Rows& table, i
     const int64_t e0 = __ldg(neg_row + kk), e1 = two ? __ldg(neg_row + kb) : e0;
     const float4* t0 = reinterpret_cast<const float4*>(table.base + e0 * table.ld + col_off);
     const float4* t1 = reinterpret_cast<const float4*>(table.base + e1 * table.ld + col_off);
-    float a0 = ns_row_partial<PAIR>(q4, t0, n4, lane);
-    float a1 = two ? ns_row_partial<PAIR>(q4, t1, n4, lane) : 0.f;
+    float a0 = ns_row_partial<PAIR, MASK>(q4, t0, n4, lane, tm, e0, table.dim, col_off);
+    float a1 = two ? ns_row_partial<PAIR, MASK>(q4, t1, n4, lane, tm, e1, table.dim, col_off) : 0.f;
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) {
       a0 += __shfl_xor_sync(0xffffffffu, a0, off);
@@ -178,16 +193,41 @@ __device__ __forceinline__ void ns_rows_vec(const float* q, const Rows& table, i
   }
 }
 
-template <int MODEL>
-__global__ void __launch_bounds__(NS_WARPS * 32)
-ns_kernel(Rows A, Rows Pr, Rows table, int sp, const int64_t* __restrict__ neg, int64_t Kneg,
-          Folded f, float l_norm, float* __restrict__ out, int64_t ldo, int col0, int vec_ok) {
-  extern __shared__ __align__(16) float sh[];  // q[K] (+ entity row for RESCAL)
+// Dropout of the `batch` negatives (ns_kernel_masked): the fixed entity row (draw `a`, mask row a.row_base + i) and the
+// relation row (draw `p`) are masked once per row before the fold, every sampled row by its entity id (draw `t`).
+struct NsRowMasks {
+  DropMask a, p, t;
+};
+
+template <int MODEL, bool MASK>
+__device__ __forceinline__ void ns_body(const Rows& A, const Rows& Pr, const Rows& table, int sp, const int64_t* __restrict__ neg,
+                                        int64_t Kneg, const Folded& f, float l_norm, float* __restrict__ out, int64_t ldo,
+                                        int col0, int vec_ok, const NsRowMasks& mk, const int64_t* __restrict__ tri = nullptr,
+                                        int ca = 0) {
+  extern __shared__ __align__(16) float sh[];  // q[K] (+ entity row for RESCAL) (MASK: + masked entity and relation rows)
   const int64_t i = blockIdx.x;
   const int D = A.dim, h = D >> 1, K = f.K;
   const float* __restrict__ a = A.row(i);
   const float* __restrict__ p = Pr.row(i);
   float* q = sh;
+  if constexpr (MASK) {       // the fold reads masked copies in shared memory (D, Dr multiples of 4)
+    a = A.base + tri[3 * i + ca] * A.ld;      // the fixed rows of triple i: entity column ca, relation column 1
+    p = Pr.base + tri[3 * i + 1] * Pr.ld;
+    float* sa = sh + ((K + 3) & ~3);
+    float* spr = sa + D;
+    for (int g = 4 * threadIdx.x; g < D + Pr.dim; g += 4 * blockDim.x) {
+      const bool ent = g < D;
+      const int k = ent ? g : g - D;
+      float m4[4];
+      drop_mask4(ent ? mk.a : mk.p, (uint64_t)((ent ? mk.a.row_base : mk.p.row_base) + i), ent ? D : Pr.dim, k, m4);
+      const float* src = ent ? a : p;
+      float* dst = ent ? sa : spr;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) dst[k + j] = src[k + j] * m4[j];
+    }
+    __syncthreads();
+    a = sa; p = spr;
+  }
   if constexpr (MODEL == B200KGE_RESCAL) {
     float* sa = sh + ((K + 3) & ~3);
     for (int k = threadIdx.x; k < D; k += blockDim.x) sa[k] = a[k];
@@ -206,13 +246,14 @@ ns_kernel(Rows A, Rows Pr, Rows table, int sp, const int64_t* __restrict__ neg, 
   if (vec_ok) {
     // 16-byte loads, two rows in flight per warp (the scalar form below gathered at 3.4 TB/s from an L2-resident table)
     switch (f.pair_op) {
-      case PAIR_DOT:     ns_rows_vec<PAIR_DOT>(q, table, f.col_off, K, neg_row, k0, kend, warp, lane, out_row); return;
-      case PAIR_L1:      ns_rows_vec<PAIR_L1>(q, table, f.col_off, K, neg_row, k0, kend, warp, lane, out_row); return;
-      case PAIR_L2:      ns_rows_vec<PAIR_L2>(q, table, f.col_off, K, neg_row, k0, kend, warp, lane, out_row); return;
-      case PAIR_CMOD_L1: ns_rows_vec<PAIR_CMOD_L1>(q, table, f.col_off, K, neg_row, k0, kend, warp, lane, out_row); return;
+      case PAIR_DOT:     ns_rows_vec<PAIR_DOT, MASK>(q, table, f.col_off, K, neg_row, k0, kend, warp, lane, out_row, mk.t); return;
+      case PAIR_L1:      ns_rows_vec<PAIR_L1, MASK>(q, table, f.col_off, K, neg_row, k0, kend, warp, lane, out_row, mk.t); return;
+      case PAIR_L2:      ns_rows_vec<PAIR_L2, MASK>(q, table, f.col_off, K, neg_row, k0, kend, warp, lane, out_row, mk.t); return;
+      case PAIR_CMOD_L1: ns_rows_vec<PAIR_CMOD_L1, MASK>(q, table, f.col_off, K, neg_row, k0, kend, warp, lane, out_row, mk.t); return;
       default: break;
     }
   }
+  if constexpr (MASK) return;          // the masked launch requires the vector path (checked by launch_ns_masked)
   const int hk = K >> 1;
   for (int64_t kk = k0 + warp; kk < kend; kk += NS_WARPS) {
     const int64_t e = neg_row[kk];
@@ -241,6 +282,20 @@ ns_kernel(Rows A, Rows Pr, Rows table, int sp, const int64_t* __restrict__ neg, 
       out_row[kk] = acc;
     }
   }
+}
+
+template <int MODEL>
+__global__ void __launch_bounds__(NS_WARPS * 32)
+ns_kernel(Rows A, Rows Pr, Rows table, int sp, const int64_t* __restrict__ neg, int64_t Kneg,
+          Folded f, float l_norm, float* __restrict__ out, int64_t ldo, int col0, int vec_ok) {
+  ns_body<MODEL, false>(A, Pr, table, sp, neg, Kneg, f, l_norm, out, ldo, col0, vec_ok, NsRowMasks{});
+}
+
+template <int MODEL>
+__global__ void __launch_bounds__(NS_WARPS * 32)
+ns_kernel_masked(Rows A, Rows Pr, Rows table, const int64_t* __restrict__ tri, int sp, const int64_t* __restrict__ neg,
+                 int64_t Kneg, Folded f, float l_norm, float* __restrict__ out, int64_t ldo, int col0, NsRowMasks mk) {
+  ns_body<MODEL, true>(A, Pr, table, sp, neg, Kneg, f, l_norm, out, ldo, col0, 1, mk, tri, sp ? 0 : 2);
 }
 
 }  // namespace
@@ -282,6 +337,40 @@ int launch_ns(int model, float l_norm, const Rows& s, const Rows& p, const Rows&
   }
 #undef B2K_NS
   B2K_LAUNCH_CHECK("ns_kernel");
+  return 0;
+}
+
+// The `batch` negatives of one slot with dropout (b200kge_ns_score_dropout): ns_kernel's gather + pair reduction with the
+// fixed rows of triple i (the slot's other entity and the relation) masked once per row and each sampled row masked by
+// its id.  Not for
+// RESCAL, whose D x D relation row does not fit the shared-memory copy.
+int launch_ns_masked(int model, float l_norm, const Rows& ent, const Rows& rel, const int64_t* triples, int slot,
+                     const int64_t* neg, int64_t n, int64_t K, const DropMask& ma, const DropMask& mp, const DropMask& mt,
+                     float* out, int64_t ldo, int col0, cudaStream_t st) {
+  const Rows& a = ent; const Rows& p = rel; const Rows& table = ent;
+  if (n == 0 || K == 0) return 0;
+  const int sp = (slot == 2) ? 1 : 0;
+  Folded f = folded_problem(model, sp ? B200KGE_SP_ : B200KGE__PO, a.dim, l_norm);
+  const bool cm = (f.pair_op == PAIR_CMOD_L1 || f.pair_op == PAIR_CMOD_LP);
+  if (model == B200KGE_RESCAL || f.pair_op == PAIR_LP || f.pair_op == PAIR_CMOD_LP || a.dim % 4 || p.dim % 4 ||
+      table.ld % 4 || f.col_off % 4 || f.K % (cm ? 8 : 4) || (reinterpret_cast<uintptr_t>(table.base) & 15)) {
+    set_error("the masked negative-sample kernel needs a 16-byte aligned table, widths that are multiples of 4 and a "
+              "non-RESCAL model with l_norm 1 / 2");
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  const size_t smem = (size_t)(((f.K + 3) & ~3) + a.dim + p.dim) * sizeof(float);
+  const int64_t by = (K + NS_PER_BLOCK - 1) / NS_PER_BLOCK;
+  if (by > 65535) { set_error("too many negatives per row (%lld)", (long long)K); return B200KGE_ERR_UNSUPPORTED; }
+  dim3 grid((unsigned)n, (unsigned)by), block(NS_WARPS * 32);
+  NsRowMasks mk{ma, mp, mt};
+#define B2K_NSM(M) case M: ns_kernel_masked<M><<<grid, block, smem, st>>>(a, p, table, triples, sp, neg, K, f, l_norm, out, ldo, col0, mk); break;
+  switch (model) {
+    B2K_NSM(B200KGE_COMPLEX) B2K_NSM(B200KGE_DISTMULT) B2K_NSM(B200KGE_SIMPLE) B2K_NSM(B200KGE_CP)
+    B2K_NSM(B200KGE_TRANSE) B2K_NSM(B200KGE_ROTATE)
+    default: set_error("unknown model %d", model); return B200KGE_ERR_INVALID;
+  }
+#undef B2K_NSM
+  B2K_LAUNCH_CHECK("ns_kernel_masked");
   return 0;
 }
 

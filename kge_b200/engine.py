@@ -11,7 +11,7 @@ from typing import NamedTuple, Optional
 import torch
 
 from . import _lib
-from ._lib import LOSS, MODELS, PREC, Dropout, Labels, Rows, SP_, _PO
+from ._lib import LOSS, MODELS, NS_IMPL, PREC, Dropout, Labels, Rows, SP_, _PO
 
 S, P, O = 0, 1, 2
 
@@ -384,10 +384,27 @@ def rank_dense(scores, true_scores, filter_labels=None, rtol: float = 1e-4, atol
 
 
 def ns_score(model: str, ent, rel, triples, negatives, slot: int, with_positive: bool = False,
-             l_norm: float = 1.0):
-    """[n, K] (or [n, 1+K] with the positive in column 0) negative-sample scores."""
+             l_norm: float = 1.0, dropout: Optional["DropoutKey"] = None, implementation: str = "batch"):
+    """[n, K] (or [n, 1+K] with the positive in column 0) negative-sample scores.
+
+    With `dropout` (an engine.DropoutKey) the slot's six embedding-dropout draws are applied
+    (b200kge_ns_score_dropout): `implementation` ("triple", "batch" or "all") selects how the negatives' masks are
+    drawn, as the reference's negative_sampling.implementation does; the block always has the positive in column 0."""
     _require_cuda(ent, rel, triples, negatives)
     lib, k = _lib.load(), _Keep()
+    if dropout is not None:
+        if not with_positive:
+            raise ValueError("ns_score with dropout returns the [n, 1+K] block (with_positive=True)")
+        re_, rr = k.rows(ent), k.rows(rel)
+        tri = triples if (triples.dtype == torch.int64 and triples.is_contiguous()) else triples.long().contiguous()
+        neg = negatives if (negatives.dtype == torch.int64 and negatives.is_contiguous()) else negatives.long().contiguous()
+        n, K = neg.shape
+        out = torch.empty((n, K + 1), dtype=torch.float32, device=ent.device)
+        _lib.check(lib.b200kge_ns_score_dropout(MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(),
+                                                int(slot), neg.data_ptr(), n, K, NS_IMPL[implementation],
+                                                C.byref(dropout.struct()), out.data_ptr(), out.stride(0),
+                                                _stream(ent.device)))
+        return out
     tri = triples.long()
     rs, rp, ro = k.rows(ent, tri[:, S].contiguous()), k.rows(rel, tri[:, P].contiguous()), \
         k.rows(ent, tri[:, O].contiguous())
@@ -659,12 +676,16 @@ def normalize_rows_(weight: torch.Tensor, p: float) -> torch.Tensor:
 
 
 def ns_backward(model: str, ent, rel, triples, negatives: dict, offset: float = 0.0, l_norm: float = 1.0,
-                  batch_size: Optional[int] = None, grad_scores: Optional[dict] = None):
+                  batch_size: Optional[int] = None, grad_scores: Optional[dict] = None,
+                  dropout: Optional["DropoutKey"] = None, implementation: str = "batch"):
     """(d_ent, d_rel) of one negative-sampling batch; negatives = {slot: [n, K] ids}, slots 0 (S), 2 (O).
 
     Without grad_scores the loss is BCE with `offset`, divided by batch_size.  With grad_scores = {slot: G}, G [n, 1+K]
     (positive first) is dL/dscores of each slot's block already scaled — e.g. the G of ns_loss(..., want_grad=True) —
-    and `offset` / `batch_size` are not used: any loss of ns_loss trains through the same kernel."""
+    and `offset` / `batch_size` are not used: any loss of ns_loss trains through the same kernel.
+
+    With `dropout` (the forward's engine.DropoutKey and `implementation`) the gradients go through the forward's masks
+    (b200kge_ns_backward_dropout); grad_scores is then required."""
     _require_cuda(ent, rel, triples)
     lib, k = _lib.load(), _Keep()
     re_, rr = k.rows(ent), k.rows(rel)
@@ -673,9 +694,28 @@ def ns_backward(model: str, ent, rel, triples, negatives: dict, offset: float = 
     dev = ent.device
     d_ent = torch.zeros_like(_f32(ent))
     d_rel = torch.zeros_like(_f32(rel))
-    ws = torch.empty(n * (ent.shape[1] + 32) * 4 + 1024, dtype=torch.uint8, device=dev)
+    if dropout is not None and grad_scores is None:
+        raise ValueError("ns_backward with dropout needs grad_scores (e.g. the G of ns_loss(..., want_grad=True))")
+    if dropout is not None:
+        nbytes = lib.b200kge_ns_dropout_workspace_bytes(MODELS[model], n, 0, ent.shape[1])
+    else:
+        nbytes = n * (ent.shape[1] + 32) * 4 + 1024
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
     for slot, neg in negatives.items():
         ng = neg if (neg.dtype == torch.int64 and neg.is_contiguous()) else neg.long().contiguous()
+        if dropout is not None:
+            g = grad_scores[slot]
+            _require_cuda(g)
+            if g.shape != (n, ng.shape[1] + 1):
+                raise ValueError(f"grad_scores[{slot}] has shape {tuple(g.shape)}, expected {(n, ng.shape[1] + 1)}")
+            g = g if (g.dtype == torch.float32 and g.stride(1) == 1) else g.float().contiguous()
+            k.refs.append(g)
+            _lib.check(lib.b200kge_ns_backward_dropout(
+                MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), int(slot), ng.data_ptr(), n,
+                ng.shape[1], NS_IMPL[implementation], C.byref(dropout.struct()), g.data_ptr(), g.stride(0),
+                d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0), ws.data_ptr(), ws.numel(),
+                _stream(dev)))
+            continue
         if grad_scores is None:
             _lib.check(lib.b200kge_ns_backward(
                 MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), int(slot), ng.data_ptr(), n,

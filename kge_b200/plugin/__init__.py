@@ -19,7 +19,9 @@ The classes subclass the reference's `KgeModel` / `RelationalScorer` (kge_model.
    reference's embedders run and the scorer-level path takes over.
  * with embedding dropout active in training, the 1vsAll / KvsAll job plugins take the dropout entry points
    (`loss_1vsall` / `loss_kvsall*` with an engine.DropoutKey: masks drawn on the device with the distribution of the
-   reference's draws); the unmodified jobs' score_sp / score_po and score_sp_po keep the routes above.
+   reference's draws), and so does the negative-sampling job plugin with `user.b200_ns_dropout: true`
+   (`loss_negatives` / `score_negatives` with a key); the unmodified jobs' score_sp / score_po and score_sp_po keep the
+   routes above.
  * extra fused methods `score_sp_loss / score_po_loss / rank_sp / rank_po` for job plugins.
 
 CUDA only: CPU tensors raise (no fallback).  Backward (SURVEY 8f-1, "next") is provided by
@@ -243,12 +245,21 @@ class _NsSlotLossFn(torch.autograd.Function):
     """One slot of a negative-sampling batch: forward = fused gather+score [n, 1+K] and the loss kernel; backward = the
     fused NS gradient kernel (b200kge_ns_backward: per-row fold, per-column recompute, scatter).  BCE runs the dense-loss
     kernel and the kernel's own BCE gradient; every other loss runs the row-loss kernel (b200kge_ns_loss), which also
-    writes G = dL/dscores, and the backward reads G (b200kge_ns_backward_grad)."""
+    writes G = dL/dscores, and the backward reads G (b200kge_ns_backward_grad).  With a dropout key (engine.DropoutKey)
+    the forward scores the masked block (b200kge_ns_score_dropout, draws of `implementation`), every loss BCE included
+    runs the row-loss kernel, and the backward regenerates the same masks from the key (b200kge_ns_backward_dropout)."""
 
     @staticmethod
-    def forward(ctx, ent_w, rel_w, model, triples, negatives, slot, offset, batch_size, loss="bce", temperature=1.0):
-        ctx.args = (model, slot, offset, batch_size, loss)
+    def forward(ctx, ent_w, rel_w, model, triples, negatives, slot, offset, batch_size, loss="bce", temperature=1.0,
+                dropout=None, implementation="batch"):
+        ctx.args = (model, slot, offset, batch_size, loss, dropout, implementation)
         ln = model._b200_args()[0]
+        if dropout is not None:
+            scores = engine.ns_score(model._b200_name, ent_w.detach(), rel_w.detach(), triples, negatives, slot, True,
+                                     ln, dropout=dropout, implementation=implementation)
+            value, G = engine.ns_loss(scores, loss, offset, temperature, batch_size=batch_size, want_grad=True)
+            ctx.save_for_backward(ent_w, rel_w, triples, negatives, G)
+            return value
         scores = engine.ns_score(model._b200_name, ent_w.detach(), rel_w.detach(), triples, negatives, slot, True, ln)
         if loss == "bce":
             ctx.save_for_backward(ent_w, rel_w, triples, negatives)
@@ -260,12 +271,15 @@ class _NsSlotLossFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
-        model, slot, offset, batch_size, loss = ctx.args
+        model, slot, offset, batch_size, loss, dropout, implementation = ctx.args
         ent_w, rel_w, triples, negatives = ctx.saved_tensors[:4]
-        kw = {} if loss == "bce" else {"grad_scores": {slot: ctx.saved_tensors[4]}}
+        if dropout is not None:
+            kw = {"grad_scores": {slot: ctx.saved_tensors[4]}, "dropout": dropout, "implementation": implementation}
+        else:
+            kw = {} if loss == "bce" else {"grad_scores": {slot: ctx.saved_tensors[4]}}
         d_ent, d_rel = engine.ns_backward(model._b200_name, ent_w.detach(), rel_w.detach(), triples, {slot: negatives},
                                           offset, model._b200_args()[0], batch_size, **kw)
-        return (d_ent * g, d_rel * g) + (None,) * 8
+        return (d_ent * g, d_rel * g) + (None,) * 10
 
 
 class _B200ModelMixin:
@@ -491,11 +505,25 @@ class _B200ModelMixin:
                                    csr_offsets, csr_cols, loss, float(offset), float(label_smoothing), int(batch_size),
                                    dropout)
 
-    def score_negatives(self, triples, negatives, slot):
+    def score_negatives(self, triples, negatives, slot, dropout=None, implementation="batch"):
         """[n, 1+K]: the positive triple's score in column 0, its K corrupted versions after it
-        (train_negative_sampling.py:139-148 + sampler.py:263-344); forward only."""
+        (train_negative_sampling.py:139-148 + sampler.py:263-344); forward only.  `dropout` (an engine.DropoutKey)
+        applies the slot's embedding-dropout draws of `implementation` ("triple" | "batch" | "all")."""
         ent, rel = self._b200_tables()
-        return engine.ns_score(self._b200_name, ent, rel, triples, negatives, slot, True, self._b200_args()[0])
+        kw = {} if dropout is None else {"dropout": dropout, "implementation": implementation}
+        return engine.ns_score(self._b200_name, ent, rel, triples, negatives, slot, True, self._b200_args()[0], **kw)
+
+    def b200_ns_dropout_ok(self, slot):
+        """The negative-sampling dropout kernels cover the S / O slots of the dot family, TransE (L1, L2) and RotatE
+        (L1), with row widths the masks' four-element groups divide (D % 4 == 0, D % 8 == 0 for the models that split a
+        row into halves).  Like b200_ns_native_backward_ok, it needs b200_backward = "native"."""
+        if self.b200_backward != "native" or slot not in (0, 2):
+            return False
+        ln = self._b200_args()[0]
+        if not {"transe": ln in (1.0, 2.0), "rotate": ln == 1.0}.get(self._b200_name, True):
+            return False
+        D = self._b200_weights()[0].shape[1]
+        return D % (8 if self._b200_name in ("complex", "simple", "cp", "rotate") else 4) == 0
 
     def loss_dense(self, scores, labels, loss="bce", offset=0.0):
         return engine.loss_dense(scores, labels, loss, offset)
@@ -507,13 +535,16 @@ class _B200ModelMixin:
         ln = self._b200_args()[0]
         return {"transe": ln in (1.0, 2.0), "rotate": ln == 1.0}.get(self._b200_name, True)
 
-    def loss_negatives(self, triples, negatives, slot, offset, batch_size, loss="bce", temperature=1.0):
+    def loss_negatives(self, triples, negatives, slot, offset, batch_size, loss="bce", temperature=1.0, dropout=None,
+                       implementation="batch"):
         """KgeLoss of one slot's [n, 1+K] block (positive first) / batch_size, differentiable through the gradient
         kernel (train_negative_sampling.py:139-164).  `loss` is a name of engine.ns_loss; `offset` its argument (the BCE
-        offset, or the margin of margin_ranking), `temperature` that of bce_self_adversarial."""
+        offset, or the margin of margin_ranking), `temperature` that of bce_self_adversarial.  `dropout` (an
+        engine.DropoutKey) applies the slot's embedding-dropout draws of `implementation` in forward and backward."""
         ent_w, rel_w = self._b200_weights()
         return _NsSlotLossFn.apply(ent_w, rel_w, self, triples.long().contiguous(), negatives.long().contiguous(),
-                                   int(slot), float(offset), int(batch_size), loss, float(temperature))
+                                   int(slot), float(offset), int(batch_size), loss, float(temperature), dropout,
+                                   implementation)
 
     def loss_negatives_forward(self, scores, loss, arg=0.0, temperature=1.0):
         """Sum over rows of the KgeLoss of a scored [n, 1+K] block (positive first); forward only."""

@@ -14,8 +14,10 @@ Everything else of the job (data loading, collate, sub-batching, trace entries, 
 checkpoints) is the reference's code, unchanged.  Whenever a fused form is not available for the configured
 combination (a non-b200 model, a loss outside the fused set, ...) the method falls through to the reference
 implementation, which then still reaches the kernels through `model.score_*`.  Embedding dropout in training takes the
-dropout entry points in the 1vsAll and KvsAll jobs (masks drawn on the device, keyed per sub-batch); the
-negative-sampling job with dropout keeps the reference step.
+dropout entry points in the 1vsAll and KvsAll jobs (masks drawn on the device, keyed per sub-batch).  The
+negative-sampling job with dropout keeps the reference step unless `user.b200_ns_dropout: true` opts into the dropout
+kernels: the option chooses which random stream supplies the masks (the library's Philox key instead of torch's
+generator), as `user.b200_device_sampling` does for the negatives.
 """
 from __future__ import annotations
 
@@ -296,7 +298,7 @@ class B200TrainingJobKvsAll(_DropoutKeys, _BatchSplit, TrainingJobKvsAll):
             result.backward_time += time.time()
 
 
-class B200TrainingJobNegativeSampling(_BatchSplit, TrainingJobNegativeSampling):
+class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNegativeSampling):
     """`TrainingJobNegativeSampling` (train_negative_sampling.py:103-164): per slot ONE kernel gathers the sampled
     rows and scores them, with the positive triple in column 0 — neither `[n*K, D]` gathers (`triple`
     implementation, sampler.py:294-305) nor scoring against all unique targets (`batch`, :306-339).
@@ -338,6 +340,26 @@ class B200TrainingJobNegativeSampling(_BatchSplit, TrainingJobNegativeSampling):
         return engine.sample_uniform(n, int(sm.num_samples[slot]), int(sm.vocabulary_size[slot]),
                                      torch.initial_seed(), offset, self.device)
 
+    def _b200_ns_dropout_route(self, kind, slots):
+        """(b200 model, (p_ent, p_rel)) if `user.b200_ns_dropout` is on, embedding dropout is active and the dropout
+        kernels serve the configuration, else (None, None).  With device sampling an unserved configuration raises
+        (the reference step cannot consume device-drawn negatives)."""
+        model, rates = _dropout_model(self.model)
+        if model is None or not _user_option(self.config, "b200_ns_dropout", False):
+            return None, None
+        reason = None
+        if kind is None:
+            reason = f"the loss {type(self.loss).__name__} has no negative-sampling kernel"
+        elif any(sl == P for sl in slots):
+            reason = "the P slot is not served"
+        elif not all(model.b200_ns_dropout_ok(sl) for sl in slots):
+            reason = f"model {model._b200_name} with l_norm {model._b200_args()[0]} and this embedding width is not served"
+        if reason is None:
+            return model, rates
+        if self._device_sampling:
+            raise NotImplementedError(f"user.b200_ns_dropout with user.b200_device_sampling: {reason}")
+        return None, None
+
     def _process_subbatch(self, batch_index, batch, subbatch_slice, result):
         subbatch_slice = self._b200_my_rows(subbatch_slice, result.size)
         if subbatch_slice is None:
@@ -347,6 +369,16 @@ class B200TrainingJobNegativeSampling(_BatchSplit, TrainingJobNegativeSampling):
         slots = [sl for sl in (S, P, O) if self._sampler.num_samples[sl] > 0]
         trainable = (model is not None and kind is not None
                      and all(model.b200_ns_native_backward_ok(sl) for sl in slots))
+        drop = None
+        if model is None:
+            model, rates = self._b200_ns_dropout_route(kind, slots)
+            if model is not None:
+                # one key per sub-batch; the S and O slots draw disjoint mask streams under it
+                drop = self._b200_dropout_key(rates, batch_index, subbatch_slice)
+                trainable = True
+        # "all" draws the masks of "batch" (embed_all() gives the same distribution); `auto` is resolved by _prepare
+        impl = "triple" if getattr(self, "_implementation", "batch") == "triple" else "batch"
+        dkw = {} if drop is None else {"dropout": drop, "implementation": impl}
         if model is None or (not self.is_forward_only and not trainable):
             if self._device_sampling:
                 raise NotImplementedError("user.b200_device_sampling needs a b200_* model whose slots the fused "
@@ -379,14 +411,14 @@ class B200TrainingJobNegativeSampling(_BatchSplit, TrainingJobNegativeSampling):
             if not self.is_forward_only:
                 # training: forward + the fused NS gradient kernel behind one autograd node
                 loss_value = model.loss_negatives(triples, negatives.to(self.device), slot, kind[1], batch_size,
-                                                  kind[0], kind[2])
+                                                  kind[0], kind[2], **dkw)
                 result.avg_loss += loss_value.item()
                 result.forward_time += time.time()
                 result.backward_time -= time.time()
                 loss_value.backward()
                 result.backward_time += time.time()
                 continue
-            scores = model.score_negatives(triples, negatives.to(self.device), slot)      # [n, 1+K], positive first
+            scores = model.score_negatives(triples, negatives.to(self.device), slot, **dkw)  # [n, 1+K], positive first
             if kind is not None and kind[0] == "bce":
                 # labels are 1 in column 0 and 0 elsewhere (train_negative_sampling.py:128-137): index labels
                 lab = torch.zeros(subbatch_size, dtype=torch.int64, device=self.device)
