@@ -490,6 +490,49 @@ int b200kge_score_1vsN_loss_csr_backward_dropout(int model, int combine, const b
                                                  const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
                                                  int64_t ldr, void* workspace, size_t workspace_bytes,
                                                  b200kge_stream_t stream);
+/* The same with the draws picked apart from the fold: `combine` is the query type's fold, `mask_dir` (B200KGE_SP_ |
+ * B200KGE__PO) selects streams 0-2 | 3-5.  A reciprocal-relations model's _po query type is the sp_ fold of
+ * (q_idx = o, p_idx = p + R) on the _po streams (reciprocal_relations_model.py:85-92); the plain entry points above
+ * are these with mask_dir = combine.  Same workspace. */
+int b200kge_score_1vsN_loss_csr_dropout_dir(int model, int combine, int mask_dir, float l_norm, int precision,
+                                            const b200kge_rows_t* ent, const b200kge_rows_t* rel, const int64_t* q_idx,
+                                            const int64_t* p_idx, int64_t n, const int64_t* csr_off,
+                                            const int64_t* csr_col, int64_t nnz, float label_smoothing, int loss_kind,
+                                            float offset, const b200kge_dropout_t* drop, float* loss_out,
+                                            float* row_loss_out, void* workspace, size_t workspace_bytes,
+                                            b200kge_stream_t stream);
+int b200kge_score_1vsN_loss_csr_backward_dropout_dir(int model, int combine, int mask_dir, const b200kge_rows_t* ent,
+                                                     const b200kge_rows_t* rel, const int64_t* q_idx,
+                                                     const int64_t* p_idx, int64_t n, const int64_t* csr_off,
+                                                     const int64_t* csr_col, float label_smoothing, int loss_kind,
+                                                     float offset, int64_t batch_size, const b200kge_dropout_t* drop,
+                                                     float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
+                                                     void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+
+/* ---- The 1vsAll step of a reciprocal-relations model ----------------------------------------------------------------
+ * LibKGE's ReciprocalRelationsModel (reciprocal_relations_model.py:85-92) keeps 2R relation rows and answers score_po
+ * as the sp_ query (o, p + R) against the same table.  The step is
+ *   (loss(score_sp(s, p), o) + loss(score_sp(o, p + R), s)) / n
+ * with rel->rows == 2 * num_relations (else B200KGE_ERR_INVALID).  Without dropout (drop == NULL) it is the stacked
+ * problem of b200kge_train_1vsall_forward with the rows [n, 2n) folded as sp_ queries (o_i, p_i + R), labelled s_i —
+ * CP included, which stacks here because both halves read the table columns [D/2, D).  The backward (OVERWRITES d_ent
+ * and all 2R rows of d_rel) runs the same G planes / split-K GEMMs or distance row-gradient passes and unfolds the
+ * second half into d_ent[o], d_rel[p + R].  With `drop`, direction 0 draws streams 0-2 as the plain step and
+ * direction 1 draws the _po streams 3-5 (embed_all, embed(p + R), embed(o)), with the mask rows of the plain step.
+ * Model coverage of both calls: that of b200kge_train_1vsall_backward (dot family, TransE L1/L2, RotatE L1 for the
+ * backward; the forward also takes the other norms).  Workspace (either call, with or without dropout):
+ * b200kge_train_1vsall_reciprocal_workspace_bytes. */
+size_t b200kge_train_1vsall_reciprocal_workspace_bytes(int model, int64_t n, int64_t E, int32_t D);
+int b200kge_train_1vsall_reciprocal_forward(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                                            const b200kge_rows_t* rel, int64_t num_relations, const int64_t* triples,
+                                            int64_t n, int loss_kind, float offset, const b200kge_dropout_t* drop,
+                                            float* loss_out, void* workspace, size_t workspace_bytes,
+                                            b200kge_stream_t stream);
+int b200kge_train_1vsall_reciprocal_backward(int model, float l_norm, const b200kge_rows_t* ent,
+                                             const b200kge_rows_t* rel, int64_t num_relations, const int64_t* triples,
+                                             int64_t n, int loss_kind, float offset, const b200kge_dropout_t* drop,
+                                             float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
+                                             size_t workspace_bytes, b200kge_stream_t stream);
 
 /* ---- Embedding dropout of the negative-sampling training step ------------------------------------------------------
  * Per slot (0 = S or 2 = O; the P slot is not served) and sub-batch, train_negative_sampling.py:139-148 makes six draws,

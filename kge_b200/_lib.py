@@ -138,6 +138,22 @@ SIGNATURES = {
                                                                C.c_float, C.c_int64, _DP, C.c_void_p, C.c_int64,
                                                                C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t,
                                                                C.c_void_p]),
+    "b200kge_score_1vsN_loss_csr_dropout_dir": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _RP, _RP,
+                                                          C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                                          C.c_int64, C.c_float, C.c_int, C.c_float, _DP, C.c_void_p,
+                                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_score_1vsN_loss_csr_backward_dropout_dir": (C.c_int, [C.c_int, C.c_int, C.c_int, _RP, _RP, C.c_void_p,
+                                                                   C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                                                   C.c_float, C.c_int, C.c_float, C.c_int64, _DP,
+                                                                   C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                                                   C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_train_1vsall_reciprocal_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32]),
+    "b200kge_train_1vsall_reciprocal_forward": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_int64, C.c_void_p,
+                                                          C.c_int64, C.c_int, C.c_float, _DP, C.c_void_p, C.c_void_p,
+                                                          C.c_size_t, C.c_void_p]),
+    "b200kge_train_1vsall_reciprocal_backward": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_int64, C.c_void_p,
+                                                           C.c_int64, C.c_int, C.c_float, _DP, C.c_void_p, C.c_int64,
+                                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_ns_score_dropout": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
                                            C.c_int64, C.c_int, _DP, C.c_void_p, C.c_int64, C.c_void_p]),
     "b200kge_ns_dropout_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32]),

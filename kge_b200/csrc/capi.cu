@@ -91,6 +91,7 @@ struct Block {
   const Rows* cand;
   int64_t n;
   const float* Qpre = nullptr;   // already-folded queries [nq, round_up(K,32)] (skips the fold launches)
+  bool same_fold = false;        // stacked halves BOTH use `combine` (the reciprocal-relations step)
 };
 
 // nchunks_out / part_out (optional): number of per-row partial chunks and the partial buffer the loss
@@ -101,7 +102,7 @@ int run_block(const Block& B, float l_norm, int precision, int epi_kind, EpiPara
   const int D = B.q0->dim;
   Folded f0 = folded_problem(B.model, B.combine, D, l_norm);
   Folded f1 = f0;
-  if (B.q1) f1 = folded_problem(B.model, 1 - B.combine, D, l_norm);
+  if (B.q1 && !B.same_fold) f1 = folded_problem(B.model, 1 - B.combine, D, l_norm);
   const bool cols_differ = B.q1 && (f0.col_off != f1.col_off);   // CP: halves read different columns
   const int K = f0.K;
   const int64_t ldq = round_up(K, 32);
@@ -161,7 +162,7 @@ int run_block(const Block& B, float l_norm, int precision, int epi_kind, EpiPara
       if (!Qw) { set_error("workspace too small for folded queries"); return B200KGE_ERR_WORKSPACE; }
       rc = launch_fold_queries(B.model, B.combine, *B.q0, *B.p, n, 0, Qw, ldq, st);
       if (rc) return rc;
-      if (B.q1) { rc = launch_fold_queries(B.model, 1 - B.combine, *B.q1, *B.p, n, n, Qw, ldq, st); if (rc) return rc; }
+      if (B.q1) { rc = launch_fold_queries(B.model, B.same_fold ? B.combine : 1 - B.combine, *B.q1, *B.p, n, n, Qw, ldq, st); if (rc) return rc; }
       Q = Qw;
     }
     if (tc_kind == 3) {
@@ -219,7 +220,7 @@ int run_block(const Block& B, float l_norm, int precision, int epi_kind, EpiPara
     if (!Qw) { set_error("workspace too small for folded queries"); return B200KGE_ERR_WORKSPACE; }
     rc = launch_fold_queries(B.model, B.combine, *B.q0, *B.p, n, 0, Qw, ldq, st);
     if (rc) return rc;
-    if (B.q1) { rc = launch_fold_queries(B.model, 1 - B.combine, *B.q1, *B.p, n, n, Qw, ldq, st); if (rc) return rc; }
+    if (B.q1) { rc = launch_fold_queries(B.model, B.same_fold ? B.combine : 1 - B.combine, *B.q1, *B.p, n, n, Qw, ldq, st); if (rc) return rc; }
     Q = Qw;
   }
   const int nch = pairwise_simt_nchunks(nq, m);
@@ -270,6 +271,22 @@ __global__ void pack_triples_kernel(const int64_t* __restrict__ q, const int64_t
   tri[3 * i + 1] = p[i];
   tri[3 * i + (combine == B200KGE_SP_ ? 0 : 2)] = q[i];
   tri[3 * i + (combine == B200KGE_SP_ ? 2 : 0)] = 0;
+}
+
+// out[i] = idx[i] + off: the reciprocal relation rows p + num_relations (reciprocal_relations_model.py:90)
+__global__ void offset_index_kernel(const int64_t* __restrict__ idx, int64_t n, int64_t off, int64_t* __restrict__ out) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i < n) out[i] = idx[i] + off;
+}
+
+// rel must hold the 2R rows of a reciprocal-relations base model
+int check_reciprocal(const b200kge_rows_t* rel, int64_t num_rel) {
+  if (num_rel <= 0 || rel->rows != 2 * num_rel) {
+    set_error("reciprocal relations need rel->rows == 2 * num_relations (got %lld rows, num_relations %lld)",
+              (long long)rel->rows, (long long)num_rel);
+    return B200KGE_ERR_INVALID;
+  }
+  return 0;
 }
 
 __global__ void __launch_bounds__(128)
@@ -562,11 +579,12 @@ int b200kge_sample_uniform(uint64_t seed, uint64_t offset, int64_t vocab, int64_
   return launch_sample_uniform(seed, offset, vocab, n * K, out, (cudaStream_t)stream);
 }
 
-int b200kge_train_1vsall_forward(int model, float l_norm, int precision,
-                                 const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                 const int64_t* triples, int64_t n, int loss_kind, float offset,
-                                 float* loss_out, void* workspace, size_t workspace_bytes,
-                                 b200kge_stream_t stream) {
+// num_rel > 0: the reciprocal-relations step (rows n..2n are the sp_ queries (o, p + num_rel), label s)
+static int train_1vsall_forward_impl(int model, float l_norm, int precision,
+                                     const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                     const int64_t* triples, int64_t n, int loss_kind, float offset,
+                                     float* loss_out, void* workspace, size_t workspace_bytes,
+                                     b200kge_stream_t stream, int64_t num_rel) {
   if (!ent || !rel || !triples || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
   int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
@@ -578,15 +596,17 @@ int b200kge_train_1vsall_forward(int model, float l_norm, int precision,
   Rows E = to_rows(ent), R = to_rows(rel);
   const int epi = (loss_kind == B200KGE_LOSS_BCE) ? EPI_BCE : EPI_KL;
   const float scale = 1.0f / (float)n;       // "/ batch_size"   train_1vsAll.py:65,76
-  Folded f0 = folded_problem(model, B200KGE_SP_, E.dim, l_norm), f1 = folded_problem(model, B200KGE__PO, E.dim, l_norm);
+  // reciprocal: both halves are sp_ queries
+  Folded f0 = folded_problem(model, B200KGE_SP_, E.dim, l_norm),
+         f1 = folded_problem(model, num_rel > 0 ? B200KGE_SP_ : B200KGE__PO, E.dim, l_norm);
   {
-    // Pre-split tensor-core path (dot family except CP, whose directions read different table columns): the whole
-    // step is THREE launches — prologue (gather + both folds + operand split of queries and table + labels), the
-    // scorer with the loss reduction in its epilogue, and the fixed-order finaliser.
+    // Pre-split tensor-core path (dot family except CP, whose directions read different table columns — CP joins in
+    // the reciprocal step): the whole step is THREE launches — prologue (gather + both folds + operand split of queries
+    // and table + labels), the scorer with the loss reduction in its epilogue, and the fixed-order finaliser.
     const char* env_v = getenv("B200KGE_TC_VERSION");
     const int tcv = (env_v && atoi(env_v) == 1) ? 1 : 3;
     const int K = f0.K;
-    const bool presplit = f0.col_off == f1.col_off && f0.pair_op == PAIR_DOT && model != B200KGE_CP &&
+    const bool presplit = f0.col_off == f1.col_off && f0.pair_op == PAIR_DOT && (model != B200KGE_CP || num_rel > 0) &&
                           (precision == B200KGE_PREC_AUTO || precision == B200KGE_PREC_F16X3) && K >= 32 && K <= 1024 &&
                           n >= 16 && E.rows < (1ll << 31) && tcv == 3 &&
                           ((size_t)round_up(K, 64) + (model == B200KGE_RESCAL ? E.dim : 0)) * 4 <= 48 * 1024;
@@ -609,7 +629,7 @@ int b200kge_train_1vsall_forward(int model, float l_norm, int precision,
         return B200KGE_ERR_WORKSPACE;
       }
       unsigned int* ticket = reinterpret_cast<unsigned int*>(scratch + 512);
-      if ((rc = launch_prep_split_1vsall(model, E, R, triples, n, SQ, ST, lab, ticket, st))) return rc;
+      if ((rc = launch_prep_split_1vsall(model, E, R, triples, n, SQ, ST, lab, ticket, st, num_rel))) return rc;
       EpiParams P = empty_epi();
       P.label_idx = lab;
       P.offset = (loss_kind == B200KGE_LOSS_BCE) ? offset : 0.f;
@@ -626,7 +646,8 @@ int b200kge_train_1vsall_forward(int model, float l_norm, int precision,
     int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
     uint8_t* scratch = (uint8_t*)ws.take(1024);      // finaliser scratch: block sums + ticket (+512)
     if (!Q || !lab || !scratch) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
-    rc = launch_prep_1vsall(model, E, R, triples, n, Q, ldq, lab, reinterpret_cast<unsigned int*>(scratch + 512), st);
+    rc = launch_prep_1vsall(model, E, R, triples, n, Q, ldq, lab, reinterpret_cast<unsigned int*>(scratch + 512), st,
+                            num_rel);
     if (rc) return rc;
     Rows S = E; S.idx = lab; S.rows = n;           // placeholders: operands are pre-folded
     Rows Pr = R; Pr.idx = lab; Pr.rows = n;
@@ -635,6 +656,7 @@ int b200kge_train_1vsall_forward(int model, float l_norm, int precision,
     P.offset = (loss_kind == B200KGE_LOSS_BCE) ? offset : 0.f;
     Block B{model, B200KGE_SP_, &S, &S, &Pr, &E, n};
     B.Qpre = Q;
+    B.same_fold = num_rel > 0;
     int nch = 0;
     float* part = nullptr;
     rc = run_block(B, l_norm, precision, epi, P, ws, st, &nch, &part);
@@ -669,6 +691,15 @@ int b200kge_train_1vsall_forward(int model, float l_norm, int precision,
     if (rc) return rc;
   }
   return 0;
+}
+
+int b200kge_train_1vsall_forward(int model, float l_norm, int precision,
+                                 const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                 const int64_t* triples, int64_t n, int loss_kind, float offset,
+                                 float* loss_out, void* workspace, size_t workspace_bytes,
+                                 b200kge_stream_t stream) {
+  return train_1vsall_forward_impl(model, l_norm, precision, ent, rel, triples, n, loss_kind, offset, loss_out,
+                                   workspace, workspace_bytes, stream, 0);
 }
 
 int b200kge_train_1vsall_forward_host(int model, float l_norm, int precision,
@@ -732,7 +763,8 @@ int backward_block(int model, const Rows& E, const Rows& R, const int64_t* tripl
                    const float* Q, int64_t ldq, const int64_t* lab, int col_off, int K, int loss_kind, float offset,
                    float* d_ent, int64_t lde, float* dQ, Arena ws, cudaStream_t st,
                    const float* Gdense = nullptr, int64_t ldg = 0, const int64_t* csr_off = nullptr,
-                   const int64_t* csr_col = nullptr, float csr_a = 1.f, float csr_b = 0.f, float inv_batch = 0.f) {
+                   const int64_t* csr_col = nullptr, float csr_a = 1.f, float csr_b = 0.f, float inv_batch = 0.f,
+                   bool same_fold = false) {
   const int64_t nq = dir < 0 ? 2 * n : n, m = E.rows;
   const int64_t ldz = round_up(m, 4), Ep = round_up(m, 64), Np = round_up(nq, 64);
   const int64_t ldE = round_up(m, 4), ldN = round_up(nq, 4);
@@ -759,6 +791,7 @@ int backward_block(int model, const Rows& E, const Rows& R, const int64_t* tripl
     P.out = z; P.ldo = ldz;
     Block B{model, dir <= 0 ? B200KGE_SP_ : B200KGE__PO, &S, dir < 0 ? &S : nullptr, &Pr, &E, n};
     B.Qpre = Q;
+    B.same_fold = same_fold;
     if ((rc = run_block(B, 1.0f, B200KGE_PREC_AUTO, EPI_STORE, P, ws, st, nullptr))) return rc;
   }
   // 2. G = sigmoid(z + off) - y as planes, both layouts
@@ -837,10 +870,11 @@ size_t b200kge_train_1vsall_backward_workspace_bytes(int model, int64_t n, int64
   return (size_t)nq * ldq * 4 + (size_t)n * 5 * 8 + 4096 + backward_block_bytes(nq, E, K, ldq);
 }
 
-int b200kge_train_1vsall_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                    const int64_t* triples, int64_t n, int loss_kind, float offset, float* d_ent,
-                                    int64_t lde, float* d_rel, int64_t ldr, void* workspace, size_t workspace_bytes,
-                                    b200kge_stream_t stream) {
+// num_rel > 0: the backward of the reciprocal-relations step (train_1vsall_forward_impl)
+static int train_1vsall_backward_impl(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                      const int64_t* triples, int64_t n, int loss_kind, float offset, float* d_ent,
+                                      int64_t lde, float* d_rel, int64_t ldr, void* workspace, size_t workspace_bytes,
+                                      b200kge_stream_t stream, int64_t num_rel) {
   if (!ent || !rel || !triples || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
   int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
@@ -871,7 +905,7 @@ int b200kge_train_1vsall_backward(int model, float l_norm, const b200kge_rows_t*
       set_error("workspace too small");
       return B200KGE_ERR_WORKSPACE;
     }
-    if ((rc = launch_prep_1vsall(model, E, R, triples, n, Q, ldq, lab, nullptr, st))) return rc;
+    if ((rc = launch_prep_1vsall(model, E, R, triples, n, Q, ldq, lab, nullptr, st, num_rel))) return rc;
     {
       Rows S = E; S.idx = lab; S.rows = n;      // placeholders: operands are pre-folded
       Rows Pr = R; Pr.idx = lab; Pr.rows = n;
@@ -879,6 +913,7 @@ int b200kge_train_1vsall_backward(int model, float l_norm, const b200kge_rows_t*
       P.out = z; P.ldo = ldz;
       Block B{model, B200KGE_SP_, &S, &S, &Pr, &E, n};
       B.Qpre = Q;
+      B.same_fold = num_rel > 0;
       if ((rc = run_block(B, l_norm, B200KGE_PREC_AUTO, EPI_STORE, P, ws, st, nullptr))) return rc;
     }
     if (row_stat && (rc = launch_row_lse(z, ldz, nq, m, lab, row_stat, st))) return rc;
@@ -888,9 +923,10 @@ int b200kge_train_1vsall_backward(int model, float l_norm, const b200kge_rows_t*
     // each pass reads its weights transposed ([column, row]): the other pass's orientation
     if ((rc = launch_pair_rowgrad(f.pair_op, Q, ldq, nq, E.base, E.ld, m, f.K, Gt, ldN, dQ, ldq, st))) return rc;
     if ((rc = launch_pair_rowgrad(f.pair_op, E.base, E.ld, m, Q, ldq, nq, f.K, G, ldz, d_ent, lde, st))) return rc;
-    return launch_unfold_distance(model, E, R, triples, n, -1, dQ, ldq, d_ent, lde, d_rel, ldr, st);
+    return launch_unfold_distance(model, E, R, triples, n, -1, dQ, ldq, d_ent, lde, d_rel, ldr, st, num_rel);
   }
-  Folded f0 = folded_problem(model, B200KGE_SP_, E.dim, 1.0f), f1 = folded_problem(model, B200KGE__PO, E.dim, 1.0f);
+  Folded f0 = folded_problem(model, B200KGE_SP_, E.dim, 1.0f),
+         f1 = folded_problem(model, num_rel > 0 ? B200KGE_SP_ : B200KGE__PO, E.dim, 1.0f);
   const int64_t ldq = round_up(f0.K, 32);
   if (f0.col_off == f1.col_off) {
     float* Q = (float*)ws.take((size_t)(2 * n) * ldq * 4);
@@ -898,9 +934,12 @@ int b200kge_train_1vsall_backward(int model, float l_norm, const b200kge_rows_t*
     if (!Q || !lab) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
     float* dQ = (float*)ws.take((size_t)(2 * n) * ldq * 4);
     if (!dQ) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
-    if ((rc = launch_prep_1vsall(model, E, R, triples, n, Q, ldq, lab, nullptr, st))) return rc;
-    if ((rc = backward_block(model, E, R, triples, n, -1, Q, ldq, lab, f0.col_off, f0.K, loss_kind, offset, d_ent, lde, dQ, ws, st))) return rc;
-    return launch_unfold(model, E, R, triples, n, -1, dQ, ldq, d_ent, lde, d_rel, ldr, st);
+    if ((rc = launch_prep_1vsall(model, E, R, triples, n, Q, ldq, lab, nullptr, st, num_rel))) return rc;
+    // reciprocal CP: the table GEMM stores columns [h, D) only; the unfold adds the rows' [0, h) into zeros
+    if (f0.col_off > 0) B2K_CUDA(cudaMemset2DAsync(d_ent, (size_t)lde * 4, 0, (size_t)f0.col_off * 4, (size_t)E.rows, st));
+    if ((rc = backward_block(model, E, R, triples, n, -1, Q, ldq, lab, f0.col_off, f0.K, loss_kind, offset, d_ent, lde, dQ, ws, st,
+                             nullptr, 0, nullptr, nullptr, 1.f, 0.f, 0.f, num_rel > 0))) return rc;
+    return launch_unfold(model, E, R, triples, n, -1, dQ, ldq, d_ent, lde, d_rel, ldr, st, num_rel);
   }
   // CP: the two directions pair with different halves of the candidate columns
   int64_t* sidx = (int64_t*)ws.take((size_t)n * 8);
@@ -925,6 +964,14 @@ int b200kge_train_1vsall_backward(int model, float l_norm, const b200kge_rows_t*
   for (int dir = 0; dir < 2; ++dir)
     if ((rc = launch_unfold(model, E, R, triples, n, dir, dQ2 + (size_t)dir * n * ldq, ldq, d_ent, lde, d_rel, ldr, st))) return rc;
   return 0;
+}
+
+int b200kge_train_1vsall_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                    const int64_t* triples, int64_t n, int loss_kind, float offset, float* d_ent,
+                                    int64_t lde, float* d_rel, int64_t ldr, void* workspace, size_t workspace_bytes,
+                                    b200kge_stream_t stream) {
+  return train_1vsall_backward_impl(model, l_norm, ent, rel, triples, n, loss_kind, offset, d_ent, lde, d_rel, ldr,
+                                    workspace, workspace_bytes, stream, 0);
 }
 
 
@@ -1295,11 +1342,13 @@ struct DirGrad {
   const int64_t* csr_off; const int64_t* csr_col; float csr_a, csr_b, inv_batch;
   int loss_kind; float offset;
 };
-int dropout_backward_dir(int model, float l_norm, int dir, const Rows& E, const Rows& R, const int64_t* q_idx,
+// `dir` is the fold (query type); `mask_dir` picks the draws (they differ for the reciprocal direction: sp_ fold, _po
+// draws).
+int dropout_backward_dir(int model, float l_norm, int dir, int mask_dir, const Rows& E, const Rows& R, const int64_t* q_idx,
                          const int64_t* p_idx, int64_t n, const b200kge_dropout_t& d, const DirGrad& g,
                          const MaskedOps& o, float* Q, float* dQ, float* dT, float* dQe, float* dPr, const int64_t* tri,
                          Arena ws, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, cudaStream_t st) {
-  const DirMasks m = dir_masks(d, dir);
+  const DirMasks m = dir_masks(d, mask_dir);
   const Folded f = folded_problem(model, dir, E.dim, l_norm);
   const int64_t ldq = round_up(f.K, 32), mE = E.rows;
   const int D = E.dim, Dr = R.dim;
@@ -1454,10 +1503,138 @@ int b200kge_train_1vsall_backward_dropout(int model, float l_norm, const b200kge
   const Arena rest = rest_of(ws);
   for (int dir = 0; dir < 2; ++dir) {
     DirGrad g{lab + dir * n, nullptr, nullptr, 1.f, 0.f, 0.f, loss_kind, offset};
-    if ((rc = dropout_backward_dir(model, l_norm, dir, E, R, dir == 0 ? sidx : oidx, pidx, n, *drop, g, b.o, b.Q, b.dQ,
-                                   b.dT, b.dQe, b.dPr, b.tri, rest, d_ent, lde, d_rel, ldr, st))) return rc;
+    if ((rc = dropout_backward_dir(model, l_norm, dir, dir, E, R, dir == 0 ? sidx : oidx, pidx, n, *drop, g, b.o, b.Q,
+                                   b.dQ, b.dT, b.dQe, b.dPr, b.tri, rest, d_ent, lde, d_rel, ldr, st))) return rc;
   }
   return 0;
+}
+
+// ---- reciprocal relations (reciprocal_relations_model.py:85-92): both directions are sp_ queries against the table;
+// the second one, (o, p + R) labelled s, is score_po and draws its masks on the _po streams in the reference's call
+// order (embed_all: B200KGE_DROP_PO_TABLE, embed(p + R): B200KGE_DROP_PO_REL, embed(o): B200KGE_DROP_PO_ENT).
+
+static int recip_forward_dropout(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                                 const b200kge_rows_t* rel, int64_t num_rel, const int64_t* triples, int64_t n,
+                                 int loss_kind, float offset, const b200kge_dropout_t* drop, float* loss_out,
+                                 void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  int rc;
+  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
+  if (n <= 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  Rows E = to_rows(ent), R = to_rows(rel);
+  int64_t* sidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* pidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* oidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* pinv = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
+  float* dir_loss = (float*)ws.take(256);
+  MaskedOps o;
+  if (!sidx || !pidx || !oidx || !pinv || !lab || !dir_loss || !take_masked(ws, n, E.rows, E.dim, R.dim, o)) {
+    set_error("workspace too small (see b200kge_train_1vsall_reciprocal_workspace_bytes)");
+    return B200KGE_ERR_WORKSPACE;
+  }
+  unpack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(triples, n, sidx, pidx, oidx, lab);
+  B2K_LAUNCH_CHECK("unpack_triples_kernel");
+  offset_index_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pidx, n, num_rel, pinv);
+  B2K_LAUNCH_CHECK("offset_index_kernel");
+  const Arena rest = rest_of(ws);
+  for (int dir = 0; dir < 2; ++dir) {
+    Rows Qr, Pr, Tr;
+    if ((rc = gather_masked(dir_masks(*drop, dir), E, R, dir == 0 ? sidx : oidx, dir == 0 ? pidx : pinv, n, o, Qr, Pr,
+                            Tr, st))) return rc;
+    const b200kge_rows_t q{Qr.base, nullptr, n, Qr.ld, Qr.dim}, p{Pr.base, nullptr, n, Pr.ld, Pr.dim},
+        c{Tr.base, nullptr, Tr.rows, Tr.ld, Tr.dim};
+    const b200kge_labels_t labels{lab + dir * n, nullptr, 0};
+    if ((rc = b200kge_score_1vsN_loss(model, B200KGE_SP_, l_norm, precision, &q, &p, &c, n, &labels, loss_kind, offset,
+                                      dir_loss + dir, nullptr, rest.base, rest.cap, st))) return rc;
+  }
+  return launch_rows_sum(dir_loss, 2, 1.0f / (float)n, loss_out, st);
+}
+
+static int recip_backward_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                  int64_t num_rel, const int64_t* triples, int64_t n, int loss_kind, float offset,
+                                  const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
+                                  void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  int rc;
+  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
+  const Folded f = folded_problem(model, B200KGE_SP_, ent->dim, l_norm);
+  if (f.pair_op != PAIR_DOT && f.pair_op != PAIR_L1 && f.pair_op != PAIR_L2 && f.pair_op != PAIR_CMOD_L1) {
+    set_error("the distance-family backward covers l_norm 1 and 2 (TransE) and 1 (RotatE)");
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  Rows E = to_rows(ent), R = to_rows(rel);
+  B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
+  B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st));
+  if (n <= 0) return 0;
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  int64_t* sidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* pidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* oidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* pinv = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
+  BackBufs b;
+  if (!sidx || !pidx || !oidx || !pinv || !lab || !take_back(ws, n, E.rows, E.dim, R.dim, round_up(f.K, 32), b)) {
+    set_error("workspace too small (see b200kge_train_1vsall_reciprocal_workspace_bytes)");
+    return B200KGE_ERR_WORKSPACE;
+  }
+  unpack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(triples, n, sidx, pidx, oidx, lab);
+  B2K_LAUNCH_CHECK("unpack_triples_kernel");
+  offset_index_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pidx, n, num_rel, pinv);
+  B2K_LAUNCH_CHECK("offset_index_kernel");
+  if ((rc = launch_identity_triples(n, b.tri, st))) return rc;
+  const Arena rest = rest_of(ws);
+  for (int dir = 0; dir < 2; ++dir) {
+    DirGrad g{lab + dir * n, nullptr, nullptr, 1.f, 0.f, 0.f, loss_kind, offset};
+    if ((rc = dropout_backward_dir(model, l_norm, B200KGE_SP_, dir, E, R, dir == 0 ? sidx : oidx, dir == 0 ? pidx : pinv,
+                                   n, *drop, g, b.o, b.Q, b.dQ, b.dT, b.dQe, b.dPr, b.tri, rest, d_ent, lde, d_rel, ldr,
+                                   st))) return rc;
+  }
+  return 0;
+}
+
+size_t b200kge_train_1vsall_reciprocal_workspace_bytes(int model, int64_t n, int64_t E, int32_t D) {
+  const size_t fwd = b200kge_workspace_bytes(model, n, E, D, 0);
+  const size_t bwd = b200kge_train_1vsall_backward_workspace_bytes(model, n, E, D);
+  const size_t drop = b200kge_train_1vsall_dropout_workspace_bytes(model, n, E, D) + (size_t)n * 8 + 256;
+  const size_t m = fwd > bwd ? fwd : bwd;
+  return m > drop ? m : drop;
+}
+
+int b200kge_train_1vsall_reciprocal_forward(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                                            const b200kge_rows_t* rel, int64_t num_relations, const int64_t* triples,
+                                            int64_t n, int loss_kind, float offset, const b200kge_dropout_t* drop,
+                                            float* loss_out, void* workspace, size_t workspace_bytes,
+                                            b200kge_stream_t stream) {
+  if (!ent || !rel || !triples || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  int rc = check_reciprocal(rel, num_relations); if (rc) return rc;
+  if (!drop)
+    return train_1vsall_forward_impl(model, l_norm, precision, ent, rel, triples, n, loss_kind, offset, loss_out,
+                                     workspace, workspace_bytes, stream, num_relations);
+  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
+  if ((rc = validate_model(model, to_rows(ent), to_rows(rel)))) return rc;
+  if ((rc = validate_norm(model, l_norm))) return rc;
+  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  return recip_forward_dropout(model, l_norm, precision, ent, rel, num_relations, triples, n, loss_kind, offset, drop,
+                               loss_out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int b200kge_train_1vsall_reciprocal_backward(int model, float l_norm, const b200kge_rows_t* ent,
+                                             const b200kge_rows_t* rel, int64_t num_relations, const int64_t* triples,
+                                             int64_t n, int loss_kind, float offset, const b200kge_dropout_t* drop,
+                                             float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
+                                             size_t workspace_bytes, b200kge_stream_t stream) {
+  if (!ent || !rel || !triples || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  int rc = check_reciprocal(rel, num_relations); if (rc) return rc;
+  if (!drop)
+    return train_1vsall_backward_impl(model, l_norm, ent, rel, triples, n, loss_kind, offset, d_ent, lde, d_rel, ldr,
+                                      workspace, workspace_bytes, stream, num_relations);
+  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
+  if ((rc = validate_model(model, to_rows(ent), to_rows(rel)))) return rc;
+  if ((rc = validate_norm(model, l_norm))) return rc;
+  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  if (lde < ent->dim || ldr < rel->dim) { set_error("gradient leading dimensions are smaller than the table widths"); return B200KGE_ERR_INVALID; }
+  return recip_backward_dropout(model, l_norm, ent, rel, num_relations, triples, n, loss_kind, offset, drop, d_ent, lde,
+                                d_rel, ldr, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 size_t b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(int model, int64_t n, int64_t E, int32_t D, int64_t nnz) {
@@ -1466,15 +1643,17 @@ size_t b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(int model, int64_t n,
   return masked_bytes(model, n, E, D) + (fwd > bwd ? fwd : bwd);
 }
 
-int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, float l_norm, int precision, const b200kge_rows_t* ent,
-                                        const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx, int64_t n,
-                                        const int64_t* csr_off, const int64_t* csr_col, int64_t nnz,
-                                        float label_smoothing, int loss_kind, float offset,
-                                        const b200kge_dropout_t* drop, float* loss_out, float* row_loss_out,
-                                        void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+int b200kge_score_1vsN_loss_csr_dropout_dir(int model, int combine, int mask_dir, float l_norm, int precision,
+                                            const b200kge_rows_t* ent, const b200kge_rows_t* rel, const int64_t* q_idx,
+                                            const int64_t* p_idx, int64_t n, const int64_t* csr_off,
+                                            const int64_t* csr_col, int64_t nnz, float label_smoothing, int loss_kind,
+                                            float offset, const b200kge_dropout_t* drop, float* loss_out,
+                                            float* row_loss_out, void* workspace, size_t workspace_bytes,
+                                            b200kge_stream_t stream) {
   if (!ent || !rel || (!q_idx && n > 0) || (!p_idx && n > 0) || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
   if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
+  if (mask_dir != B200KGE_SP_ && mask_dir != B200KGE__PO) { set_error("bad mask direction %d", mask_dir); return B200KGE_ERR_INVALID; }
   int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
   if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1487,7 +1666,7 @@ int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, float l_norm, in
     return B200KGE_ERR_WORKSPACE;
   }
   Rows Qr, Pr, Tr;
-  if ((rc = gather_masked(dir_masks(*drop, combine), E, R, q_idx, p_idx, n, o, Qr, Pr, Tr, st))) return rc;
+  if ((rc = gather_masked(dir_masks(*drop, mask_dir), E, R, q_idx, p_idx, n, o, Qr, Pr, Tr, st))) return rc;
   const b200kge_rows_t q{Qr.base, nullptr, n, Qr.ld, Qr.dim}, p{Pr.base, nullptr, n, Pr.ld, Pr.dim},
       c{Tr.base, nullptr, Tr.rows, Tr.ld, Tr.dim};
   const Arena rest = rest_of(ws);
@@ -1496,16 +1675,28 @@ int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, float l_norm, in
                                      stream);
 }
 
-int b200kge_score_1vsN_loss_csr_backward_dropout(int model, int combine, const b200kge_rows_t* ent,
-                                                 const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx,
-                                                 int64_t n, const int64_t* csr_off, const int64_t* csr_col,
-                                                 float label_smoothing, int loss_kind, float offset, int64_t batch_size,
-                                                 const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
-                                                 int64_t ldr, void* workspace, size_t workspace_bytes,
-                                                 b200kge_stream_t stream) {
+int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, float l_norm, int precision, const b200kge_rows_t* ent,
+                                        const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx, int64_t n,
+                                        const int64_t* csr_off, const int64_t* csr_col, int64_t nnz,
+                                        float label_smoothing, int loss_kind, float offset,
+                                        const b200kge_dropout_t* drop, float* loss_out, float* row_loss_out,
+                                        void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+  return b200kge_score_1vsN_loss_csr_dropout_dir(model, combine, combine, l_norm, precision, ent, rel, q_idx, p_idx, n,
+                                                 csr_off, csr_col, nnz, label_smoothing, loss_kind, offset, drop,
+                                                 loss_out, row_loss_out, workspace, workspace_bytes, stream);
+}
+
+int b200kge_score_1vsN_loss_csr_backward_dropout_dir(int model, int combine, int mask_dir, const b200kge_rows_t* ent,
+                                                     const b200kge_rows_t* rel, const int64_t* q_idx,
+                                                     const int64_t* p_idx, int64_t n, const int64_t* csr_off,
+                                                     const int64_t* csr_col, float label_smoothing, int loss_kind,
+                                                     float offset, int64_t batch_size, const b200kge_dropout_t* drop,
+                                                     float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
+                                                     void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
   if (!ent || !rel || !q_idx || !p_idx || !csr_off || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
   if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
+  if (mask_dir != B200KGE_SP_ && mask_dir != B200KGE__PO) { set_error("bad mask direction %d", mask_dir); return B200KGE_ERR_INVALID; }
   int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
   if (model > B200KGE_RESCAL) { set_error("the tensor-core backward covers the dot family only (model %d)", model); return B200KGE_ERR_UNSUPPORTED; }
   if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
@@ -1527,8 +1718,20 @@ int b200kge_score_1vsN_loss_csr_backward_dropout(int model, int combine, const b
   if ((rc = launch_identity_triples(n, b.tri, st))) return rc;
   const float a = 1.0f - label_smoothing, bb = label_smoothing > 0.f ? 1.0f / (float)E.rows : 0.f;
   DirGrad g{q_idx /* placeholder index vector */, csr_off, csr_col, a, bb, 1.0f / (float)batch_size, loss_kind, offset};
-  return dropout_backward_dir(model, 1.0f, combine, E, R, q_idx, p_idx, n, *drop, g, b.o, b.Q, b.dQ, b.dT, b.dQe, b.dPr,
-                              b.tri, rest_of(ws), d_ent, lde, d_rel, ldr, st);
+  return dropout_backward_dir(model, 1.0f, combine, mask_dir, E, R, q_idx, p_idx, n, *drop, g, b.o, b.Q, b.dQ, b.dT,
+                              b.dQe, b.dPr, b.tri, rest_of(ws), d_ent, lde, d_rel, ldr, st);
+}
+
+int b200kge_score_1vsN_loss_csr_backward_dropout(int model, int combine, const b200kge_rows_t* ent,
+                                                 const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx,
+                                                 int64_t n, const int64_t* csr_off, const int64_t* csr_col,
+                                                 float label_smoothing, int loss_kind, float offset, int64_t batch_size,
+                                                 const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
+                                                 int64_t ldr, void* workspace, size_t workspace_bytes,
+                                                 b200kge_stream_t stream) {
+  return b200kge_score_1vsN_loss_csr_backward_dropout_dir(model, combine, combine, ent, rel, q_idx, p_idx, n, csr_off,
+                                                          csr_col, label_smoothing, loss_kind, offset, batch_size, drop,
+                                                          d_ent, lde, d_rel, ldr, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -327,9 +327,11 @@ __device__ __forceinline__ float finalize_row(const float* __restrict__ part, in
 int launch_fold_queries(int model, int combine, const Rows& q, const Rows& p, int64_t n,
                         int64_t row0, float* Q, int64_t ldq, cudaStream_t st);
 // one launch: unpack triples [n,3], fold sp_ rows (0..n) and _po rows (n..2n) into Q, write the
-// stacked labels [o ; s] and zero the finalisation ticket
+// stacked labels [o ; s] and zero the finalisation ticket.  num_rel > 0 (reciprocal relations): rows n..2n fold
+// (o, p + num_rel) with the sp_ fold instead
 int launch_prep_1vsall(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n,
-                       float* Q, int64_t ldq, int64_t* labels2n, unsigned int* ticket, cudaStream_t st);
+                       float* Q, int64_t ldq, int64_t* labels2n, unsigned int* ticket, cudaStream_t st,
+                       int64_t num_rel = 0);
 int launch_gather_rows(const Rows& src, int col_off, int K, float* dst, int64_t ldd,
                        cudaStream_t st);
 int launch_pairwise_simt(int epi_kind, int pair_op, float l_norm, const float* Q, int64_t ldq,

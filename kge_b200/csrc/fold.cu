@@ -43,20 +43,23 @@ fold_kernel(int combine, Rows qa, Rows pr, int64_t row0, float* __restrict__ Q, 
 // One launch for a whole 1vsAll step's prologue: block b < n folds (s_b, p_b) for the sp_ direction
 // into Q row b and labels it with o_b; block n+b folds (o_b, p_b) for _po into Q row n+b, label s_b
 // (train_1vsAll.py:59-65,75-76).  Replaces unpack + two fold launches.
-template <int MODEL>
+// RECIP (reciprocal relations, reciprocal_relations_model.py:85-92): block n+b folds (o_b, p_b + num_rel) with the sp_
+// fold instead, label s_b — both halves are sp_ queries against the same table columns.
+template <int MODEL, bool RECIP>
 __global__ void __launch_bounds__(128)
 prep_1vsall_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t n, float* __restrict__ Q,
-                   int64_t ldq, int64_t* __restrict__ labels2n, unsigned int* ticket, int K) {
+                   int64_t ldq, int64_t* __restrict__ labels2n, unsigned int* ticket, int K, int64_t num_rel) {
   const int64_t b = blockIdx.x;
-  const bool sp = b < n;
-  const int64_t i = sp ? b : b - n;
+  const bool first = b < n;
+  const bool sp = RECIP || first;
+  const int64_t i = first ? b : b - n;
   const int64_t si = tri[3 * i], pi = tri[3 * i + 1], oi = tri[3 * i + 2];
-  const float* __restrict__ a = ent.base + (sp ? si : oi) * ent.ld;
-  const float* __restrict__ p = rel.base + pi * rel.ld;
+  const float* __restrict__ a = ent.base + (first ? si : oi) * ent.ld;
+  const float* __restrict__ p = rel.base + (RECIP && !first ? pi + num_rel : pi) * rel.ld;
   const int D = ent.dim, h = D >> 1;
   const int64_t obase = b * ldq;
   if (threadIdx.x == 0) {
-    labels2n[b] = sp ? oi : si;
+    labels2n[b] = first ? oi : si;
     if (b == 0 && ticket) *ticket = 0u;
   }
   if constexpr (MODEL == B200KGE_RESCAL) {
@@ -71,18 +74,30 @@ prep_1vsall_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t 
 }
 
 int launch_prep_1vsall(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n,
-                       float* Q, int64_t ldq, int64_t* labels2n, unsigned int* ticket, cudaStream_t st) {
+                       float* Q, int64_t ldq, int64_t* labels2n, unsigned int* ticket, cudaStream_t st,
+                       int64_t num_rel) {
   if (n == 0) return 0;
   const int D = ent.dim;
   const int K = (model == B200KGE_CP) ? D / 2 : D;
   dim3 grid((unsigned)(2 * n)), block(128);
-#define B2K_PREP(M, SM) case M: prep_1vsall_kernel<M><<<grid, block, SM, st>>>(ent, rel, triples, n, Q, ldq, labels2n, ticket, K); break;
-  switch (model) {
-    B2K_PREP(B200KGE_COMPLEX, 0) B2K_PREP(B200KGE_DISTMULT, 0) B2K_PREP(B200KGE_SIMPLE, 0)
-    B2K_PREP(B200KGE_RESCAL, D * sizeof(float)) B2K_PREP(B200KGE_TRANSE, 0) B2K_PREP(B200KGE_ROTATE, 0)
-    default: set_error("model %d has no stacked 1vsAll prologue", model); return B200KGE_ERR_INVALID;
+#define B2K_PREP(M, SM) case M: prep_1vsall_kernel<M, false><<<grid, block, SM, st>>>(ent, rel, triples, n, Q, ldq, labels2n, ticket, K, 0); break;
+#define B2K_PREP_R(M, SM) case M: prep_1vsall_kernel<M, true><<<grid, block, SM, st>>>(ent, rel, triples, n, Q, ldq, labels2n, ticket, K, num_rel); break;
+  if (num_rel > 0) {
+    // reciprocal: CP joins the stacked problem (both halves read the table columns [h, D))
+    switch (model) {
+      B2K_PREP_R(B200KGE_COMPLEX, 0) B2K_PREP_R(B200KGE_DISTMULT, 0) B2K_PREP_R(B200KGE_SIMPLE, 0) B2K_PREP_R(B200KGE_CP, 0)
+      B2K_PREP_R(B200KGE_RESCAL, D * sizeof(float)) B2K_PREP_R(B200KGE_TRANSE, 0) B2K_PREP_R(B200KGE_ROTATE, 0)
+      default: set_error("model %d has no stacked 1vsAll prologue", model); return B200KGE_ERR_INVALID;
+    }
+  } else {
+    switch (model) {
+      B2K_PREP(B200KGE_COMPLEX, 0) B2K_PREP(B200KGE_DISTMULT, 0) B2K_PREP(B200KGE_SIMPLE, 0)
+      B2K_PREP(B200KGE_RESCAL, D * sizeof(float)) B2K_PREP(B200KGE_TRANSE, 0) B2K_PREP(B200KGE_ROTATE, 0)
+      default: set_error("model %d has no stacked 1vsAll prologue", model); return B200KGE_ERR_INVALID;
+    }
   }
 #undef B2K_PREP
+#undef B2K_PREP_R
   B2K_LAUNCH_CHECK("prep_1vsall_kernel");
   return 0;
 }

@@ -203,17 +203,20 @@ csr_grad_fix_kernel(const float* __restrict__ z, int64_t ldz, int64_t n, const i
 
 // ---------------------------------------------------------------------------------------------
 // Row-wise unfold: block b handles query row b.  dir < 0: rows [0,n) are sp_ (a = subject), rows [n,2n) are
-// _po (a = object) — the stacked layout of prep_1vsall_kernel; dir = 0 / 1: all rows sp_ / _po.
-template <int MODEL>
+// _po (a = object) — the stacked layout of prep_1vsall_kernel; dir = 0 / 1: all rows sp_ / _po.  RECIP (dir < 0): the
+// reciprocal layout, rows [n,2n) are sp_ with a = object and relation row p + num_rel.
+template <int MODEL, bool RECIP>
 __global__ void __launch_bounds__(128)
 unfold_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t n, int dir,
               const float* __restrict__ dQ, int64_t ldq, float* __restrict__ d_ent, int64_t lde,
-              float* __restrict__ d_rel, int64_t ldr) {
+              float* __restrict__ d_rel, int64_t ldr, int64_t num_rel) {
   const int64_t b = blockIdx.x;
-  const bool sp = dir < 0 ? (b < n) : (dir == 0);
-  const int64_t i = (dir < 0 && b >= n) ? b - n : b;
-  const int64_t si = tri[3 * i], pi = tri[3 * i + 1], oi = tri[3 * i + 2];
-  const int64_t ai = sp ? si : oi;
+  const bool second = dir < 0 && b >= n;
+  const bool sp = RECIP || (dir < 0 ? (b < n) : (dir == 0));
+  const int64_t i = second ? b - n : b;
+  const int64_t si = tri[3 * i], oi = tri[3 * i + 2];
+  const int64_t pi = RECIP && second ? tri[3 * i + 1] + num_rel : tri[3 * i + 1];
+  const int64_t ai = RECIP ? (second ? oi : si) : (sp ? si : oi);
   const float* __restrict__ a = ent.base + ai * ent.ld;
   const float* __restrict__ p = rel.base + pi * rel.ld;
   const float* __restrict__ g = dQ + b * ldq;
@@ -521,16 +524,19 @@ ns_backward_kernel_masked(Rows fa, Rows ent, Rows rel, const int64_t* __restrict
 }
 
 // unfold for the distance family (TransE: Q = a +- p; RotatE: rotation) — appended to the dot-family unfold
-template <int MODEL>
+// (RECIP: the reciprocal layout of unfold_kernel)
+template <int MODEL, bool RECIP>
 __global__ void __launch_bounds__(128)
 unfold_distance_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t n, int dir,
                        const float* __restrict__ dQ, int64_t ldq, float* __restrict__ d_ent, int64_t lde,
-                       float* __restrict__ d_rel, int64_t ldr) {
+                       float* __restrict__ d_rel, int64_t ldr, int64_t num_rel) {
   const int64_t b = blockIdx.x;
-  const bool sp = dir < 0 ? (b < n) : (dir == 0);
-  const int64_t i = (dir < 0 && b >= n) ? b - n : b;
-  const int64_t si = tri[3 * i], pi = tri[3 * i + 1], oi = tri[3 * i + 2];
-  const int64_t ai = sp ? si : oi;
+  const bool second = dir < 0 && b >= n;
+  const bool sp = RECIP || (dir < 0 ? (b < n) : (dir == 0));
+  const int64_t i = second ? b - n : b;
+  const int64_t si = tri[3 * i], oi = tri[3 * i + 2];
+  const int64_t pi = RECIP && second ? tri[3 * i + 1] + num_rel : tri[3 * i + 1];
+  const int64_t ai = RECIP ? (second ? oi : si) : (sp ? si : oi);
   const float* __restrict__ a = ent.base + ai * ent.ld;
   const float* __restrict__ p = rel.base + pi * rel.ld;
   const float* __restrict__ g = dQ + b * ldq;
@@ -591,9 +597,9 @@ int launch_ns_backward(int model, float l_norm, const Rows& ent, const Rows& rel
   if (model == B200KGE_TRANSE || model == B200KGE_ROTATE) {
     dim3 g2((unsigned)n), b2(128);
     if (model == B200KGE_TRANSE)
-      unfold_distance_kernel<B200KGE_TRANSE><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr);
+      unfold_distance_kernel<B200KGE_TRANSE, false><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, 0);
     else
-      unfold_distance_kernel<B200KGE_ROTATE><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr);
+      unfold_distance_kernel<B200KGE_ROTATE, false><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, 0);
     B2K_LAUNCH_CHECK("unfold_distance_kernel");
     return 0;
   }
@@ -640,13 +646,18 @@ int launch_ns_backward_masked(int model, float l_norm, const Rows& a, const Rows
 
 int launch_unfold_distance(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n, int dir,
                            const float* dQ, int64_t ldq, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                           cudaStream_t st) {
+                           cudaStream_t st, int64_t num_rel) {
   if (n == 0) return 0;
+  if (num_rel > 0 && dir >= 0) { set_error("the reciprocal unfold needs the stacked layout"); return B200KGE_ERR_INVALID; }
   dim3 g2((unsigned)(dir < 0 ? 2 * n : n)), b2(128);
-  if (model == B200KGE_TRANSE)
-    unfold_distance_kernel<B200KGE_TRANSE><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr);
+  if (model == B200KGE_TRANSE && num_rel > 0)
+    unfold_distance_kernel<B200KGE_TRANSE, true><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, num_rel);
+  else if (model == B200KGE_ROTATE && num_rel > 0)
+    unfold_distance_kernel<B200KGE_ROTATE, true><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, num_rel);
+  else if (model == B200KGE_TRANSE)
+    unfold_distance_kernel<B200KGE_TRANSE, false><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, 0);
   else if (model == B200KGE_ROTATE)
-    unfold_distance_kernel<B200KGE_ROTATE><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr);
+    unfold_distance_kernel<B200KGE_ROTATE, false><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, 0);
   else { set_error("not a distance-family model (%d)", model); return B200KGE_ERR_INVALID; }
   B2K_LAUNCH_CHECK("unfold_distance_kernel");
   return 0;
@@ -729,18 +740,30 @@ int launch_grad_planes_csr(const float* z, int64_t ldz, int64_t nq, int64_t E, c
 }
 
 int launch_unfold(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n, int dir,
-                  const float* dQ, int64_t ldq, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, cudaStream_t st) {
+                  const float* dQ, int64_t ldq, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, cudaStream_t st,
+                  int64_t num_rel) {
   if (n == 0) return 0;
+  if (num_rel > 0 && dir >= 0) { set_error("the reciprocal unfold needs the stacked layout"); return B200KGE_ERR_INVALID; }
   const int64_t nq = dir < 0 ? 2 * n : n;
   dim3 grid((unsigned)nq), block(128);
   const int D = ent.dim;
-#define B2K_UNFOLD(M, SM) case M: unfold_kernel<M><<<grid, block, SM, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr); break;
-  switch (model) {
-    B2K_UNFOLD(B200KGE_COMPLEX, 0) B2K_UNFOLD(B200KGE_DISTMULT, 0) B2K_UNFOLD(B200KGE_SIMPLE, 0)
-    B2K_UNFOLD(B200KGE_CP, 0) B2K_UNFOLD(B200KGE_RESCAL, 2 * D * sizeof(float))
-    default: set_error("the analytic backward covers the dot family only (model %d)", model); return B200KGE_ERR_UNSUPPORTED;
+#define B2K_UNFOLD(M, SM) case M: unfold_kernel<M, false><<<grid, block, SM, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, 0); break;
+#define B2K_UNFOLD_R(M, SM) case M: unfold_kernel<M, true><<<grid, block, SM, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, num_rel); break;
+  if (num_rel > 0) {
+    switch (model) {
+      B2K_UNFOLD_R(B200KGE_COMPLEX, 0) B2K_UNFOLD_R(B200KGE_DISTMULT, 0) B2K_UNFOLD_R(B200KGE_SIMPLE, 0)
+      B2K_UNFOLD_R(B200KGE_CP, 0) B2K_UNFOLD_R(B200KGE_RESCAL, 2 * D * sizeof(float))
+      default: set_error("the analytic backward covers the dot family only (model %d)", model); return B200KGE_ERR_UNSUPPORTED;
+    }
+  } else {
+    switch (model) {
+      B2K_UNFOLD(B200KGE_COMPLEX, 0) B2K_UNFOLD(B200KGE_DISTMULT, 0) B2K_UNFOLD(B200KGE_SIMPLE, 0)
+      B2K_UNFOLD(B200KGE_CP, 0) B2K_UNFOLD(B200KGE_RESCAL, 2 * D * sizeof(float))
+      default: set_error("the analytic backward covers the dot family only (model %d)", model); return B200KGE_ERR_UNSUPPORTED;
+    }
   }
 #undef B2K_UNFOLD
+#undef B2K_UNFOLD_R
   B2K_LAUNCH_CHECK("unfold_kernel");
   return 0;
 }

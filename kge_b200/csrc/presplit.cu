@@ -154,10 +154,12 @@ presplit_longrow_kernel(const SplitSet A, const SplitSet B, const int rows_a) {
 // matrix never reaches HBM).
 constexpr int PQ_THREADS = PS_WARPS * 32;
 
-template <int MODEL>
+// RECIP: the reciprocal layout of prep_1vsall_kernel (fold.cu) — block n+b folds (o_b, p_b + num_rel) with the sp_ fold.
+template <int MODEL, bool RECIP>
 __global__ void __launch_bounds__(PQ_THREADS)
 prep_split_1vsall_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t n, const SplitSet Qs,
-                         const SplitSet Ts, int64_t* __restrict__ labels2n, unsigned int* ticket, int K) {
+                         const SplitSet Ts, int64_t* __restrict__ labels2n, unsigned int* ticket, int K,
+                         int64_t num_rel) {
   extern __shared__ float sh[];      // [Kp] folded row (+ [D] entity row for RESCAL)
   const int64_t b = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -167,14 +169,15 @@ prep_split_1vsall_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, in
   }
   __shared__ float red[PS_WARPS];
   __shared__ int bad_any;
-  const bool sp = b < n;
-  const int64_t i = sp ? b : b - n;
+  const bool first = b < n;
+  const bool sp = RECIP || first;
+  const int64_t i = first ? b : b - n;
   const int64_t si = tri[3 * i], pi = tri[3 * i + 1], oi = tri[3 * i + 2];
-  const float* __restrict__ a = ent.base + (sp ? si : oi) * ent.ld;
-  const float* __restrict__ p = rel.base + pi * rel.ld;
+  const float* __restrict__ a = ent.base + (first ? si : oi) * ent.ld;
+  const float* __restrict__ p = rel.base + (RECIP && !first ? pi + num_rel : pi) * rel.ld;
   const int D = ent.dim, h = D >> 1, Kp = Qs.Kp;
   if (threadIdx.x == 0) {
-    labels2n[b] = sp ? oi : si;
+    labels2n[b] = first ? oi : si;
     bad_any = 0;
   }
   if (b == 0 && ticket && threadIdx.x == 0) *ticket = 0u;                   // the finaliser's last-block counter
@@ -231,7 +234,7 @@ prep_split_1vsall_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, in
 
 int launch_prep_split_1vsall(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n,
                              const SplitSet& Qs, const SplitSet& Ts, int64_t* labels2n, unsigned int* ticket,
-                             cudaStream_t st) {
+                             cudaStream_t st, int64_t num_rel) {
   if (n == 0) return 0;
   const int D = ent.dim;
   const int K = (model == B200KGE_CP) ? D / 2 : D;
@@ -240,12 +243,23 @@ int launch_prep_split_1vsall(int model, const Rows& ent, const Rows& rel, const 
   const size_t smem = ((size_t)Qs.Kp + (model == B200KGE_RESCAL ? D : 0)) * sizeof(float);
   if (smem > 48 * 1024) { set_error("embedding too wide for the fused prologue"); return B200KGE_ERR_UNSUPPORTED; }
   dim3 grid((unsigned)(2 * n + tb)), block(PQ_THREADS);
-#define B2K_PS(M) case M: prep_split_1vsall_kernel<M><<<grid, block, smem, st>>>(ent, rel, triples, n, Qs, Ts, labels2n, ticket, K); break;
-  switch (model) {
-    B2K_PS(B200KGE_COMPLEX) B2K_PS(B200KGE_DISTMULT) B2K_PS(B200KGE_SIMPLE) B2K_PS(B200KGE_RESCAL)
-    default: set_error("model %d has no fused pre-split prologue", model); return B200KGE_ERR_UNSUPPORTED;
+#define B2K_PS(M) case M: prep_split_1vsall_kernel<M, false><<<grid, block, smem, st>>>(ent, rel, triples, n, Qs, Ts, labels2n, ticket, K, 0); break;
+#define B2K_PS_R(M) case M: prep_split_1vsall_kernel<M, true><<<grid, block, smem, st>>>(ent, rel, triples, n, Qs, Ts, labels2n, ticket, K, num_rel); break;
+  if (num_rel > 0) {
+    // reciprocal: both halves are sp_ queries, so CP (table columns [h, D)) stacks too
+    switch (model) {
+      B2K_PS_R(B200KGE_COMPLEX) B2K_PS_R(B200KGE_DISTMULT) B2K_PS_R(B200KGE_SIMPLE) B2K_PS_R(B200KGE_CP)
+      B2K_PS_R(B200KGE_RESCAL)
+      default: set_error("model %d has no fused pre-split prologue", model); return B200KGE_ERR_UNSUPPORTED;
+    }
+  } else {
+    switch (model) {
+      B2K_PS(B200KGE_COMPLEX) B2K_PS(B200KGE_DISTMULT) B2K_PS(B200KGE_SIMPLE) B2K_PS(B200KGE_RESCAL)
+      default: set_error("model %d has no fused pre-split prologue", model); return B200KGE_ERR_UNSUPPORTED;
+    }
   }
 #undef B2K_PS
+#undef B2K_PS_R
   B2K_LAUNCH_CHECK("prep_split_1vsall_kernel");
   return 0;
 }

@@ -439,9 +439,10 @@ struct SplitSet {
 };
 int launch_presplit(const SplitSet& A, const SplitSet& B, cudaStream_t st);   // B.rows may be 0
 // fold + split of the 2n stacked query rows of a 1vsAll batch AND the split of the table, labels, ticket: one launch
+// (num_rel > 0: the reciprocal layout of launch_prep_1vsall)
 int launch_prep_split_1vsall(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n,
                              const SplitSet& Qs, const SplitSet& Ts, int64_t* labels2n, unsigned int* ticket,
-                             cudaStream_t st);
+                             cudaStream_t st, int64_t num_rel = 0);
 int launch_pairwise_tc3(int epi_kind, const SplitSet& Q, const SplitSet& T, const EpiParams& P, cudaStream_t st);
 
 // Backward pieces (grad.cu), experimental.
@@ -459,9 +460,10 @@ int launch_div_scores(const float* g, int64_t ldg, const float* z, int64_t ldz, 
                       cudaStream_t st);
 int launch_row_lse(const float* z, int64_t ldz, int64_t nq, int64_t E, const int64_t* label_idx, float* row_stat,
                    cudaStream_t st);
+// num_rel > 0 (dir < 0 only): the reciprocal layout, rows [n,2n) unfold as sp_ into d_ent[o], d_rel[p + num_rel]
 int launch_unfold_distance(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n, int dir,
                            const float* dQ, int64_t ldq, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                           cudaStream_t st);
+                           cudaStream_t st, int64_t num_rel = 0);
 int launch_grad_planes_csr(const float* z, int64_t ldz, int64_t nq, int64_t E, const int64_t* csr_off,
                            const int64_t* csr_col, float a, float b, float* row_stat, float offset, float inv_n,
                            void* g_hi, void* g_lo, int64_t Ep, void* gt_hi, void* gt_lo, int64_t Np, float* g_scale,
@@ -487,6 +489,7 @@ int launch_penalty(const Rows& tab, const float* counts, float p, int complex_ab
                    size_t scratch_floats, float* out, cudaStream_t st);
 int launch_normalize_rows(float* w, int64_t ld, int64_t rows, int dim, float p, cudaStream_t st);
 int launch_unfold(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n, int dir,
-                  const float* dQ, int64_t ldq, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, cudaStream_t st);
+                  const float* dQ, int64_t ldq, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, cudaStream_t st,
+                  int64_t num_rel = 0);
 
 }  // namespace b200kge

@@ -578,6 +578,50 @@ def train_1vsall_backward(model: str, ent, rel, triples, loss: str = "bce", offs
     return d_ent, d_rel
 
 
+def train_1vsall_reciprocal_forward(model: str, ent, rel, triples, num_relations: int, loss: str = "bce",
+                                    offset: float = 0.0, l_norm: float = 1.0, precision: str = "auto",
+                                    dropout: Optional["DropoutKey"] = None):
+    """The 1vsAll step of a reciprocal-relations model (rel holds 2 * num_relations rows): 0-d
+    (loss(score_sp(s, p), o) + loss(score_sp(o, p + R), s)) / n  (reciprocal_relations_model.py:85-92), with the
+    embedding-dropout draws of `dropout` (direction 1 on the _po streams) — b200kge_train_1vsall_reciprocal_forward."""
+    _require_cuda(ent, rel, triples)
+    lib, k = _lib.load(), _Keep()
+    re_, rr = k.rows(ent), k.rows(rel)
+    tri = triples if (triples.dtype == torch.int64 and triples.is_contiguous()) else triples.long().contiguous()
+    n = tri.shape[0]
+    dev = ent.device
+    out = torch.empty((), dtype=torch.float32, device=dev)
+    ws = torch.empty(lib.b200kge_train_1vsall_reciprocal_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1]),
+                     dtype=torch.uint8, device=dev)
+    drop = None if dropout is None else C.byref(dropout.struct())
+    _lib.check(lib.b200kge_train_1vsall_reciprocal_forward(
+        MODELS[model], l_norm, PREC[precision], C.byref(re_), C.byref(rr), int(num_relations), tri.data_ptr(), n,
+        LOSS[loss], offset, drop, out.data_ptr(), ws.data_ptr(), ws.numel(), _stream(dev)))
+    return out
+
+
+def train_1vsall_reciprocal_backward(model: str, ent, rel, triples, num_relations: int, loss: str = "bce",
+                                     offset: float = 0.0, l_norm: float = 1.0, dropout: Optional["DropoutKey"] = None):
+    """(d_ent, d_rel): dense table gradients (all 2R relation rows) of train_1vsall_reciprocal_forward's loss, under the
+    forward's masks when `dropout` is the forward's key (dot family; TransE L1/L2; RotatE L1)."""
+    _require_cuda(ent, rel, triples)
+    lib, k = _lib.load(), _Keep()
+    re_, rr = k.rows(ent), k.rows(rel)
+    tri = triples if (triples.dtype == torch.int64 and triples.is_contiguous()) else triples.long().contiguous()
+    n = tri.shape[0]
+    dev = ent.device
+    d_ent = torch.empty_like(_f32(ent))
+    d_rel = torch.empty_like(_f32(rel))
+    ws = torch.empty(lib.b200kge_train_1vsall_reciprocal_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1]),
+                     dtype=torch.uint8, device=dev)
+    drop = None if dropout is None else C.byref(dropout.struct())
+    _lib.check(lib.b200kge_train_1vsall_reciprocal_backward(
+        MODELS[model], l_norm, C.byref(re_), C.byref(rr), int(num_relations), tri.data_ptr(), n, LOSS[loss], offset,
+        drop, d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0), ws.data_ptr(), ws.numel(),
+        _stream(dev)))
+    return d_ent, d_rel
+
+
 def score_1vsN_backward(model: str, combine: str, ent, rel, q, p, grad_scores, l_norm: float = 1.0):
     """(d_ent, d_rel) of a dense [n, E] score block given dL/dscores (fresh tensors): dot family (tensor cores), TransE
     L1 / L2 and RotatE L1 (row-gradient kernel)."""
@@ -601,9 +645,9 @@ def score_1vsN_backward(model: str, combine: str, ent, rel, q, p, grad_scores, l
 
 def score_1vsN_loss_csr_backward(model: str, combine: str, ent, rel, q, p, csr_offsets, csr_cols, loss: str = "kl",
                                  offset: float = 0.0, label_smoothing: float = 0.0, batch_size: Optional[int] = None,
-                                 dropout: Optional["DropoutKey"] = None):
+                                 dropout: Optional["DropoutKey"] = None, dropout_streams: Optional[str] = None):
     """(d_ent, d_rel) of score_1vsN_loss_csr(...) / batch_size over the whole entity table (dot family), with the
-    forward's dropout masks when `dropout` is the forward's key."""
+    forward's dropout masks when `dropout` is the forward's key (and `dropout_streams` the forward's)."""
     _require_cuda(ent, rel, csr_offsets, csr_cols)
     lib, k = _lib.load(), _Keep()
     re_, rr = k.rows(ent), k.rows(rel)
@@ -615,6 +659,14 @@ def score_1vsN_loss_csr_backward(model: str, combine: str, ent, rel, q, p, csr_o
     if dropout is not None:
         ws = torch.empty(lib.b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(
             MODELS[model], n, ent.shape[0], ent.shape[1], int(cols.numel())), dtype=torch.uint8, device=dev)
+        if dropout_streams is not None:
+            _lib.check(lib.b200kge_score_1vsN_loss_csr_backward_dropout_dir(
+                MODELS[model], SP_ if combine == "sp_" else _PO, SP_ if dropout_streams == "sp_" else _PO,
+                C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(),
+                cols.data_ptr() if cols.numel() else None, label_smoothing, LOSS[loss], offset, batch_size or n,
+                C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0),
+                ws.data_ptr(), ws.numel(), _stream(dev)))
+            return d_ent, d_rel
         _lib.check(lib.b200kge_score_1vsN_loss_csr_backward_dropout(
             MODELS[model], SP_ if combine == "sp_" else _PO, C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n,
             offs.data_ptr(), cols.data_ptr() if cols.numel() else None, label_smoothing, LOSS[loss], offset,
@@ -769,10 +821,13 @@ def ns_loss(scores, loss: str, arg: float = 0.0, temperature: float = 1.0, label
 
 def score_1vsN_loss_csr(model: str, combine: str, q_tab, rel, cand_tab, csr_offsets, csr_cols, q=None, p=None,
                           loss: str = "kl", offset: float = 0.0, label_smoothing: float = 0.0, l_norm: float = 1.0,
-                          precision: str = "auto", return_rows: bool = False, dropout: Optional["DropoutKey"] = None):
+                          precision: str = "auto", return_rows: bool = False, dropout: Optional["DropoutKey"] = None,
+                          dropout_streams: Optional[str] = None):
     """KvsAll loss (sum over rows) with CSR multi-hot labels — see b200kge_score_1vsN_loss_csr.  With `dropout` the three
     embedding-dropout draws of the query type are applied (b200kge_score_1vsN_loss_csr_dropout): the queries are rows
-    q of the entity table q_tab, which must also be the candidate table."""
+    q of the entity table q_tab, which must also be the candidate table.  `dropout_streams` ("sp_" | "_po") draws the
+    masks of that query type instead of `combine`'s (a reciprocal-relations model's _po queries: combine "sp_",
+    streams "_po"; b200kge_score_1vsN_loss_csr_dropout_dir)."""
     _require_cuda(q_tab, rel, cand_tab, csr_offsets, csr_cols)
     lib, k = _lib.load(), _Keep()
     rq, rp, rc = k.rows(q_tab, q), k.rows(rel, p), k.rows(cand_tab)
@@ -790,6 +845,13 @@ def score_1vsN_loss_csr(model: str, combine: str, q_tab, rel, cand_tab, csr_offs
         k.refs += [qi, pi]
         ws = torch.empty(lib.b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(MODELS[model], n, m, rq.dim, nnz),
                          dtype=torch.uint8, device=dev)
+        if dropout_streams is not None:
+            _lib.check(lib.b200kge_score_1vsN_loss_csr_dropout_dir(
+                MODELS[model], SP_ if combine == "sp_" else _PO, SP_ if dropout_streams == "sp_" else _PO, l_norm,
+                PREC[precision], C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(),
+                cols.data_ptr() if nnz else None, nnz, label_smoothing, LOSS[loss], offset, C.byref(dropout.struct()),
+                out.data_ptr(), rows.data_ptr() if rows is not None else None, ws.data_ptr(), ws.numel(), _stream(dev)))
+            return (out, rows) if return_rows else out
         _lib.check(lib.b200kge_score_1vsN_loss_csr_dropout(
             MODELS[model], SP_ if combine == "sp_" else _PO, l_norm, PREC[precision], C.byref(re_), C.byref(rr),
             qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(), cols.data_ptr() if nnz else None, nnz, label_smoothing,

@@ -129,10 +129,13 @@ class _Loss1vsAllFn(torch.autograd.Function):
     (engine.DropoutKey) the step applies embedding dropout and the backward regenerates the same masks from the key."""
 
     @staticmethod
-    def forward(ctx, ent_w, rel_w, model, triples, loss, offset, dropout=None):
-        ctx.model, ctx.loss, ctx.offset, ctx.dropout = model, loss, offset, dropout
+    def forward(ctx, ent_w, rel_w, model, triples, loss, offset, dropout=None, reciprocal=None):
+        ctx.model, ctx.loss, ctx.offset, ctx.dropout, ctx.reciprocal = model, loss, offset, dropout, reciprocal
         ctx.save_for_backward(ent_w, rel_w, triples)
         ln, prec = model._b200_args()
+        if reciprocal is not None:
+            return engine.train_1vsall_reciprocal_forward(model._b200_name, ent_w.detach(), rel_w.detach(), triples,
+                                                          reciprocal, loss, offset, ln, prec, dropout=dropout)
         kw = {} if dropout is None else {"dropout": dropout}
         return engine.train_1vsall_forward(model._b200_name, ent_w.detach(), rel_w.detach(), triples, loss, offset,
                                            ln, prec, **kw)
@@ -140,8 +143,13 @@ class _Loss1vsAllFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         ent_w, rel_w, triples = ctx.saved_tensors
-        d_ent, d_rel = ctx.model._b200_loss_1vsall_backward(ent_w, rel_w, triples, ctx.loss, ctx.offset, ctx.dropout)
-        return d_ent * g, d_rel * g, None, None, None, None, None
+        if ctx.reciprocal is not None:
+            d_ent, d_rel = engine.train_1vsall_reciprocal_backward(
+                ctx.model._b200_name, ent_w.detach(), rel_w.detach(), triples, ctx.reciprocal, ctx.loss, ctx.offset,
+                ctx.model._b200_args()[0], dropout=ctx.dropout)
+        else:
+            d_ent, d_rel = ctx.model._b200_loss_1vsall_backward(ent_w, rel_w, triples, ctx.loss, ctx.offset, ctx.dropout)
+        return d_ent * g, d_rel * g, None, None, None, None, None, None
 
 
 def _penalty_torch(emb, w, regularize, rw, p, weighted, indexes):
@@ -223,22 +231,27 @@ class _KvsAllLossFn(torch.autograd.Function):
     the dropout entry points under the same masks."""
 
     @staticmethod
-    def forward(ctx, ent_w, rel_w, model, combine, a, p, offs, cols, loss, offset, smoothing, batch_size, dropout=None):
-        ctx.args = (model, combine, loss, offset, smoothing, batch_size, dropout)
+    def forward(ctx, ent_w, rel_w, model, combine, a, p, offs, cols, loss, offset, smoothing, batch_size, dropout=None,
+                dropout_streams=None):
+        ctx.args = (model, combine, loss, offset, smoothing, batch_size, dropout, dropout_streams)
         ctx.save_for_backward(ent_w, rel_w, a, p, offs, cols)
         ln, prec = model._b200_args()
         kw = {} if dropout is None else {"dropout": dropout}
+        if dropout_streams is not None:
+            kw["dropout_streams"] = dropout_streams
         return engine.score_1vsN_loss_csr(model._b200_name, combine, ent_w.detach(), rel_w.detach(), ent_w.detach(), offs,
                                           cols, a, p, loss, offset, smoothing, ln, prec, **kw) / batch_size
 
     @staticmethod
     def backward(ctx, g):
         ent_w, rel_w, a, p, offs, cols = ctx.saved_tensors
-        model, combine, loss, offset, smoothing, batch_size, dropout = ctx.args
+        model, combine, loss, offset, smoothing, batch_size, dropout, dropout_streams = ctx.args
         kw = {} if dropout is None else {"dropout": dropout}
+        if dropout_streams is not None:
+            kw["dropout_streams"] = dropout_streams
         d_ent, d_rel = engine.score_1vsN_loss_csr_backward(model._b200_name, combine, ent_w.detach(), rel_w.detach(), a, p,
                                                            offs, cols, loss, offset, smoothing, batch_size, **kw)
-        return (d_ent * g, d_rel * g) + (None,) * 11
+        return (d_ent * g, d_rel * g) + (None,) * 12
 
 
 class _NsSlotLossFn(torch.autograd.Function):
@@ -454,12 +467,20 @@ class _B200ModelMixin:
         return self._b200_call("sp_po", torch.cat((s.reshape(-1), o.reshape(-1))), p, entity_subset)
 
     # -- fused forms for the job plugins (kge_b200/plugin/jobs.py): scores never reach HBM
-    def loss_1vsall(self, triples, loss="bce", offset=0.0, need_grad=None, dropout=None):
+    def loss_1vsall(self, triples, loss="bce", offset=0.0, need_grad=None, dropout=None, reciprocal=None):
         """(loss(score_sp, o) + loss(score_po, s)) / n for a [n,3] batch (train_1vsAll.py:48-82); `dropout` (an
-        engine.DropoutKey) applies embedding dropout with the masks of that key."""
+        engine.DropoutKey) applies embedding dropout with the masks of that key.  `reciprocal` = R when this model is
+        the base model of a ReciprocalRelationsModel (2R relation rows): score_po is then the sp_ query (o, p + R)
+        (reciprocal_relations_model.py:85-92).  The reciprocal step has the native backward only."""
         ent_w, rel_w = self._b200_weights()
         if need_grad is None:
             need_grad = self._b200_needs_grad()
+        if reciprocal is not None:
+            if need_grad and self._b200_needs_grad():
+                return _Loss1vsAllFn.apply(ent_w, rel_w, self, triples, loss, offset, dropout, int(reciprocal))
+            ln, prec = self._b200_args()
+            return engine.train_1vsall_reciprocal_forward(self._b200_name, ent_w.detach(), rel_w.detach(), triples,
+                                                          int(reciprocal), loss, offset, ln, prec, dropout=dropout)
         if need_grad and self._b200_needs_grad():
             return _Loss1vsAllFn.apply(ent_w, rel_w, self, triples, loss, offset, dropout)
         if dropout is not None:
@@ -485,12 +506,16 @@ class _B200ModelMixin:
         return self._b200_prepared_step(ent_w, rel_w, triples_host.shape[0], loss, offset).call_host(triples_host)
 
     def loss_kvsall(self, combine, a, p, csr_offsets, csr_cols, loss="kl", offset=0.0, label_smoothing=0.0,
-                    dropout=None):
+                    dropout=None, dropout_streams=None):
         """Sum over rows of the KvsAll loss with CSR multi-hot labels (train_KvsAll.py:242-294); forward only.
-        `dropout` (an engine.DropoutKey) applies embedding dropout with the masks of that key."""
+        `dropout` (an engine.DropoutKey) applies embedding dropout with the masks of that key, drawn on the streams of
+        query type `dropout_streams` (default: `combine`'s; a reciprocal-relations _po query is the sp_ fold of
+        (o, p + R) on the _po streams)."""
         ent, rel = self._b200_tables()
         ln, prec = self._b200_args()
         kw = {} if dropout is None else {"dropout": dropout}
+        if dropout is not None and dropout_streams is not None:
+            kw["dropout_streams"] = dropout_streams
         return engine.score_1vsN_loss_csr(self._b200_name, combine, ent, rel, ent, csr_offsets, csr_cols, a, p,
                                           loss, offset, label_smoothing, ln, prec, **kw)
 
@@ -498,12 +523,12 @@ class _B200ModelMixin:
         return self.b200_backward == "native" and self._b200_name in ("complex", "distmult", "simple", "cp", "rescal")
 
     def loss_kvsall_train(self, combine, a, p, csr_offsets, csr_cols, loss, offset, label_smoothing, batch_size,
-                          dropout=None):
+                          dropout=None, dropout_streams=None):
         """loss_kvsall / batch_size as a differentiable scalar (train_KvsAll.py:286-294)."""
         ent_w, rel_w = self._b200_weights()
         return _KvsAllLossFn.apply(ent_w, rel_w, self, combine, a.long().contiguous(), p.long().contiguous(),
                                    csr_offsets, csr_cols, loss, float(offset), float(label_smoothing), int(batch_size),
-                                   dropout)
+                                   dropout, None if dropout is None else dropout_streams)
 
     def score_negatives(self, triples, negatives, slot, dropout=None, implementation="batch"):
         """[n, 1+K]: the positive triple's score in column 0, its K corrupted versions after it

@@ -18,6 +18,10 @@ dropout entry points in the 1vsAll and KvsAll jobs (masks drawn on the device, k
 negative-sampling job with dropout keeps the reference step unless `user.b200_ns_dropout: true` opts into the dropout
 kernels: the option chooses which random stream supplies the masks (the library's Philox key instead of torch's
 generator), as `user.b200_device_sampling` does for the negatives.
+
+LibKGE's `reciprocal_relations_model` over a b200 base model takes the base model's fused and dropout forms too: the
+1vsAll reciprocal step, KvsAll's _po query type as the sp_ query (o, p + R), and the negative-sampling S slot as
+O-slot triples (o, p + R, s).  The P slot, `s_o` and negative-sampling dropout keep the reference's step.
 """
 from __future__ import annotations
 
@@ -29,6 +33,7 @@ from kge.job.train_1vsAll import TrainingJob1vsAll
 from kge.job.train_KvsAll import TrainingJobKvsAll
 from kge.job.train_negative_sampling import TrainingJobNegativeSampling
 from kge.job import Job
+from kge.model.reciprocal_relations_model import ReciprocalRelationsModel
 from kge.util.loss import (BCEWithLogitsKgeLoss, KLDivWithSoftmaxKgeLoss, MarginRankingKgeLoss, SEKgeLoss,
                            SoftMarginKgeLoss)
 
@@ -81,6 +86,18 @@ def _dropout_model(model):
         return None, None
     rates = model.b200_dropout_rates()
     return (model, rates) if rates is not None else (None, None)
+
+
+def _reciprocal_base(model):
+    """(base model, R) for a LibKGE ReciprocalRelationsModel whose base model is a b200 model, else (None, None).  Its
+    score_po is the base model's sp_ query (o, p + R) against the same table (reciprocal_relations_model.py:85-92), so
+    the fused and dropout forms of the base model serve both directions; R = dataset.num_relations()."""
+    if type(model) is not ReciprocalRelationsModel:
+        return None, None
+    base = getattr(model, "_base_model", None)
+    if getattr(base, "_b200_name", None) is None or not hasattr(base, "b200_fusable"):
+        return None, None
+    return base, int(model.dataset.num_relations())
 
 
 def dropout_call(epoch, batch_index, ordinal):
@@ -178,20 +195,24 @@ class B200TrainingJob1vsAll(_DropoutKeys, _BatchSplit, TrainingJob1vsAll):
         subbatch_slice = self._b200_my_rows(subbatch_slice, result.size)
         if subbatch_slice is None:
             return
-        model, kind = _fused_model(self.model), _fused_loss_kind(self.loss)
+        base, recip = _reciprocal_base(self.model)
+        target = self.model if base is None else base
+        model, kind = _fused_model(target), _fused_loss_kind(self.loss)
         rates = None
         if model is None:
-            model, rates = _dropout_model(self.model)
+            model, rates = _dropout_model(target)
             if model is not None and not self.is_forward_only and not model.b200_1vsall_native_backward_ok():
                 model = None
+        elif recip is not None and not self.is_forward_only and not model.b200_1vsall_native_backward_ok():
+            model = None                # the reciprocal step has no recompute backward
         if model is None or kind is None:
             return super()._process_subbatch(batch_index, batch, subbatch_slice, result)
         batch_size = result.size
         drop = None if rates is None else self._b200_dropout_key(rates, batch_index, subbatch_slice)
 
         host = batch["triples"][subbatch_slice]
-        if (drop is None and self.is_forward_only and not host.is_cuda and host.dtype == torch.int64 and host.is_contiguous()
-                and len(host) > 0):
+        if (drop is None and recip is None and self.is_forward_only and not host.is_cuda and host.dtype == torch.int64
+                and host.is_contiguous() and len(host) > 0):
             # forward only: batch copy, kernels and the scalar read-back in ONE library call (no torch ops in between)
             result.forward_time -= time.time()
             value = model.loss_1vsall_host(host, kind[0], kind[1])
@@ -209,6 +230,8 @@ class B200TrainingJob1vsAll(_DropoutKeys, _BatchSplit, TrainingJob1vsAll):
         # sum over both directions and all rows of the sub-batch, divided by the sub-batch size by the kernel's
         # finaliser; the reference divides by the size of the whole batch (train_1vsAll.py:65,76)
         kw = {} if drop is None else {"dropout": drop}
+        if recip is not None:
+            kw["reciprocal"] = recip
         loss_value = model.loss_1vsall(triples, kind[0], kind[1], need_grad=not self.is_forward_only, **kw)
         if len(triples) != batch_size:
             loss_value = loss_value * (len(triples) / batch_size)
@@ -236,10 +259,12 @@ class B200TrainingJobKvsAll(_DropoutKeys, _BatchSplit, TrainingJobKvsAll):
         subbatch_slice = self._b200_my_rows(subbatch_slice, result.size)
         if subbatch_slice is None:
             return
-        model, kind = _fused_model(self.model), _fused_loss_kind(self.loss)
+        base, recip = _reciprocal_base(self.model)
+        target = self.model if base is None else base
+        model, kind = _fused_model(target), _fused_loss_kind(self.loss)
         rates = None
         if model is None:
-            model, rates = _dropout_model(self.model)
+            model, rates = _dropout_model(target)
         qtypes = [q for q in self.query_types]
         if (model is None or kind is None or "s_o" in qtypes or not model.b200_csr_labels_ok(self.label_smoothing)
                 or (not self.is_forward_only and not model.b200_kvsall_native_backward_ok())):
@@ -280,16 +305,22 @@ class B200TrainingJobKvsAll(_DropoutKeys, _BatchSplit, TrainingJobKvsAll):
 
             result.forward_time -= time.time()
             # sp_ queries are (s, p) pairs, _po queries are (p, o) pairs (indexing.py:197-235)
+            qkw = kw
             if query_type == "sp_":
                 combine, ent_idx, rel_idx = "sp_", queries[examples, 0], queries[examples, 1]
+            elif recip is not None:
+                # reciprocal relations: the sp_ query (o, p + R), masks on the _po streams
+                combine, ent_idx, rel_idx = "sp_", queries[examples, 1], queries[examples, 0] + recip
+                if rates is not None:
+                    qkw = dict(kw, dropout_streams="_po")
             else:
                 combine, ent_idx, rel_idx = "_po", queries[examples, 1], queries[examples, 0]
             if self.is_forward_only:
                 loss_value = model.loss_kvsall(combine, ent_idx, rel_idx, offsets, ccols, kind[0], kind[1],
-                                               self.label_smoothing, **kw) / batch_size
+                                               self.label_smoothing, **qkw) / batch_size
             else:
                 loss_value = model.loss_kvsall_train(combine, ent_idx, rel_idx, offsets, ccols, kind[0], kind[1],
-                                                     self.label_smoothing, batch_size, **kw)
+                                                     self.label_smoothing, batch_size, **qkw)
             result.avg_loss += loss_value.item()
             result.forward_time += time.time()
             result.backward_time -= time.time()
@@ -364,13 +395,25 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
         subbatch_slice = self._b200_my_rows(subbatch_slice, result.size)
         if subbatch_slice is None:
             return
-        model = _fused_model(self.model)
         kind = _ns_loss_kind(self.loss)
         slots = [sl for sl in (S, P, O) if self._sampler.num_samples[sl] > 0]
+        base, recip = _reciprocal_base(self.model)
+        if base is None:
+            model = _fused_model(self.model)
+        else:
+            # reciprocal relations: the S slot scores (o, p + R, s') through the O-slot kernels
+            # (reciprocal_relations_model.py:74-78); the P slot falls through (the reference raises there), and so
+            # does embedding dropout (the NS dropout kernels do not serve the wrapper)
+            model = _fused_model(base) if P not in slots else None
+            if model is None and self._device_sampling:
+                why = ("the P slot is not served" if P in slots else
+                       "embedding dropout is not served" if base.b200_dropout_rates() is not None else
+                       "the base model's tables cannot be read in place")
+                raise NotImplementedError(f"user.b200_device_sampling with reciprocal_relations_model: {why}")
         trainable = (model is not None and kind is not None
-                     and all(model.b200_ns_native_backward_ok(sl) for sl in slots))
+                     and all(model.b200_ns_native_backward_ok(O if recip is not None else sl) for sl in slots))
         drop = None
-        if model is None:
+        if model is None and base is None:
             model, rates = self._b200_ns_dropout_route(kind, slots)
             if model is not None:
                 # one key per sub-batch; the S and O slots draw disjoint mask streams under it
@@ -405,12 +448,15 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
                 negatives = negs[slot][subbatch_slice]
             else:
                 negatives = negs[slot].samples(subbatch_slice if (subbatch_size != batch_size) else None)
+            tri, kslot = triples, slot
+            if recip is not None and slot == S:
+                tri, kslot = torch.stack((triples[:, 2], triples[:, 1] + recip, triples[:, 0]), dim=1), O
             result.prepare_time += time.time()
 
             result.forward_time -= time.time()
             if not self.is_forward_only:
                 # training: forward + the fused NS gradient kernel behind one autograd node
-                loss_value = model.loss_negatives(triples, negatives.to(self.device), slot, kind[1], batch_size,
+                loss_value = model.loss_negatives(tri, negatives.to(self.device), kslot, kind[1], batch_size,
                                                   kind[0], kind[2], **dkw)
                 result.avg_loss += loss_value.item()
                 result.forward_time += time.time()
@@ -418,7 +464,7 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
                 loss_value.backward()
                 result.backward_time += time.time()
                 continue
-            scores = model.score_negatives(triples, negatives.to(self.device), slot, **dkw)  # [n, 1+K], positive first
+            scores = model.score_negatives(tri, negatives.to(self.device), kslot, **dkw)  # [n, 1+K], positive first
             if kind is not None and kind[0] == "bce":
                 # labels are 1 in column 0 and 0 elsewhere (train_negative_sampling.py:128-137): index labels
                 lab = torch.zeros(subbatch_size, dtype=torch.int64, device=self.device)
