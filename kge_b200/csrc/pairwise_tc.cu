@@ -15,18 +15,26 @@
 //   MIXED   raw fp32 tiles, splitter warps derive bf16 hi / lo tiles: Q*T [tf32] + Ql16*Th16 + Qh16*Tl16 [bf16].
 // The reference is a true fp32 GEMM; single-pass TF32 misses the 1e-4 bar, the three split forms meet it.
 //
-// CTA = 3 (4 with splitters) warpgroups, one CTA per SM, persistent over (query tile, range of entity tiles):
-//   warpgroup 0   warp 0 lane 0: TMA producer
-//   warpgroups 1-2 consumers: warpgroup g owns query rows [64g, 64g+64) of the 128-row tile; wgmma m64n128 with the
-//                 fp32 accumulator in registers, then the accumulator goes to a shared-memory tile (one row per
-//                 thread) and the same warps run the epilogue: warp w of the group takes rows 32*(w&1) and
-//                 columns 64*(w>>1) of the 128-entity tile
+// CTA = 3 (4 with splitters) warpgroups, one CTA per SM, persistent over a contiguous range of the flattened work
+// items (query tile, entity tile[, K segment]): every CTA runs floor or ceil of items / SMs, so a range may straddle
+// query tiles.
+//   warpgroup 0   warp 0 lane 0: TMA producer (the warpgroup hands its registers to the consumers)
+//   warpgroups 1-2 consumers, wgmma m64n128 with the fp32 accumulator in registers; the epilogue runs on the
+//                 accumulator fragment itself (no shared-memory staging).
+//                 F16X3 / TF32, "ping-pong": warpgroup g owns whole 128x128 tiles (two accumulators), the CTA's tiles
+//                 g, g+2, g+4, ... of its range, so one warpgroup's epilogue runs under the other's wgmmas.
+//                 TF32X3 / MIXED (four warpgroups, 128 registers per thread): warpgroup g owns query rows [64g, +64)
+//                 of every tile.
 //   warpgroup 3   (TF32X3 / MIXED) splitters
-// Ring of NSTAGE stages of 64 KB; a stage is one K chunk of both operands in every plane the mode uses.
+// Ring of NSTAGE stages of 64 KB; a stage is one K chunk of both operands in every plane the mode uses.  Chunks are
+// consumed in ring order, which is also what hands the tensor cores from one ping-pong warpgroup to the other.
 //   full[s]    TMA bytes landed                              -> splitters, consumers
 //   split[s]   splitter warps wrote + fenced derived tiles    -> consumers
-//   empty[s]   every consumer warp's wgmmas on s retired      -> producer
-// While the consumers run the epilogue of tile i the producer already fills the ring for tile i+1.
+//   empty[s]   every consuming warp's wgmmas on s retired     -> producer
+// Loss rows: the per-row state is flushed once per (query tile, CTA) into slot 2j + h of the row: j = the CTA's place
+// among the CTAs covering the query tile, h = the consumer warpgroup (ping-pong) or the half of the lane quad (row
+// split).  The CTA that ends a query tile writes neutral states into the slots no CTA reached, so the finaliser sums
+// the same slots in the same order whatever the schedule.
 #include "tc_common.cuh"
 
 namespace b200kge {
@@ -35,42 +43,58 @@ namespace {
 
 enum Mode : int { MODE_F16X3 = 0, MODE_TF32 = 1, MODE_TF32X3 = 2, MODE_MIXED = 3 };
 
-constexpr int TM = 128;             // queries per tile (two consumer warpgroups x 64)
+constexpr int TM = 128;             // queries per tile
 constexpr int TN = 128;             // entities per tile (wgmma N)
-constexpr int NSTAGE = 2;
+constexpr int NSTAGE = 3;
 constexpr int STAGE_BYTES = 64 * 1024;
 constexpr int BOX_BYTES = 16 * 1024;        // one 128-row box of 128-byte rows
-constexpr int ACC_LD = TN + 1;              // padded row of the staged accumulator (conflict-free row-per-thread reads)
-constexpr int ACC_BYTES = TM * ACC_LD * 4;
-constexpr int EPI_WARPS = 8;
-using tc::STG_LD;
-constexpr int STG_BYTES = EPI_WARPS * 32 * STG_LD * 4;
-constexpr int SMEM_BYTES = 1024 /*align slack*/ + NSTAGE * STAGE_BYTES + ACC_BYTES + STG_BYTES + 256 /*barriers*/;
+// per-row loss / rank state of the consumers between tiles: 256 consumer threads x 4 rows x the largest RowState
+constexpr int STATE_BYTES = 256 * 4 * (int)sizeof(RowState<EPI_KL>);
+constexpr int SMEM_BYTES = 1024 /*align slack*/ + NSTAGE * STAGE_BYTES + 256 /*barriers*/ + STATE_BYTES;
 static_assert(SMEM_BYTES <= 227 * 1024, "exceeds the H100's 227 KB of shared memory per block");
 
 template <int MODE> struct ModeCfg {
   static constexpr bool SPLIT = MODE == MODE_TF32X3 || MODE == MODE_MIXED;
+  static constexpr bool PP = !SPLIT;                                              // ping-pong consumers
+  static constexpr int MH = PP ? 2 : 1;                                           // m64 accumulators per consumer
   static constexpr int NTHREADS = (SPLIT ? 4 : 3) * 128;
   static constexpr int TK = MODE == MODE_F16X3 ? 64 : 32;                        // K elements per chunk
   static constexpr uint32_t TX = MODE == MODE_F16X3 ? 4 * BOX_BYTES : 2 * BOX_BYTES;   // TMA bytes per stage
+  static constexpr uint32_t STAGE_CONSUMERS = PP ? 4 : 8;                        // warps releasing each stage
 };
 
 struct TcParams {
   int64_t nq, m;
   int nk;           // K chunks
-  int q_tiles, e_tiles, echunks;
+  int q_tiles, e_tiles;
   int ksplit;       // > 1: split-K GEMM mode (EPI_STORE only): the reduction is cut into `ksplit` segments of `kseg`
   int kseg;         //      K chunks; every (tile, segment) is its own work item and ADDS into the zeroed output
+  int64_t items;    // q_tiles * e_tiles * ksplit; CTA b runs items [b * items / grid, (b + 1) * items / grid)
+  int grid;
+  int nsl;          // slot pairs per row (EpiParams::nchunks = 2 * nsl)
   const float* q_scale;   // F16X3: [nq]
   const float* t_scale;   // F16X3: [m + 32], zero beyond m
   EpiParams epi;
 };
 
+struct Item { int qt, et, k0, k1; };
+__device__ __forceinline__ Item item_at(const TcParams& p, int64_t i) {
+  Item it;
+  int ks = 0;
+  if (p.ksplit > 1) { ks = (int)(i % p.ksplit); i /= p.ksplit; }
+  it.qt = (int)(i / p.e_tiles);
+  it.et = (int)(i - (int64_t)it.qt * p.e_tiles);
+  it.k0 = ks * p.kseg;
+  it.k1 = it.k0 + p.kseg < p.nk ? it.k0 + p.kseg : p.nk;
+  return it;
+}
+
 // Stage layout (byte offsets).  F16X3: Qh | Th | Ql | Tl.  Raw modes: Q | T | derived tiles:
 //   TF32X3: Ql (16 KB) | Tl (16 KB)      MIXED: Qh16 | Ql16 | Th16 | Tl16 (8 KB each, 64-byte rows)
+// h: which 64 query rows of the stage's 128
 template <int MODE>
-__device__ __forceinline__ void mma_chunk(float (&d)[64], uint32_t st, int g) {
-  const uint32_t a = st + (uint32_t)g * (BOX_BYTES / 2), b = st + BOX_BYTES;   // this warpgroup's 64 query rows
+__device__ __forceinline__ void mma_chunk(float (&d)[64], uint32_t st, int h) {
+  const uint32_t a = st + (uint32_t)h * (BOX_BYTES / 2), b = st + BOX_BYTES;
   if constexpr (MODE == MODE_F16X3) {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -90,13 +114,13 @@ __device__ __forceinline__ void mma_chunk(float (&d)[64], uint32_t st, int g) {
         ptx::wgmma_tf32(d, ptx::wg_desc_sw128(a + k * 32), ptx::wg_desc_sw128(b + 2 * BOX_BYTES + k * 32));
       }
     } else if constexpr (MODE == MODE_MIXED) {
-      const uint32_t h = st + 2 * BOX_BYTES + (uint32_t)g * (BOX_BYTES / 4);    // Qh16 rows of this warpgroup
-      const uint32_t l = h + BOX_BYTES / 2;                                      // Ql16
+      const uint32_t hq = st + 2 * BOX_BYTES + (uint32_t)h * (BOX_BYTES / 4);   // Qh16 rows of these 64 queries
+      const uint32_t lq = hq + BOX_BYTES / 2;                                    // Ql16
       const uint32_t th = st + 3 * BOX_BYTES, tl = th + BOX_BYTES / 2;           // Th16, Tl16
 #pragma unroll
       for (int k = 0; k < 2; ++k) {
-        ptx::wgmma_bf16(d, ptx::wg_desc_sw64(l + k * 32), ptx::wg_desc_sw64(th + k * 32));
-        ptx::wgmma_bf16(d, ptx::wg_desc_sw64(h + k * 32), ptx::wg_desc_sw64(tl + k * 32));
+        ptx::wgmma_bf16(d, ptx::wg_desc_sw64(lq + k * 32), ptx::wg_desc_sw64(th + k * 32));
+        ptx::wgmma_bf16(d, ptx::wg_desc_sw64(hq + k * 32), ptx::wg_desc_sw64(tl + k * 32));
       }
     }
   }
@@ -110,15 +134,14 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   using C = ModeCfg<MODE>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* accs = reinterpret_cast<float*>(smem + NSTAGE * STAGE_BYTES);
-  float* stg = reinterpret_cast<float*>(smem + NSTAGE * STAGE_BYTES + ACC_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NSTAGE * STAGE_BYTES + ACC_BYTES + STG_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NSTAGE * STAGE_BYTES);
   uint64_t* full = bars;                  // [NSTAGE]
   uint64_t* split = bars + NSTAGE;        // [NSTAGE]
   uint64_t* empty = bars + 2 * NSTAGE;    // [NSTAGE]
+  uint64_t* turn = bars + 3 * NSTAGE;     // [2] ping-pong: warpgroup g may start waiting on its next tile's chunks
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int total_work = prm.q_tiles * prm.echunks * prm.ksplit;
+  const int64_t i0 = (int64_t)blockIdx.x * prm.items / prm.grid, i1 = (int64_t)(blockIdx.x + 1) * prm.items / prm.grid;
 
   if (threadIdx.x == 0) {
     ptx::prefetch_tensormap(&tmQ);
@@ -130,46 +153,31 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     for (int s = 0; s < NSTAGE; ++s) {
       ptx::mbar_init(&full[s], 1);
       ptx::mbar_init(&split[s], 4);
-      ptx::mbar_init(&empty[s], EPI_WARPS);
+      ptx::mbar_init(&empty[s], C::STAGE_CONSUMERS);
     }
+    ptx::mbar_init(&turn[0], 1);
+    ptx::mbar_init(&turn[1], 1);
     ptx::fence_barrier_init();
   }
   __syncthreads();
 
-  int k0 = 0, k1 = prm.nk;      // K-chunk range of the current work item (split-K mode: one segment)
-  auto work_range = [&](int w, int& qt, int& et0, int& et1, int& ec) {
-    if (prm.ksplit > 1) {
-      const int ks = w % prm.ksplit;
-      w /= prm.ksplit;
-      k0 = ks * prm.kseg;
-      k1 = (k0 + prm.kseg < prm.nk) ? k0 + prm.kseg : prm.nk;
-    }
-    qt = w / prm.echunks;
-    ec = w - qt * prm.echunks;
-    const int base = prm.e_tiles / prm.echunks, rem = prm.e_tiles % prm.echunks;
-    et0 = ec * base + (ec < rem ? ec : rem);
-    et1 = et0 + base + (ec < rem ? 1 : 0);
-  };
-
-  if (warp == 0) {
+  if (warp < 4) {
     // ================================ TMA producer =========================================
-    if (lane == 0) {
+    if constexpr (C::PP) ptx::setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
       uint32_t c = 0;
-      for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
-        int qt, et0, et1, ec;
-        work_range(w, qt, et0, et1, ec);
-        for (int et = et0; et < et1; ++et) {
-          for (int kc = k0; kc < k1; ++kc, ++c) {
-            const int s = (int)(c % NSTAGE);
-            ptx::mbar_wait_bounded(&empty[s], ((c / NSTAGE) & 1) ^ 1);
-            uint8_t* sp = smem + s * STAGE_BYTES;
-            ptx::mbar_arrive_expect_tx(&full[s], C::TX);
-            ptx::tma_load_2d(sp, &tmQ, &full[s], kc * C::TK, qt * TM);
-            ptx::tma_load_2d(sp + BOX_BYTES, &tmT, &full[s], kc * C::TK, et * TN);
-            if constexpr (MODE == MODE_F16X3) {
-              ptx::tma_load_2d(sp + 2 * BOX_BYTES, &tmQl, &full[s], kc * C::TK, qt * TM);
-              ptx::tma_load_2d(sp + 3 * BOX_BYTES, &tmTl, &full[s], kc * C::TK, et * TN);
-            }
+      for (int64_t i = i0; i < i1; ++i) {
+        const Item it = item_at(prm, i);
+        for (int kc = it.k0; kc < it.k1; ++kc, ++c) {
+          const int s = (int)(c % NSTAGE);
+          ptx::mbar_wait_bounded(&empty[s], ((c / NSTAGE) & 1) ^ 1);
+          uint8_t* sp = smem + s * STAGE_BYTES;
+          ptx::mbar_arrive_expect_tx(&full[s], C::TX);
+          ptx::tma_load_2d(sp, &tmQ, &full[s], kc * C::TK, it.qt * TM);
+          ptx::tma_load_2d(sp + BOX_BYTES, &tmT, &full[s], kc * C::TK, it.et * TN);
+          if constexpr (MODE == MODE_F16X3) {
+            ptx::tma_load_2d(sp + 2 * BOX_BYTES, &tmQl, &full[s], kc * C::TK, it.qt * TM);
+            ptx::tma_load_2d(sp + 3 * BOX_BYTES, &tmTl, &full[s], kc * C::TK, it.et * TN);
           }
         }
       }
@@ -179,90 +187,139 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     if constexpr (C::SPLIT) {
       const int t = threadIdx.x - 12 * 32;
       uint32_t c = 0;
-      for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
-        int qt, et0, et1, ec;
-        work_range(w, qt, et0, et1, ec);
-        for (int et = et0; et < et1; ++et) {
-          for (int kc = k0; kc < k1; ++kc, ++c) {
-            const int s = (int)(c % NSTAGE);
-            ptx::mbar_wait_bounded(&full[s], (c / NSTAGE) & 1);
-            const uint32_t sp = ptx::smem_u32(smem + s * STAGE_BYTES);
-            if constexpr (MODE == MODE_TF32X3) {
-              tc::split_tile<BOX_BYTES, 128>(sp, sp + 2 * BOX_BYTES, t);
-              tc::split_tile<BOX_BYTES, 128>(sp + BOX_BYTES, sp + 3 * BOX_BYTES, t);
-            } else {
-              tc::split_tile_bf16<TM, 128>(sp, sp + 2 * BOX_BYTES, sp + 2 * BOX_BYTES + BOX_BYTES / 2, t);
-              tc::split_tile_bf16<TN, 128>(sp + BOX_BYTES, sp + 3 * BOX_BYTES, sp + 3 * BOX_BYTES + BOX_BYTES / 2, t);
-            }
-            ptx::fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&split[s]);
+      for (int64_t i = i0; i < i1; ++i) {
+        const Item it = item_at(prm, i);
+        for (int kc = it.k0; kc < it.k1; ++kc, ++c) {
+          const int s = (int)(c % NSTAGE);
+          ptx::mbar_wait_bounded(&full[s], (c / NSTAGE) & 1);
+          const uint32_t sp = ptx::smem_u32(smem + s * STAGE_BYTES);
+          if constexpr (MODE == MODE_TF32X3) {
+            tc::split_tile<BOX_BYTES, 128>(sp, sp + 2 * BOX_BYTES, t);
+            tc::split_tile<BOX_BYTES, 128>(sp + BOX_BYTES, sp + 3 * BOX_BYTES, t);
+          } else {
+            tc::split_tile_bf16<TM, 128>(sp, sp + 2 * BOX_BYTES, sp + 2 * BOX_BYTES + BOX_BYTES / 2, t);
+            tc::split_tile_bf16<TN, 128>(sp + BOX_BYTES, sp + 3 * BOX_BYTES, sp + 3 * BOX_BYTES + BOX_BYTES / 2, t);
           }
+          ptx::fence_proxy_async_smem();
+          __syncwarp();
+          if (lane == 0) ptx::mbar_arrive(&split[s]);
         }
       }
     }
-  } else if (warp >= 4) {
+  } else {
     // ================================ consumers: wgmma + epilogue ===========================
-    const int g = (warp - 4) >> 2;            // consumer warpgroup: query rows [64g, +64) of the tile
-    const int wl = warp & 3;                  // warp within the group
-    const int quad = wl & 1, half = wl >> 1;  // epilogue: rows [32*quad, +32) of the group, columns [64*half, +64)
-    const int tg = threadIdx.x & 127;
-    float* acc_g = accs + g * 64 * ACC_LD;
-    float* my_stg = stg + (warp - 4) * 32 * STG_LD;
+    if constexpr (C::PP) ptx::setmaxnreg_inc<232>();
+    const int g = (warp - 4) >> 2;            // consumer warpgroup
+    const int tg = threadIdx.x & 127, q = tg & 3;
+    // tile row of this thread's accumulator row rr: accumulator rr / 2, +8 for odd rr (fragment layout in ptx.cuh)
+    const int row_in_tile = (C::PP ? 0 : 64 * g) + 16 * (tg >> 5) + ((tg & 31) >> 2);
     const EpiParams& P = prm.epi;
-    uint32_t c = 0;
-    for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
-      int qt, et0, et1, ec;
-      work_range(w, qt, et0, et1, ec);
-      const int64_t tile_row0 = (int64_t)qt * TM + g * 64 + quad * 32;
-      const int64_t row = tile_row0 + lane;   // this thread's query row in the epilogue
-      const bool row_ok = row < prm.nq;
-      RowState<EPI> st;
-      st.init();
-      const float aux = row_ok ? epi_row_aux<EPI>(P, row) : 0.f;
-      const float qs = (MODE == MODE_F16X3 && row_ok) ? __ldg(prm.q_scale + row) : 0.f;
-      const int64_t csr_end = (P.csr_off && row_ok) ? __ldg(P.csr_off + row + 1) : 0;
-      for (int et = et0; et < et1; ++et) {
-        float d[64];
+    // Row state lives in shared memory between tiles (thread-private slots, stride 256 states), so it does not hold
+    // registers next to the accumulators during the main loop.
+    RowState<EPI>* st = reinterpret_cast<RowState<EPI>*>(smem + NSTAGE * STAGE_BYTES + 256) + (threadIdx.x - 128);
 #pragma unroll
-        for (int i = 0; i < 64; ++i) d[i] = 0.f;
-        for (int kc = k0; kc < k1; ++kc, ++c) {
-          const int s = (int)(c % NSTAGE);
-          ptx::mbar_wait_bounded(&full[s], (c / NSTAGE) & 1);
-          if constexpr (C::SPLIT) ptx::mbar_wait_bounded(&split[s], (c / NSTAGE) & 1);
+    for (int rr = 0; rr < 2 * C::MH; ++rr) st[256 * rr].init();
+    uint32_t c = 0;
+    for (int64_t i = i0; i < i1; ++i) {
+      const Item it = item_at(prm, i);
+      const int nkc = it.k1 - it.k0;
+      if (!C::PP || (int)((i - i0) & 1) == g) {
+        // Ping-pong: the k-th tile of warpgroup g waits until the other warpgroup has waited on every chunk of the
+        // tile before it.  Without this a warpgroup would wait on a full[] phase two ring passes ahead, and the
+        // parity wait would return on an earlier chunk.
+        const uint32_t k = (uint32_t)((i - i0) >> 1);
+        if (C::PP && (g == 1 || k > 0)) ptx::mbar_wait_bounded(&turn[g], (g == 1 ? k : k - 1) & 1);
+        float d[C::MH][64];
+#pragma unroll
+        for (int h = 0; h < C::MH; ++h)
+#pragma unroll
+          for (int e = 0; e < 64; ++e) d[h][e] = 0.f;
+        for (int kk = 0; kk < nkc; ++kk) {
+          const uint32_t cc = c + kk;
+          const int s = (int)(cc % NSTAGE);
+          ptx::mbar_wait_bounded(&full[s], (cc / NSTAGE) & 1);
+          if constexpr (C::SPLIT) ptx::mbar_wait_bounded(&split[s], (cc / NSTAGE) & 1);
           ptx::wg_fence();
-          mma_chunk<MODE>(d, ptx::smem_u32(smem + s * STAGE_BYTES), g);
+#pragma unroll
+          for (int h = 0; h < C::MH; ++h) mma_chunk<MODE>(d[h], ptx::smem_u32(smem + s * STAGE_BYTES), C::PP ? h : g);
           ptx::wg_commit();
-          if (kc > k0) {
+          if (kk > 0) {
             ptx::wg_wait<1>();                 // the previous chunk's wgmmas retired: release its stage
             __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&empty[(c - 1) % NSTAGE]);
+            if (lane == 0) ptx::mbar_arrive(&empty[(cc - 1) % NSTAGE]);
           }
         }
+        if (C::PP && tg == 0) ptx::mbar_arrive(&turn[g ^ 1]);   // this tile's chunks all landed: the other may go
         ptx::wg_wait<0>();
         __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&empty[(c - 1) % NSTAGE]);
-        // accumulator -> shared tile (one row per thread afterwards)
-        ptx::bar_sync(1 + g, 128);             // the previous tile's epilogue is done reading acc_g
-        {
-          const int r = 16 * (tg >> 5) + ((tg & 31) >> 2), cc = 2 * (tg & 3);
+        if (lane == 0) ptx::mbar_arrive(&empty[(c + nkc - 1) % NSTAGE]);
+
+        const int64_t e0 = (int64_t)it.et * TN;
+        if constexpr (MODE == MODE_F16X3) {
+          // score = acc * (row factor * column factor), both exact powers of two; one column pair at a time, so the
+          // factors do not hold registers next to the accumulators
+          float qs[2 * C::MH];
+#pragma unroll
+          for (int rr = 0; rr < 2 * C::MH; ++rr) {
+            const int64_t row = (int64_t)it.qt * TM + row_in_tile + 64 * (rr >> 1) + 8 * (rr & 1);
+            qs[rr] = row < prm.nq ? __ldg(prm.q_scale + row) : 0.f;
+          }
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
-            acc_g[r * ACC_LD + 8 * j + cc] = d[4 * j];
-            acc_g[r * ACC_LD + 8 * j + cc + 1] = d[4 * j + 1];
-            acc_g[(r + 8) * ACC_LD + 8 * j + cc] = d[4 * j + 2];
-            acc_g[(r + 8) * ACC_LD + 8 * j + cc + 1] = d[4 * j + 3];
+            const int64_t col = e0 + 2 * q + 8 * j;
+            const float2 ts = col < prm.m ? __ldg(reinterpret_cast<const float2*>(prm.t_scale + col)) : make_float2(0.f, 0.f);
+#pragma unroll
+            for (int rr = 0; rr < 2 * C::MH; ++rr) {
+              float* a = &d[rr >> 1][4 * j + 2 * (rr & 1)];
+              a[0] = a[0] * (qs[rr] * ts.x);
+              a[1] = a[1] * (qs[rr] * ts.y);
+            }
           }
         }
-        ptx::bar_sync(1 + g, 128);
-        const int64_t tile_end = (int64_t)(et + 1) * TN;
-        tc::epilogue_tile<EPI, 2, MODE == MODE_F16X3>(P, st, aux, acc_g + (quad * 32 + lane) * ACC_LD + half * 64,
-                                                      tile_row0, (int64_t)et * TN + half * 64, prm.nq,
-                                                      tile_end < prm.m ? tile_end : prm.m, my_stg, lane, qs,
-                                                      prm.t_scale, csr_end);
+#pragma unroll
+        for (int rr = 0; rr < 2 * C::MH; ++rr) {
+          const int64_t row = (int64_t)it.qt * TM + row_in_tile + 64 * (rr >> 1) + 8 * (rr & 1);
+          if (row < prm.nq) {
+            float v[32];
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+              v[2 * j] = d[rr >> 1][4 * j + 2 * (rr & 1)];
+              v[2 * j + 1] = d[rr >> 1][4 * j + 2 * (rr & 1) + 1];
+            }
+            RowState<EPI> rs = st[256 * rr];
+            tc::epi_row<EPI>(P, rs, v, row, e0, prm.m, q);
+            st[256 * rr] = rs;
+          }
+        }
       }
+      c += nkc;
       if constexpr (EPI != EPI_STORE) {
-        if (row_ok) epi_flush<EPI>(P, st, row, ec * 2 + half);
+        // losses and ranks never split K: item i is tile (i / e_tiles, i % e_tiles)
+        const bool ends_qt = (i + 1) % prm.e_tiles == 0;
+        if (ends_qt || i + 1 == i1) {
+          const int qt = (int)(i / prm.e_tiles);
+          const int64_t first = (((int64_t)qt * prm.e_tiles + 1) * prm.grid - 1) / prm.items;   // CTA of its 1st item
+          const int j = (int)(blockIdx.x - first);
+          const int h = C::PP ? g : (q >> 1);
+          const bool writer = C::PP ? q == 0 : (q & 1) == 0;
+#pragma unroll
+          for (int rr = 0; rr < 2 * C::MH; ++rr) {
+            RowState<EPI> rs = st[256 * rr];
+            epi_lane_reduce<EPI>(rs, C::PP ? 4 : 2);
+            const int64_t row = (int64_t)qt * TM + row_in_tile + 64 * (rr >> 1) + 8 * (rr & 1);
+            if (writer && row < prm.nq) {
+              epi_flush<EPI>(P, rs, row, 2 * j + h);
+              if constexpr (EPI != EPI_RANK) {
+                if (ends_qt) {
+                  RowState<EPI> z;
+                  z.init();
+                  for (int jj = j + 1; jj < prm.nsl; ++jj) epi_flush<EPI>(P, z, row, 2 * jj + h);
+                }
+              }
+            }
+            st[256 * rr].init();
+          }
+        }
       }
     }
   }
@@ -271,15 +328,19 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 // ---------------------------------------------------------------------------------------------
 using tc::num_sms;
 
-// entity tiles split into `echunks` ranges so that q_tiles * echunks ~ #SMs
-void plan(int64_t nq, int64_t m, int& q_tiles, int& e_tiles, int& echunks) {
-  q_tiles = (int)((nq + TM - 1) / TM);
-  if (q_tiles < 1) q_tiles = 1;
-  e_tiles = (int)((m + TN - 1) / TN);
-  int per = num_sms() / q_tiles;
-  if (per < 1) per = 1;
-  if (per > e_tiles) per = e_tiles;
-  echunks = per;
+// Flattened work items split into contiguous ranges over min(#SMs, items) CTAs.
+void schedule(int64_t nq, int64_t m, int ksplit, TcParams& prm) {
+  prm.q_tiles = (int)((nq + TM - 1) / TM);
+  if (prm.q_tiles < 1) prm.q_tiles = 1;
+  prm.e_tiles = (int)((m + TN - 1) / TN);
+  prm.ksplit = ksplit;
+  prm.items = (int64_t)prm.q_tiles * prm.e_tiles * ksplit;
+  prm.grid = prm.items < num_sms() ? (int)prm.items : num_sms();
+  // every range holds >= per items, so a query tile's e_tiles items meet at most ceil(e_tiles / per) + 1 ranges, and
+  // never more than there are CTAs: nsl <= #SMs keeps the partials within 2 * #SMs slots per row (the workspace size)
+  const int64_t per = prm.items / prm.grid;
+  const int64_t nsl = (prm.e_tiles + per - 1) / per + 1;
+  prm.nsl = nsl < prm.grid ? (int)nsl : prm.grid;
 }
 
 template <int EPI, int MODE>
@@ -287,10 +348,8 @@ int launch_k(const CUtensorMap (&maps)[4], const TcParams& prm, cudaStream_t st)
   auto kern = pairwise_tc_kernel<EPI, MODE>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(pairwise_tc_kernel)");
-  const int total = prm.q_tiles * prm.echunks * prm.ksplit;
-  const int grid = total < num_sms() ? total : num_sms();
   profile_begin(st);
-  kern<<<grid, ModeCfg<MODE>::NTHREADS, SMEM_BYTES, st>>>(maps[0], maps[1], maps[2], maps[3], prm);
+  kern<<<prm.grid, ModeCfg<MODE>::NTHREADS, SMEM_BYTES, st>>>(maps[0], maps[1], maps[2], maps[3], prm);
   profile_end(st);
   B2K_LAUNCH_CHECK("pairwise_tc_kernel");
   return 0;
@@ -320,9 +379,9 @@ bool tc_supported(int pair_op, int K, const Rows& cand, int col_off) {
 }
 
 int tc_nchunks(int64_t nq, int64_t m) {
-  int qt, et, ec;
-  plan(nq, m, qt, et, ec);
-  return 2 * ec;
+  TcParams prm;
+  schedule(nq, m, 1, prm);
+  return 2 * prm.nsl;
 }
 
 // in-kernel split of raw fp32 operands: passes 1 = TF32, 2 = MIXED, 3 = TF32X3
@@ -337,11 +396,11 @@ int launch_pairwise_tc(int epi_kind, int passes, const float* Q, int64_t ldq,
   maps[2] = maps[0]; maps[3] = maps[1];
   TcParams prm;
   prm.nq = nq; prm.m = m; prm.nk = (K + 31) / 32;
-  plan(nq, m, prm.q_tiles, prm.e_tiles, prm.echunks);
-  prm.ksplit = 1; prm.kseg = prm.nk;
+  schedule(nq, m, 1, prm);
+  prm.kseg = prm.nk;
   prm.q_scale = nullptr; prm.t_scale = nullptr;
   prm.epi = P;
-  prm.epi.nchunks = 2 * prm.echunks;   // two epilogue threads (column halves) per row
+  prm.epi.nchunks = 2 * prm.nsl;
   if (passes == 3) return launch_mode<MODE_TF32X3>(epi_kind, maps, prm, st);
   if (passes == 2) return launch_mode<MODE_MIXED>(epi_kind, maps, prm, st);
   return launch_mode<MODE_TF32>(epi_kind, maps, prm, st);
@@ -354,17 +413,14 @@ int launch_pairwise_tc3(int epi_kind, const SplitSet& Q, const SplitSet& T, cons
   if (Q.Kp != T.Kp || Q.Kp % 64 != 0) { set_error("operand planes disagree on the padded reduction length"); return B200KGE_ERR_INVALID; }
   TcParams prm;
   prm.nq = nq; prm.m = m; prm.nk = Q.Kp / 64;
-  plan(nq, m, prm.q_tiles, prm.e_tiles, prm.echunks);
-  prm.ksplit = 1; prm.kseg = prm.nk;
+  prm.kseg = prm.nk;
   if (P.accumulate_out) {
     // split-K GEMM: segments of 8 chunks (512 reduction elements) bound the tensor core's accumulator error, which
-    // grows with the reduction length; segment results are added in fp32 by the epilogue (red.global.add).  One
-    // entity tile per work item.
+    // grows with the reduction length; segment results are added in fp32 by the epilogue (red.global.add).
     if (epi_kind != EPI_STORE) { set_error("split-K accumulation is a GEMM (store) mode"); return B200KGE_ERR_INVALID; }
     prm.kseg = 8;
-    prm.ksplit = (prm.nk + prm.kseg - 1) / prm.kseg;
-    prm.echunks = prm.e_tiles;
   }
+  schedule(nq, m, (prm.nk + prm.kseg - 1) / prm.kseg, prm);
   prm.q_scale = Q.inv_scale; prm.t_scale = T.inv_scale;
   CUtensorMap maps[4];
   int rc;
@@ -373,7 +429,7 @@ int launch_pairwise_tc3(int epi_kind, const SplitSet& Q, const SplitSet& T, cons
   if ((rc = tc::make_map_f16(&maps[2], Q.lo, nq, Q.Kp, Q.Kp, TM))) return rc;
   if ((rc = tc::make_map_f16(&maps[3], T.lo, m, T.Kp, T.Kp, TN))) return rc;
   prm.epi = P;
-  prm.epi.nchunks = 2 * prm.echunks;
+  prm.epi.nchunks = 2 * prm.nsl;
   return launch_mode<MODE_F16X3>(epi_kind, maps, prm, st);
 }
 

@@ -8,8 +8,6 @@
 namespace b200kge {
 namespace tc {
 
-constexpr int STG_LD = 33;   // padded row of the per-warp transpose staging buffer
-
 __device__ __forceinline__ float tf32_rna(float x) {
   uint32_t u;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
@@ -105,10 +103,10 @@ __device__ __forceinline__ void split_tile_bf16(uint32_t src, uint32_t dst_hi, u
   }
 }
 
-// Epilogue.  The accumulator tile is staged in shared memory with one row per thread, so one thread owns
-// one query row and walks 32-column chunks; every per-row reduction is thread-local.  Warp-uniform fast
-// paths for full chunks, optional operands resolved once per chunk, the one-hot label handled outside the
-// element loop, and two threads per row (each takes half of the tile's columns).
+// Epilogue, straight from the wgmma accumulator fragment (layout in ptx.cuh).  The calling thread holds 32 scores of
+// one query row of a 128-column tile: v[2j + p] is column c0 + 8j + p (j < 16, p < 2) with c0 = tile start +
+// 2 * (lane % 4), so the four lanes of a quad together hold the row's 128 columns.  Per-row state stays lane-local
+// until the flush, which combines the quad's states (epi_lane_reduce) in a fixed order.  Columns >= m are skipped.
 
 constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
 
@@ -118,88 +116,96 @@ __device__ __forceinline__ float fast_ex2(float x) {
   return y;
 }
 
-// 32 columns [c0, c0+32) of row `row`; v = raw accumulator bits.  FULL: all 32 columns < m.
-// `side`: this row's 32 entries of the dense label matrix (BCE/KL) or of the filter matrix (rank),
-// already staged in shared memory by the warp (coalesced loads), or nullptr.
+// offset of fragment element k from the lane's first column
+__device__ __forceinline__ constexpr int frag_col(int k) { return 8 * (k >> 1) + (k & 1); }
+
+// fragment element holding tile column `tc` (0..127) if lane q of the quad holds it, else -1
+__device__ __forceinline__ int frag_elem(int tc, int q) {
+  return ((tc >> 1) & 3) == q ? 2 * (tc >> 3) + (tc & 1) : -1;
+}
+
+__device__ __forceinline__ float frag_get(const float (&v)[32], int k) {
+  float x = 0.f;
+#pragma unroll
+  for (int i = 0; i < 32; ++i)
+    if (i == k) x = v[i];
+  return x;
+}
+
+// FULL: all 128 columns of the tile are < m (then nvalid is not read)
 template <int EPI, bool FULL>
-__device__ __forceinline__ void epi_chunk32(const EpiParams& P, RowState<EPI>& st, int64_t row, float aux,
-                                            const uint32_t (&v)[32], int64_t c0, int64_t m,
-                                            const float* __restrict__ side) {
-  const int nvalid = FULL ? 32 : (int)(m - c0);   // > 0 by construction
+__device__ __forceinline__ void epi_row_body(const EpiParams& P, RowState<EPI>& st, const float (&v)[32], int64_t row,
+                                             int64_t e0, int64_t c0, int nvalid, int q) {
   if constexpr (EPI == EPI_BCE) {
     // sum softplus(z) - sum y*z,  softplus(z) = max(z,0) + log(1 + exp(-|z|))   (loss.py:150-157;
     // torch's kernel also evaluates log(1+e) with a plain log, so tiny e drop out identically)
     const float off = P.offset;
     float amax = 0.f, alg = 0.f;
 #pragma unroll
-    for (int c = 0; c < 32; ++c) {
-      if (FULL || c < nvalid) {
-        const float z = __uint_as_float(v[c]) + off;
+    for (int k = 0; k < 32; ++k) {
+      if (FULL || frag_col(k) < nvalid) {
+        const float z = v[k] + off;
         const float e = fast_ex2(-fabsf(z) * LOG2E);
         alg += __log2f(1.0f + e);
         amax += fmaxf(z, 0.f);
       }
     }
     st.a += fmaf(alg, LN2, amax);
-    if (side) {
+    if (P.label_dense) {
+      const float* __restrict__ y = P.label_dense + row * P.ldl + c0;
       float b = 0.f;
 #pragma unroll
-      for (int c = 0; c < 32; ++c)
-        if (FULL || c < nvalid) b = fmaf(side[c], __uint_as_float(v[c]) + off, b);
+      for (int k = 0; k < 32; ++k)
+        if (FULL || frag_col(k) < nvalid) b = fmaf(__ldg(y + frag_col(k)), v[k] + off, b);
       st.b += b;
-    } else {
-      const int rel = __float_as_int(aux) - (int)c0;      // one-hot label relative to this chunk
-      if ((unsigned)rel < (unsigned)nvalid) {
-#pragma unroll
-        for (int c = 0; c < 32; ++c)
-          if (c == rel) st.b += __uint_as_float(v[c]) + off;
-      }
+    } else if (P.label_idx) {
+      const int64_t lab = P.label_idx[row];
+      const int k = (lab >= e0 && lab < e0 + 128 && (FULL || lab - c0 < nvalid)) ? frag_elem((int)(lab - e0), q) : -1;
+      if (k >= 0) st.b += frag_get(v, k) + off;
     }
   } else if constexpr (EPI == EPI_KL) {
-    // online logsumexp: chunk max first, then ONE exp per element   (loss.py:198-213)
+    // online logsumexp: the lane's max first, then ONE exp per element   (loss.py:198-213)
     float cm = B2K_NEG_HUGE;
 #pragma unroll
-    for (int c = 0; c < 32; ++c)
-      if (FULL || c < nvalid) cm = fmaxf(cm, __uint_as_float(v[c]));
+    for (int k = 0; k < 32; ++k)
+      if (FULL || frag_col(k) < nvalid) cm = fmaxf(cm, v[k]);
     const float mn = fmaxf(st.m, cm);
     const float mn2 = mn * LOG2E;
     float acc = 0.f;
 #pragma unroll
-    for (int c = 0; c < 32; ++c)
-      if (FULL || c < nvalid) acc += fast_ex2(fmaf(__uint_as_float(v[c]), LOG2E, -mn2));
+    for (int k = 0; k < 32; ++k)
+      if (FULL || frag_col(k) < nvalid) acc += fast_ex2(fmaf(v[k], LOG2E, -mn2));
     st.s = fmaf(st.s, fast_ex2((st.m - mn) * LOG2E), acc);
     st.m = mn;
-    if (side) {
+    if (P.label_dense) {
+      const float* __restrict__ y = P.label_dense + row * P.ldl + c0;
 #pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        if (FULL || c < nvalid) {
-          const float yy = side[c];
+      for (int k = 0; k < 32; ++k) {
+        if (FULL || frag_col(k) < nvalid) {
+          const float yy = __ldg(y + frag_col(k));
           if (yy != 0.f) {
             st.y_sum += yy;
-            st.yx = fmaf(yy, __uint_as_float(v[c]), st.yx);
+            st.yx = fmaf(yy, v[k], st.yx);
             st.ylogy = fmaf(yy, __logf(yy), st.ylogy);
           }
         }
       }
-    } else {
-      const int rel = __float_as_int(aux) - (int)c0;
-      if ((unsigned)rel < (unsigned)nvalid) {
-#pragma unroll
-        for (int c = 0; c < 32; ++c)
-          if (c == rel) { st.y_sum += 1.0f; st.yx += __uint_as_float(v[c]); }
-      }
+    } else if (P.label_idx) {
+      const int64_t lab = P.label_idx[row];
+      const int k = (lab >= e0 && lab < e0 + 128 && (FULL || lab - c0 < nvalid)) ? frag_elem((int)(lab - e0), q) : -1;
+      if (k >= 0) { st.y_sum += 1.0f; st.yx += frag_get(v, k); }
     }
   } else if constexpr (EPI == EPI_RANK) {
     // eval_entity_ranking.py:561-596; `allowed` depends on the row only -> hoisted
-    const float t = aux;
+    const float t = epi_row_aux<EPI_RANK>(P, row);
     const float allowed = __fadd_rn(P.atol, fabsf(__fmul_rn(P.rtol, t)));
-    const float* __restrict__ f = side;
+    const float* __restrict__ f = P.filter ? P.filter + row * P.ldf + c0 : nullptr;
     unsigned int gt = 0, cl = 0;
 #pragma unroll
-    for (int c = 0; c < 32; ++c) {
-      if (FULL || c < nvalid) {
-        float x = __uint_as_float(v[c]);
-        if (f) x = __fsub_rn(x, f[c]);
+    for (int k = 0; k < 32; ++k) {
+      if (FULL || frag_col(k) < nvalid) {
+        float x = v[k];
+        if (f) x = __fsub_rn(x, __ldg(f + frag_col(k)));
         if (isnan(x)) x = -INFINITY;
         const float actual = fabsf(__fsub_rn(x, t));
         const bool close = (x == t) || (isfinite(actual) && actual <= allowed);
@@ -209,149 +215,70 @@ __device__ __forceinline__ void epi_chunk32(const EpiParams& P, RowState<EPI>& s
     }
     st.greater += gt;
     st.close += cl;
+  } else if constexpr (EPI == EPI_STORE) {
+    int64_t r = row, cb = 0;
+    if (P.n_rows_out > 0 && r >= P.n_rows_out) { r -= P.n_rows_out; cb = P.col_block; }   // sp|po seam
+    const int64_t at = r * P.ldo + cb + c0;
+    // a quad writes 32 contiguous bytes of the row per j: full sectors whatever the row stride is
+    auto put = [&](float* __restrict__ p) {
+      const bool vec = (reinterpret_cast<uintptr_t>(p) & 7) == 0;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        if (vec && (FULL || 8 * j + 1 < nvalid)) {
+          *reinterpret_cast<float2*>(p + 8 * j) = make_float2(v[2 * j], v[2 * j + 1]);
+        } else {
+          if (FULL || 8 * j < nvalid) p[8 * j] = v[2 * j];
+          if (FULL || 8 * j + 1 < nvalid) p[8 * j + 1] = v[2 * j + 1];
+        }
+      }
+    };
+    if (P.accumulate_out) {
+      float* __restrict__ p = P.out + at;
+#pragma unroll
+      for (int k = 0; k < 32; ++k)
+        if (FULL || frag_col(k) < nvalid) atomicAdd(p + frag_col(k), v[k]);
+    } else {
+      put(P.out + at);
+      for (int g = 0; g < P.n_peers; ++g) put(P.out_peer[g] + at);   // same offsets in the peers' symmetric buffers
+    }
   }
 }
 
-// Epilogue of NCH 32-column chunks of one accumulator tile for the warp owning 32 of its rows and columns
-// [col_first, col_first + 32*NCH); `acc` points at this thread's row, first column of the span.
-// SCALED (pre-split fp16 planes): the accumulator holds the product of row-scaled
-// operands; score = acc * row_scale * col_scale[column] (both exact powers of two).  col_scale must be
-// readable (and 16-byte aligned) for 32 floats from any chunk start < m.
-template <int EPI, int NCH, bool SCALED = false>
-__device__ __forceinline__ void epilogue_tile(const EpiParams& P, RowState<EPI>& st, float aux,
-                                              const float* acc,
-                                              int64_t tile_row0 /* first row of this warp's 32 */,
-                                              int64_t e0 /* global column of the first chunk */, int64_t nq,
-                                              int64_t m, float* my_stg, int lane, float row_scale = 1.f,
-                                              const float* __restrict__ col_scale = nullptr,
-                                              int64_t csr_end = 0 /* end of this row's CSR segment (0: none) */) {
-  const int64_t row = tile_row0 + lane;
-  const bool row_ok = row < nq;
-  // CSR side input: position of the first listed column >= e0 in this row's segment (one binary search per span)
-  int64_t csr_cur = 0;
-  if (csr_end > 0) csr_cur = csr_lower_bound(P.csr_col, __ldg(P.csr_off + row), csr_end, e0);
-#pragma unroll 1
-  for (int j = 0; j < NCH; ++j) {
-    const int64_t c0 = e0 + j * 32;
-    if (c0 >= m) break;                                   // warp-uniform: chunk entirely out of range
-    uint32_t v[32];
-#pragma unroll
-    for (int c = 0; c < 32; ++c) v[c] = __float_as_uint(acc[j * 32 + c]);
-    if constexpr (SCALED) {
-      float4 cs[8];
-#pragma unroll
-      for (int g = 0; g < 8; ++g) cs[g] = __ldg(reinterpret_cast<const float4*>(col_scale + c0) + g);
-#pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        v[4 * g + 0] = __float_as_uint(__uint_as_float(v[4 * g + 0]) * (row_scale * cs[g].x));
-        v[4 * g + 1] = __float_as_uint(__uint_as_float(v[4 * g + 1]) * (row_scale * cs[g].y));
-        v[4 * g + 2] = __float_as_uint(__uint_as_float(v[4 * g + 2]) * (row_scale * cs[g].z));
-        v[4 * g + 3] = __float_as_uint(__uint_as_float(v[4 * g + 3]) * (row_scale * cs[g].w));
-      }
-    }
-    if (csr_cur < csr_end) {
-      // listed columns of this row inside [c0, c0 + 32): emit their scores (losses) or filter them (rank)
-      int64_t cj = __ldg(P.csr_col + csr_cur);
-      while (cj < c0 + 32) {
-        const int rel = (int)(cj - c0);
+// One row's share of a tile: e0 = first column of the tile, q = lane % 4, c0 = e0 + 2q.  v is clobbered (rank: CSR
+// filtered columns become -inf).
+template <int EPI>
+__device__ __forceinline__ void epi_row(const EpiParams& P, RowState<EPI>& st, float (&v)[32], int64_t row,
+                                        int64_t e0, int64_t m, int q) {
+  const int64_t c0 = e0 + 2 * q;
+  if constexpr (EPI != EPI_STORE) {
+    if (P.csr_off) {
+      // listed columns of this row inside the tile: emit their scores (losses) or filter them (rank).  Every lane of
+      // the quad walks the list and acts on the columns it holds.
+      const int64_t end = __ldg(P.csr_off + row + 1);
+      const int64_t lim = e0 + 128 < m ? e0 + 128 : m;
+      const int64_t skip = (EPI == EPI_RANK && P.csr_skip) ? __ldg(P.csr_skip + row) : -1;
+      for (int64_t cur = csr_lower_bound(P.csr_col, __ldg(P.csr_off + row), end, e0); cur < end; ++cur) {
+        const int64_t cj = __ldg(P.csr_col + cur);
+        if (cj >= lim) break;
+        const int k = frag_elem((int)(cj - e0), q);
+        if (k < 0) continue;
         if constexpr (EPI == EPI_RANK) {
-          if (!P.csr_skip || __ldg(P.csr_skip + row) != cj) {
+          if (cj != skip) {
 #pragma unroll
-            for (int c = 0; c < 32; ++c)
-              if (c == rel) v[c] = 0xff800000u;            // -inf: neither greater nor close (for a finite true score)
+            for (int i = 0; i < 32; ++i)
+              if (i == k) v[i] = -INFINITY;               // neither greater nor close (for a finite true score)
           }
         } else {
-          uint32_t x = 0;
-#pragma unroll
-          for (int c = 0; c < 32; ++c)
-            if (c == rel) x = v[c];
-          if (cj < m) P.csr_out[csr_cur] = __uint_as_float(x);
+          P.csr_out[cur] = frag_get(v, k);
         }
-        if (++csr_cur >= csr_end) break;
-        cj = __ldg(P.csr_col + csr_cur);
       }
     }
     if constexpr (EPI == EPI_BCE || EPI == EPI_KL) {
-      if (P.csr_extra && c0 == 0 && row_ok) P.csr_out[P.csr_nnz + row] = __uint_as_float(v[0]);
-    }
-    if constexpr (EPI == EPI_STORE) {
-      // transpose a 32x32 block through smem: each store instruction then writes 32 consecutive
-      // entities of ONE query row (coalesced 128 B) whatever the row stride is
-#pragma unroll
-      for (int c = 0; c < 32; ++c) my_stg[lane * STG_LD + c] = __uint_as_float(v[c]);
-      __syncwarp();
-      const int64_t col = c0 + lane;
-      // rows of this warp map to consecutive output rows unless the block straddles the sp|po seam
-      const bool seam = P.n_rows_out > 0 && tile_row0 < P.n_rows_out && tile_row0 + 32 > P.n_rows_out;
-      if (!seam) {
-        int64_t r0 = tile_row0, cb = 0;
-        if (P.n_rows_out > 0 && r0 >= P.n_rows_out) { r0 -= P.n_rows_out; cb = P.col_block; }
-        float* __restrict__ p = P.out + r0 * P.ldo + cb + col;
-        const int nrows = (int)((nq - tile_row0) < 32 ? (nq - tile_row0) : 32);
-        float t[32];
-#pragma unroll
-        for (int rr = 0; rr < 32; ++rr) t[rr] = my_stg[rr * STG_LD + lane];
-        if (col < m && P.accumulate_out) {
-#pragma unroll
-          for (int rr = 0; rr < 32; ++rr)
-            if (rr < nrows) atomicAdd(p + rr * P.ldo, t[rr]);
-        } else if (col < m) {
-          if (nrows == 32) {
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) p[rr * P.ldo] = t[rr];
-          } else {
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr)
-              if (rr < nrows) p[rr * P.ldo] = t[rr];
-          }
-          for (int g = 0; g < P.n_peers; ++g) {        // same offsets in the peers' symmetric buffers
-            float* __restrict__ pp = P.out_peer[g] + (p - P.out);
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr)
-              if (rr < nrows) pp[rr * P.ldo] = t[rr];
-          }
-        }
-      } else if (col < m) {
-        for (int rr = 0; rr < 32; ++rr) {
-          int64_t r = tile_row0 + rr;
-          if (r < nq) {
-            int64_t cb = 0;
-            if (r >= P.n_rows_out) { r -= P.n_rows_out; cb = P.col_block; }
-            const int64_t at = r * P.ldo + cb + col;
-            const float xv = my_stg[rr * STG_LD + lane];
-            P.out[at] = xv;
-            for (int g = 0; g < P.n_peers; ++g) P.out_peer[g][at] = xv;
-          }
-        }
-      }
-      __syncwarp();
-    } else {
-      // dense side matrix (labels / filter): the warp stages its 32x32 block through shared memory
-      // with coalesced 128-B row reads; each thread then reads its own row from smem (reading the
-      // matrix directly would touch 32 different rows per load instruction)
-      const float* gside = nullptr;
-      int64_t gld = 0;
-      if constexpr (EPI == EPI_RANK) { gside = P.filter; gld = P.ldf; }
-      else { gside = P.label_dense; gld = P.ldl; }
-      const float* side = nullptr;
-      if (gside) {
-        const int64_t col = c0 + lane;
-        const bool col_ok = col < m;
-#pragma unroll 8
-        for (int rr = 0; rr < 32; ++rr) {
-          const int64_t r = tile_row0 + rr;
-          my_stg[rr * STG_LD + lane] = (col_ok && r < nq) ? __ldg(gside + r * gld + col) : 0.f;
-        }
-        __syncwarp();
-        side = my_stg + lane * STG_LD;
-      }
-      if (row_ok) {
-        if (c0 + 32 <= m) epi_chunk32<EPI, true>(P, st, row, aux, v, c0, m, side);
-        else              epi_chunk32<EPI, false>(P, st, row, aux, v, c0, m, side);
-      }
-      if (gside) __syncwarp();
+      if (P.csr_extra && e0 == 0 && q == 0) P.csr_out[P.csr_nnz + row] = v[0];
     }
   }
+  if (e0 + 128 <= m) epi_row_body<EPI, true>(P, st, v, row, e0, c0, 128, q);
+  else               epi_row_body<EPI, false>(P, st, v, row, e0, c0, (int)(m - c0), q);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

@@ -132,6 +132,17 @@ CASES = {
     "tc3_step_n128": lambda: case_1vsall("complex", 14541, 237, 512, 128, "3xtf32", "step"),
     "tc3_step_n4096": lambda: case_1vsall("complex", 14541, 237, 512, 4096, "3xtf32", "step"),
     "rescal_step": lambda: case_1vsall("rescal", 123182, 37, 200, 1024, "3xtf32", "step"),
+    # the default pre-split fp16 path ("auto") at the shapes of the explicit-precision cases above
+    "auto_step": lambda: case_1vsall("complex", 14541, 237, 512, 1024, "auto", "step"),
+    "auto_store": lambda: case_1vsall("complex", 14541, 237, 512, 1024, "auto", "store"),
+    "auto_kl": lambda: case_1vsall("complex", 14541, 237, 512, 1024, "auto", "kl"),
+    "auto_step_n128": lambda: case_1vsall("complex", 14541, 237, 512, 128, "auto", "step"),
+    "auto_step_n4096": lambda: case_1vsall("complex", 14541, 237, 512, 4096, "auto", "step"),
+    "auto_store_n128": lambda: case_1vsall("complex", 14541, 237, 512, 128, "auto", "store"),
+    "auto_store_n4096": lambda: case_1vsall("complex", 14541, 237, 512, 4096, "auto", "store"),
+    "auto_kl_n128": lambda: case_1vsall("complex", 14541, 237, 512, 128, "auto", "kl"),
+    "auto_kl_n4096": lambda: case_1vsall("complex", 14541, 237, 512, 4096, "auto", "kl"),
+    "auto_rescal_step": lambda: case_1vsall("rescal", 123182, 37, 200, 1024, "auto", "step"),
     "transe_step": lambda: case_1vsall("transe", 14541, 237, 512, 1024, "auto", "step"),
     "transe_store": lambda: case_1vsall("transe", 14541, 237, 512, 1024, "auto", "store"),
     "rotate_step": lambda: case_1vsall("rotate", 14541, 237, 512, 1024, "auto", "step"),
