@@ -202,6 +202,29 @@ int b200kge_rank_sp_po_csr(int model, float l_norm, int precision, const b200kge
                            int64_t* rank, int64_t* ties, void* workspace, size_t workspace_bytes,
                            b200kge_stream_t stream);
 
+/* Every ranking EntityRankingJob computes for one batch (raw, _filt and, with filter_with_test, _filt_test), from ONE
+ * scoring pass over the whole entity table (eval_entity_ranking.py:184-315,533-596) without materialising scores or
+ * label matrices.  ent / rel are the plain tables (idx == NULL), s / p / o the batch's n index triples (device int64);
+ * the candidates are all rows of ent.  Rows are stacked as in b200kge_rank_sp_po: rows 0..n-1 the sp_ queries (s, p),
+ * rows n..2n-1 the _po queries (p, o) — or, with num_relations = R > 0 (reciprocal relations, rel->rows == 2R), the sp_
+ * queries (o, p + R) (reciprocal_relations_model.py:85-92).  Per stacked row r:
+ *   true_score[r]   the score of the row's true answer; own_col[r] that answer (o for sp_ rows, s for _po rows);
+ *   F               filter_col[filter_off[r] .. filter_off[r+1]): the known answers (entity_ranking.filter_splits),
+ *                   sorted and unique per row (filter_col may be NULL when F is empty);
+ *   T (optional)    test_col[test_off[r] .. test_off[r+1]): the test answers NOT in F, sorted and unique per row.
+ * rank / ties are int64 [Rk][2n], Rk = 2 (raw, _filt) or 3 with T (_filt_test), and are ACCUMULATED INTO.  Raw counts
+ * compare every column as b200kge_rank_sp_po; _filt counts every column of F except own_col as -inf (:286-290,561-566),
+ * _filt_test every column of F and T except own_col (:277-307).  own_score [2n] receives the score computed at
+ * own_col[r], for the reference's tie-handling consistency check (:240-274).  Workspace: b200kge_workspace_bytes(model,
+ * n, ent->rows, ent->dim, 0).  CP runs its two directions as two launches.  The in-kernel split precision modes return
+ * B200KGE_ERR_UNSUPPORTED before anything is launched. */
+int b200kge_rank_sp_po_eval(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                            const b200kge_rows_t* rel, int64_t num_relations, const int64_t* s, const int64_t* p,
+                            const int64_t* o, int64_t n, const float* true_score, const int64_t* own_col,
+                            const int64_t* filter_off, const int64_t* filter_col, const int64_t* test_off,
+                            const int64_t* test_col, float rtol, float atol, int64_t* rank, int64_t* ties,
+                            float* own_score, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+
 /* b200kge_score_sp_po FUSED WITH THE ALL-GATHER of an entity-sharded table: `cand` is this rank's shard; the two
  * halves are written at out[i*ldo + j] (sp_) and out[i*ldo + col_block + j] (_po), j < cand->rows, AND at the same
  * offsets into each of the n_peers (<= 7) buffers peer_out[g] — peer-mapped device pointers to the other ranks'

@@ -65,7 +65,11 @@ SIGNATURES = {
     "b200kge_rank_sp_po_csr": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, _RP, _RP, C.c_int64, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
-    "b200kge_shard_gather_rows": (C.c_int, [_RP, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
+    "b200kge_rank_sp_po_eval": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_int64, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_shard_gather_rows":(C.c_int, [_RP, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
     "b200kge_loss_dense": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.POINTER(Labels), C.c_int,
                                      C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_rank_dense": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,

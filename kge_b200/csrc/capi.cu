@@ -129,11 +129,18 @@ int run_block(const Block& B, float l_norm, int precision, int epi_kind, EpiPara
     if (f0.pair_op != PAIR_DOT) { set_error("tensor-core precision modes apply to dot-product scorers only"); return B200KGE_ERR_UNSUPPORTED; }
   }
   { const char* env_v = getenv("B200KGE_TC_VERSION");      // experiments: 1 forces the in-kernel split
-    if (env_v && atoi(env_v) == 1 && tc_kind == 3 && tc_supported(f0.pair_op, K, *B.cand, f0.col_off)) {
+    if (env_v && atoi(env_v) == 1 && tc_kind == 3 && epi_kind != EPI_RANK_EVAL &&
+        tc_supported(f0.pair_op, K, *B.cand, f0.col_off)) {
       tc_kind = 1; precision = B200KGE_PREC_TF32_BF16X2;
     } }
 
-  if (P.csr_off && (cols_differ || B.cand->idx || tc_kind == 1 || (tc_kind == 0 && epi_kind != EPI_RANK))) {
+  if (epi_kind == EPI_RANK_EVAL) {
+    // every ranking in one pass: the pre-split tensor-core kernel and the CUDA-core kernel; CP runs per direction below
+    if (B.cand->idx || tc_kind == 1) {
+      set_error("the evaluation ranking runs on the pre-split tensor-core or the CUDA-core kernel over a plain table");
+      return B200KGE_ERR_UNSUPPORTED;
+    }
+  } else if (P.csr_off && (cols_differ || B.cand->idx || tc_kind == 1 || (tc_kind == 0 && epi_kind != EPI_RANK))) {
     // CSR side inputs: the pre-split tensor-core epilogue (losses and rank) and the CUDA-core kernel's rank epilogue.
     // Nothing has been launched or taken from the workspace yet: callers fall back to their dense / composed form.
     set_error("this CSR side input is not consumed by the kernel serving this call (losses: pre-split tensor-core path; "
@@ -148,6 +155,11 @@ int run_block(const Block& B, float l_norm, int precision, int epi_kind, EpiPara
     EpiParams P0 = P, P1 = P;
     P0.n_rows_out = 0; P1.n_rows_out = 0;
     if (epi_kind == EPI_STORE) { P1.out = P.out + P.col_block; }
+    else if (epi_kind == EPI_RANK_EVAL) {
+      // the second half's rows of every per-row operand (CSR row offsets included: they index the shared col arrays)
+      P1.true_score += n; P1.csr_skip += n; P1.csr_off += n; P1.own_score += n; P1.rank += n; P1.ties += n;
+      if (P1.csr2_off) P1.csr2_off += n;
+    }
     else { set_error("stacked fused epilogues are not available for CP"); return B200KGE_ERR_UNSUPPORTED; }
     int rc = run_block(h0, l_norm, precision, epi_kind, P0, ws, st, nchunks_out);
     if (rc) return rc;
@@ -501,6 +513,60 @@ int b200kge_rank_sp_po_csr(int model, float l_norm, int precision, const b200kge
   P.csr_off = filter_off; P.csr_col = filter_col; P.csr_skip = own_col;
   Block B{model, B200KGE_SP_, &Sr, &Or, &Pr, &C, n};
   return run_block(B, l_norm, precision, EPI_RANK, P, ws, (cudaStream_t)stream, nullptr);
+}
+
+int b200kge_rank_sp_po_eval(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                            const b200kge_rows_t* rel, int64_t num_relations, const int64_t* s, const int64_t* p,
+                            const int64_t* o, int64_t n, const float* true_score, const int64_t* own_col,
+                            const int64_t* filter_off, const int64_t* filter_col, const int64_t* test_off,
+                            const int64_t* test_col, float rtol, float atol, int64_t* rank, int64_t* ties,
+                            float* own_score, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+  if (!ent || !rel || !s || !p || !o || !true_score || !own_col || !filter_off || !rank || !ties || !own_score) {
+    set_error("null rank operand");
+    return B200KGE_ERR_INVALID;
+  }
+  if (ent->idx || rel->idx) { set_error("ent and rel must be plain tables (idx == NULL)"); return B200KGE_ERR_INVALID; }
+  if (n < 0) { set_error("negative batch size"); return B200KGE_ERR_INVALID; }
+  if (num_relations < 0) { set_error("num_relations must be >= 0"); return B200KGE_ERR_INVALID; }
+  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
+  if ((rc = validate_norm(model, l_norm))) return rc;
+  if (num_relations > 0 && (rc = check_reciprocal(rel, num_relations))) return rc;
+  if (precision == B200KGE_PREC_TF32 || precision == B200KGE_PREC_3XTF32 || precision == B200KGE_PREC_TF32_BF16X2) {
+    set_error("the evaluation ranking does not run the in-kernel split precision modes");
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  if (n == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const Rows E = to_rows(ent), R = to_rows(rel);
+  Rows S = E, O = E, Pr = R;
+  S.idx = s; S.rows = n; O.idx = o; O.rows = n; Pr.idx = p; Pr.rows = n;
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  EpiParams P = empty_epi();
+  P.true_score = true_score; P.rtol = rtol; P.atol = atol;
+  P.rank = reinterpret_cast<unsigned long long*>(rank);
+  P.ties = reinterpret_cast<unsigned long long*>(ties);
+  P.csr_off = filter_off; P.csr_col = filter_col; P.csr_skip = own_col;
+  P.csr2_off = test_off; P.csr2_col = test_col;
+  P.rank_ld = 2 * n; P.n_rank = test_off ? 3 : 2;
+  P.own_score = own_score;
+  Block B{model, B200KGE_SP_, &S, &O, &Pr, &E, n};
+  if (num_relations > 0) {
+    // reciprocal relations: rows n..2n-1 are the sp_ queries (o, p + R) (reciprocal_relations_model.py:85-92), folded
+    // here with the sp_ fold; both halves then read the same table columns, so CP stacks too
+    const Folded f = folded_problem(model, B200KGE_SP_, E.dim, l_norm);
+    const int64_t ldq = round_up(f.K, 32);
+    float* Q = (float*)ws.take((size_t)2 * n * ldq * 4);
+    int64_t* p2 = (int64_t*)ws.take((size_t)n * 8);
+    if (!Q || !p2) { set_error("workspace too small for folded queries"); return B200KGE_ERR_WORKSPACE; }
+    offset_index_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(p, n, num_relations, p2);
+    B2K_LAUNCH_CHECK("offset_index_kernel");
+    Rows P2 = R; P2.idx = p2; P2.rows = n;
+    if ((rc = launch_fold_queries(model, B200KGE_SP_, S, Pr, n, 0, Q, ldq, st))) return rc;
+    if ((rc = launch_fold_queries(model, B200KGE_SP_, O, P2, n, n, Q, ldq, st))) return rc;
+    B.Qpre = Q;
+    B.same_fold = true;
+  }
+  return run_block(B, l_norm, precision, EPI_RANK_EVAL, P, ws, st, nullptr);
 }
 
 int b200kge_shard_gather_rows(const b200kge_rows_t* shard, int64_t lo, const int64_t* idx, int64_t n,

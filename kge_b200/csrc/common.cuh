@@ -74,7 +74,7 @@ __host__ __device__ inline int relation_dim(int model, int D) {
 // ---------------------------------------------------------------------------------------------
 // Epilogues.  A kernel computes x = score(row, col) for a tile and hands every valid element to
 // one of these functors; per-row state lives in registers and is flushed once per (row, chunk).
-enum EpiKind : int { EPI_STORE = 0, EPI_BCE = 1, EPI_KL = 2, EPI_RANK = 3 };
+enum EpiKind : int { EPI_STORE = 0, EPI_BCE = 1, EPI_KL = 2, EPI_RANK = 3, EPI_RANK_EVAL = 4 };
 
 struct FinalizeArgs;
 struct EpiParams {
@@ -120,6 +120,15 @@ struct EpiParams {
   float* out_peer[7];
   int n_peers;
   int store_vec4;      // set by launch_pairwise_simt: every destination row start is 16-byte aligned
+  // EPI_RANK_EVAL (all rankings of EntityRankingJob from one pass, eval_entity_ranking.py:277-313): csr_off / csr_col
+  // list the known answers F of each row and csr_skip its own answer; csr2_off / csr2_col (optional) the test answers
+  // not in F.  Both lists are sorted and unique per row.  rank / ties hold n_rank rows of rank_ld counters (raw,
+  // _filt[, _filt_test]); own_score[r] receives the score at column csr_skip[r].
+  const int64_t* csr2_off;
+  const int64_t* csr2_col;
+  int64_t rank_ld;
+  int n_rank;
+  float* own_score;
 };
 
 // lower bound of `key` in the sorted segment col[lo, hi)
@@ -181,6 +190,16 @@ template <> struct RowState<EPI_RANK> {
   __device__ __forceinline__ void combine(const RowState& o) { greater += o.greater; close += o.close; }
 };
 
+// EPI_RANK_EVAL: every ranking of one row (eval_entity_ranking.py:277-313).  The row state holds the raw counts over all
+// columns, which the flush adds to every ranking; the listed columns of a tile correct the filtered rankings right away
+// (RankFix).  Both are integers, so the sums are exact whatever their order.
+template <> struct RowState<EPI_RANK_EVAL> {
+  static constexpr int F = 0;
+  unsigned int greater, close;
+  __device__ __forceinline__ void init() { greater = 0u; close = 0u; }
+  __device__ __forceinline__ void combine(const RowState& o) { greater += o.greater; close += o.close; }
+};
+
 // torch.isclose(x, t, rtol, atol) for fp32 operands (equal_nan=False), evaluated in fp32 exactly
 // as ATen does: (x == t) | (isfinite(|x-t|) & (|x-t| <= atol + |rtol*t|)).
 __device__ __forceinline__ bool isclose_f(float x, float t, float rtol, float atol) {
@@ -188,6 +207,34 @@ __device__ __forceinline__ bool isclose_f(float x, float t, float rtol, float at
   float actual = fabsf(__fsub_rn(x, t));
   return (x == t) || (isfinite(actual) && actual <= allowed);
 }
+
+// The corrections of one row's listed columns within one tile: a filtered column becomes score - inf = -inf (:565-566),
+// which is never greater and is close iff the true score is -inf, so each listed column swaps its raw contribution for
+// that one.  f* correct _filt and _filt_test (columns of F), t* _filt_test only (test answers not in F).
+struct RankFix {
+  unsigned int fg, fc, tg, tc;     // greater counts taken out; close counts put in minus taken out (wrap-around)
+  __device__ __forceinline__ RankFix() : fg(0u), fc(0u), tg(0u), tc(0u) {}
+  __device__ __forceinline__ void add(bool test, float x, float t, float rtol, float atol) {
+    if (isnan(x)) x = -INFINITY;
+    const bool c = isclose_f(x, t, rtol, atol);
+    const unsigned int gt = (!c && x > t) ? 1u : 0u;
+    const unsigned int dcl = (t == -INFINITY ? 1u : 0u) - (c ? 1u : 0u);
+    if (test) { tg += gt; tc += dcl; }
+    else      { fg += gt; fc += dcl; }
+  }
+  // rank / ties rows 1 (_filt) and 2 (_filt_test) as signed deltas: the 64-bit sums wrap back to the exact counts once
+  // the flushes of the raw counts have landed
+  __device__ __forceinline__ void commit(const EpiParams& P, int64_t row) const {
+    const long long g1 = -(long long)fg, c1 = (long long)(int)fc;
+    if (g1) atomicAdd(P.rank + P.rank_ld + row, (unsigned long long)g1);
+    if (c1) atomicAdd(P.ties + P.rank_ld + row, (unsigned long long)c1);
+    if (P.n_rank > 2) {
+      const long long g2 = g1 - (long long)tg, c2 = c1 + (long long)(int)tc;
+      if (g2) atomicAdd(P.rank + 2 * P.rank_ld + row, (unsigned long long)g2);
+      if (c2) atomicAdd(P.ties + 2 * P.rank_ld + row, (unsigned long long)c2);
+    }
+  }
+};
 
 template <int KIND>
 __device__ __forceinline__ void epi_elem(const EpiParams& P, RowState<KIND>& st, int64_t row,
@@ -228,6 +275,11 @@ __device__ __forceinline__ void epi_elem(const EpiParams& P, RowState<KIND>& st,
     bool c = isclose_f(v, row_aux, P.rtol, P.atol);
     st.close += c ? 1u : 0u;
     st.greater += (!c && v > row_aux) ? 1u : 0u;
+  } else if constexpr (KIND == EPI_RANK_EVAL) {            // raw counts; the lists are corrected per tile
+    const float v = isnan(x) ? -INFINITY : x;
+    const bool c = isclose_f(v, row_aux, P.rtol, P.atol);
+    st.close += c ? 1u : 0u;
+    st.greater += (!c && v > row_aux) ? 1u : 0u;
   }
 }
 
@@ -237,7 +289,7 @@ template <int KIND>
 __device__ __forceinline__ float epi_row_aux(const EpiParams& P, int64_t row) {
   if constexpr (KIND == EPI_BCE || KIND == EPI_KL) {
     return P.label_idx ? __int_as_float((int)P.label_idx[row]) : __int_as_float(-1);
-  } else if constexpr (KIND == EPI_RANK) {
+  } else if constexpr (KIND == EPI_RANK || KIND == EPI_RANK_EVAL) {
     float t = P.true_score[row];
     return isnan(t) ? -INFINITY : t;                                // :585-586
   } else {
@@ -258,6 +310,14 @@ __device__ __forceinline__ void epi_flush(const EpiParams& P, const RowState<KIN
     // integer atomics: order-independent, hence bit-exact
     if (st.greater) atomicAdd(P.rank + row, (unsigned long long)st.greater);
     if (st.close) atomicAdd(P.ties + row, (unsigned long long)st.close);
+  } else if constexpr (KIND == EPI_RANK_EVAL) {
+    // the raw counts enter every ranking; the listed columns' corrections were committed per tile (RankFix)
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      if (k >= P.n_rank) break;
+      if (st.greater) atomicAdd(P.rank + k * P.rank_ld + row, (unsigned long long)st.greater);
+      if (st.close) atomicAdd(P.ties + k * P.rank_ld + row, (unsigned long long)st.close);
+    }
   }
 }
 

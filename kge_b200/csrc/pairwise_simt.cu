@@ -73,6 +73,41 @@ __device__ __forceinline__ void fetch8(const float* __restrict__ rowp, bool row_
   for (int c = 0; c < 8; ++c) r[c] = (row_ok && k + c < kmax) ? __ldg(rowp + k + c) : 0.f;
 }
 
+// EPI_RANK_EVAL after the raw counts of a tile (the tensor-core form is tc_common.cuh: rank_eval_row).  The thread holds
+// columns col0 + 4 tx + 64 (j >> 2) + (j & 3) of the row, acc[j] their unfinished scores, t the NaN-cleaned true score.
+// One binary search per list, row and tile: the lists are short, and forward-moving cursors for two lists would cost
+// 32 registers.
+template <int PAIR>
+__device__ __forceinline__ void rank_eval_tile(const EpiParams& P, const float (&acc)[8], float p_norm, int64_t row,
+                                               int64_t col0, int64_t m, int tx, float t) {
+  const int64_t lim = col0 + BN < m ? col0 + BN : m;
+  const int64_t own = __ldg(P.csr_skip + row);
+  auto holds = [&](int64_t cj) { return (((int)(cj - col0) & 63) >> 2) == tx; };
+  auto pick = [&](int64_t cj) {
+    const int rel = (int)(cj - col0), j = (rel >> 6) * 4 + (rel & 3);
+    float x = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      if (i == j) x = acc[i];
+    return pair_finish<PAIR>(x, p_norm);
+  };
+  if (own >= col0 && own < lim && holds(own)) P.own_score[row] = pick(own);
+  RankFix fix;
+#pragma unroll
+  for (int list = 0; list < 2; ++list) {
+    const int64_t* __restrict__ off = list ? P.csr2_off : P.csr_off;
+    const int64_t* __restrict__ col = list ? P.csr2_col : P.csr_col;
+    if (!off) continue;
+    const int64_t end = __ldg(off + row + 1);
+    for (int64_t cur = csr_lower_bound(col, __ldg(off + row), end, col0); cur < end; ++cur) {
+      const int64_t cj = __ldg(col + cur);
+      if (cj >= lim) break;
+      if (holds(cj) && cj != own) fix.add(list == 1, pick(cj), t, P.rtol, P.atol);
+    }
+  }
+  fix.commit(P, row);
+}
+
 // CSR: the ranking epilogue with a CSR filter is its own instantiation — its 16 cursor registers would otherwise cost the
 // plain rank kernel its second resident CTA (168 vs <= 128 registers: 5.83 -> 6.59 ms on the cfg5 shard).
 template <int PAIR, int EPI, bool VEC, bool CSR = false>
@@ -243,6 +278,9 @@ pairwise_simt_kernel(const float* __restrict__ Q, int64_t ldq, int64_t nq, Rows 
         }
         if (row_ok && col < m) epi_elem<EPI>(P, st[i], row, col, x, aux[i]);
       }
+      if constexpr (EPI == EPI_RANK_EVAL) {
+        if (row_ok) rank_eval_tile<PAIR>(P, acc[i], p_norm, row, col0, m, tx, aux[i]);
+      }
     }
   }
 
@@ -287,6 +325,7 @@ int launch_p(int epi, bool vec, dim3 grid, cudaStream_t st, const float* Q, int6
     case EPI_BCE:   return launch_pe<PAIR, EPI_BCE>(vec, grid, st, Q, ldq, nq, cand, col_off, K, p, P);
     case EPI_KL:    return launch_pe<PAIR, EPI_KL>(vec, grid, st, Q, ldq, nq, cand, col_off, K, p, P);
     case EPI_RANK:  return launch_pe<PAIR, EPI_RANK>(vec, grid, st, Q, ldq, nq, cand, col_off, K, p, P);
+    case EPI_RANK_EVAL: return launch_pe<PAIR, EPI_RANK_EVAL>(vec, grid, st, Q, ldq, nq, cand, col_off, K, p, P);
   }
   set_error("bad epilogue kind %d", epi);
   return B200KGE_ERR_INVALID;

@@ -50,6 +50,7 @@ constexpr int STAGE_BYTES = 64 * 1024;
 constexpr int BOX_BYTES = 16 * 1024;        // one 128-row box of 128-byte rows
 // per-row loss / rank state of the consumers between tiles: 256 consumer threads x 4 rows x the largest RowState
 constexpr int STATE_BYTES = 256 * 4 * (int)sizeof(RowState<EPI_KL>);
+static_assert(sizeof(RowState<EPI_RANK_EVAL>) <= sizeof(RowState<EPI_KL>), "row state slots are sized for KL");
 constexpr int SMEM_BYTES = 1024 /*align slack*/ + NSTAGE * STAGE_BYTES + 256 /*barriers*/ + STATE_BYTES;
 static_assert(SMEM_BYTES <= 227 * 1024, "exceeds the H100's 227 KB of shared memory per block");
 
@@ -309,7 +310,7 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
             const int64_t row = (int64_t)qt * TM + row_in_tile + 64 * (rr >> 1) + 8 * (rr & 1);
             if (writer && row < prm.nq) {
               epi_flush<EPI>(P, rs, row, 2 * j + h);
-              if constexpr (EPI != EPI_RANK) {
+              if constexpr (EPI != EPI_RANK && EPI != EPI_RANK_EVAL) {
                 if (ends_qt) {
                   RowState<EPI> z;
                   z.init();
@@ -362,6 +363,9 @@ int launch_mode(int epi_kind, const CUtensorMap (&maps)[4], const TcParams& prm,
     case EPI_BCE:   return launch_k<EPI_BCE, MODE>(maps, prm, st);
     case EPI_KL:    return launch_k<EPI_KL, MODE>(maps, prm, st);
     case EPI_RANK:  return launch_k<EPI_RANK, MODE>(maps, prm, st);
+    case EPI_RANK_EVAL:   // pre-split planes only; run_block refuses the in-kernel split modes before any launch
+      if constexpr (MODE == MODE_F16X3) return launch_k<EPI_RANK_EVAL, MODE>(maps, prm, st);
+      break;
   }
   set_error("bad epilogue kind %d", epi_kind);
   return B200KGE_ERR_INVALID;

@@ -195,11 +195,11 @@ __device__ __forceinline__ void epi_row_body(const EpiParams& P, RowState<EPI>& 
       const int k = (lab >= e0 && lab < e0 + 128 && (FULL || lab - c0 < nvalid)) ? frag_elem((int)(lab - e0), q) : -1;
       if (k >= 0) { st.y_sum += 1.0f; st.yx += frag_get(v, k); }
     }
-  } else if constexpr (EPI == EPI_RANK) {
+  } else if constexpr (EPI == EPI_RANK || EPI == EPI_RANK_EVAL) {
     // eval_entity_ranking.py:561-596; `allowed` depends on the row only -> hoisted
     const float t = epi_row_aux<EPI_RANK>(P, row);
     const float allowed = __fadd_rn(P.atol, fabsf(__fmul_rn(P.rtol, t)));
-    const float* __restrict__ f = P.filter ? P.filter + row * P.ldf + c0 : nullptr;
+    const float* __restrict__ f = (EPI == EPI_RANK && P.filter) ? P.filter + row * P.ldf + c0 : nullptr;
     unsigned int gt = 0, cl = 0;
 #pragma unroll
     for (int k = 0; k < 32; ++k) {
@@ -244,12 +244,47 @@ __device__ __forceinline__ void epi_row_body(const EpiParams& P, RowState<EPI>& 
   }
 }
 
+// EPI_RANK_EVAL after the raw counts of a tile: the row's listed columns inside the tile (F, then the test answers not
+// in F) swap their raw contribution for that of -inf (RankFix), except the own answer, whose score goes to own_score.
+// Every lane of the quad walks the lists and acts on the columns it holds.
+__device__ __forceinline__ void rank_eval_row(const EpiParams& P, const float (&v)[32], int64_t row, int64_t e0, int64_t m,
+                                              int q) {
+  const float t = epi_row_aux<EPI_RANK_EVAL>(P, row);
+  const int64_t lim = e0 + 128 < m ? e0 + 128 : m;
+  const int64_t own = __ldg(P.csr_skip + row);
+  if (own >= e0 && own < lim) {
+    const int k = frag_elem((int)(own - e0), q);
+    if (k >= 0) P.own_score[row] = frag_get(v, k);
+  }
+  RankFix fix;
+#pragma unroll
+  for (int list = 0; list < 2; ++list) {
+    const int64_t* __restrict__ off = list ? P.csr2_off : P.csr_off;
+    const int64_t* __restrict__ col = list ? P.csr2_col : P.csr_col;
+    if (!off) continue;
+    const int64_t end = __ldg(off + row + 1);
+    for (int64_t cur = csr_lower_bound(col, __ldg(off + row), end, e0); cur < end; ++cur) {
+      const int64_t cj = __ldg(col + cur);
+      if (cj >= lim) break;
+      const int k = frag_elem((int)(cj - e0), q);
+      if (k >= 0 && cj != own) fix.add(list == 1, frag_get(v, k), t, P.rtol, P.atol);
+    }
+  }
+  fix.commit(P, row);
+}
+
 // One row's share of a tile: e0 = first column of the tile, q = lane % 4, c0 = e0 + 2q.  v is clobbered (rank: CSR
 // filtered columns become -inf).
 template <int EPI>
 __device__ __forceinline__ void epi_row(const EpiParams& P, RowState<EPI>& st, float (&v)[32], int64_t row,
                                         int64_t e0, int64_t m, int q) {
   const int64_t c0 = e0 + 2 * q;
+  if constexpr (EPI == EPI_RANK_EVAL) {
+    if (e0 + 128 <= m) epi_row_body<EPI, true>(P, st, v, row, e0, c0, 128, q);
+    else               epi_row_body<EPI, false>(P, st, v, row, e0, c0, (int)(m - c0), q);
+    rank_eval_row(P, v, row, e0, m, q);
+    return;
+  }
   if constexpr (EPI != EPI_STORE) {
     if (P.csr_off) {
       // listed columns of this row inside the tile: emit their scores (losses) or filter them (rank).  Every lane of

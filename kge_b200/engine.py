@@ -266,6 +266,50 @@ def rank_sp_po_csr(model: str, s_tab, rel, o_tab, cand_tab, true_scores, filter_
     return rank, ties
 
 
+def rank_sp_po_eval(model: str, ent, rel, s, p, o, true_scores, own_col, filter_off, filter_col, test_off=None,
+                    test_col=None, rtol: float = 1e-4, atol: float = 1e-5, l_norm: float = 1.0, precision: str = "auto",
+                    num_relations: int = 0):
+    """Every ranking of one evaluation batch from ONE scoring pass over the whole table (b200kge_rank_sp_po_eval).
+
+    Stacked rows: 0..n-1 the sp_ queries (s, p), n..2n-1 the _po queries (p, o), or with num_relations = R > 0 the sp_
+    queries (o, p + R) of a reciprocal-relations base model.  true_scores / own_col are [2n]; (filter_off, filter_col)
+    the CSR of the known answers and (test_off, test_col) (optional) that of the test answers not among them, both
+    sorted and unique per row.  Returns (rank, ties, own_score): rank / ties int64 [2 or 3, 2n] (raw, _filt[,
+    _filt_test]), own_score [2n] the scores the kernel computed at own_col."""
+    _require_cuda(ent, rel, s, p, o, true_scores, own_col, filter_off, filter_col, test_off, test_col)
+    if (test_off is None) != (test_col is None):
+        raise ValueError("test_off and test_col go together")
+    lib, k = _lib.load(), _Keep()
+    re, rr = k.rows(ent), k.rows(rel)
+    si, pi, oi = _i64(s), _i64(p), _i64(o)
+    n = si.numel()
+    if pi.numel() != n or oi.numel() != n:
+        raise ValueError("s, p and o must have the same length")
+    dev = ent.device
+    t = true_scores.reshape(-1).float().contiguous()
+    own = _i64(own_col)
+    offs, cols = _i64(filter_off), _i64(filter_col)
+    toffs, tcols = _i64(test_off), _i64(test_col)
+    if t.numel() != 2 * n or own.numel() != 2 * n or offs.numel() != 2 * n + 1 or (
+            toffs is not None and toffs.numel() != 2 * n + 1):
+        raise ValueError("true_scores / own_col / the CSR offsets must cover the 2n stacked rows")
+    k.refs += [si, pi, oi, t, own, offs, cols, toffs, tcols]
+    nr = 2 if toffs is None else 3
+    rank = torch.zeros((nr, 2 * n), dtype=torch.int64, device=dev)
+    ties = torch.zeros((nr, 2 * n), dtype=torch.int64, device=dev)
+    own_score = torch.empty(2 * n, dtype=torch.float32, device=dev)
+    ws = _workspace(MODELS[model], n, re.rows, re.dim, False, dev)
+
+    def ptr(x):
+        return x.data_ptr() if x is not None and x.numel() else None
+    _lib.check(lib.b200kge_rank_sp_po_eval(
+        MODELS[model], l_norm, PREC[precision], C.byref(re), C.byref(rr), int(num_relations), si.data_ptr(),
+        pi.data_ptr(), oi.data_ptr(), n, t.data_ptr(), own.data_ptr(), offs.data_ptr(), ptr(cols),
+        toffs.data_ptr() if toffs is not None else None, ptr(tcols), rtol, atol, rank.data_ptr(), ties.data_ptr(),
+        own_score.data_ptr(), ws.data_ptr(), ws.numel(), _stream(dev)))
+    return rank, ties, own_score
+
+
 def shard_gather_rows(shard: torch.Tensor, lo: int, idx: torch.Tensor, out: Optional[torch.Tensor] = None):
     """This rank's contribution to the query-row exchange of an entity-sharded table: out[i] = shard[idx[i] - lo]
     if lo <= idx[i] < lo + rows else 0 (one kernel, no host synchronisation)."""

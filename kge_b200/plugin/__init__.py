@@ -585,6 +585,19 @@ class _B200ModelMixin:
         ln, prec = self._b200_args()
         return engine.score_1vsN_loss(self._b200_name, "_po", ent, rel, ent, labels, o, p, None, loss, offset, ln, prec)
 
+    def rank_eval(self, s, p, o, true2n, F, T, rtol, atol, reciprocal=None, own_col=None):
+        """Every ranking of an evaluation batch against the whole table in one call (engine.rank_sp_po_eval):
+        F = (offsets, cols) the stacked-row CSR of the known answers, T the same for the test answers not in F, or None.
+        `reciprocal` = R when this model is the base model of a ReciprocalRelationsModel.  own_col defaults to [o | s].
+        Returns (rank, ties, own_score) with rank / ties [2 or 3, 2n]."""
+        ent, rel = self._b200_tables()
+        ln, prec = self._b200_args()
+        if own_col is None:
+            own_col = torch.cat((o.reshape(-1), s.reshape(-1)))
+        return engine.rank_sp_po_eval(self._b200_name, ent, rel, s, p, o, true2n, own_col, F[0], F[1],
+                                      None if T is None else T[0], None if T is None else T[1], rtol, atol, ln, prec,
+                                      num_relations=int(reciprocal or 0))
+
     def rank_sp(self, s, p, true_scores, entity_subset=None, filter_labels=None, rtol=1e-4, atol=1e-5,
                 rank=None, ties=None):
         ent, rel = self._b200_tables()
@@ -613,10 +626,12 @@ B200Rescal = _model("B200Rescal", "rescal", Rescal, RescalScorer)
 B200TransE = _model("B200TransE", "transe", TransE, TransEScorer)
 B200RotatE = _model("B200RotatE", "rotate", RotatE, RotatEScorer)
 
-from .jobs import B200TrainingJob1vsAll, B200TrainingJobKvsAll, B200TrainingJobNegativeSampling  # noqa: E402
+from .jobs import (B200EntityRankingJob, B200TrainingJob1vsAll, B200TrainingJobKvsAll,  # noqa: E402
+                   B200TrainingJobNegativeSampling)
 
 __all__ = ["B200ComplEx", "B200DistMult", "B200SimplE", "B200CP", "B200Rescal", "B200TransE", "B200RotatE",
-           "B200TrainingJob1vsAll", "B200TrainingJobKvsAll", "B200TrainingJobNegativeSampling"]
+           "B200TrainingJob1vsAll", "B200TrainingJobKvsAll", "B200TrainingJobNegativeSampling",
+           "B200EntityRankingJob"]
 
 
 def install_native_indexes(dataset, splits=("train", "valid", "test")):

@@ -22,13 +22,19 @@ generator), as `user.b200_device_sampling` does for the negatives.
 LibKGE's `reciprocal_relations_model` over a b200 base model takes the base model's fused and dropout forms too: the
 1vsAll reciprocal step, KvsAll's _po query type as the sp_ query (o, p + R), and the negative-sampling S slot as
 O-slot triples (o, p + R, s).  The P slot, `s_o` and negative-sampling dropout keep the reference's step.
+
+Evaluation: `entity_ranking.class_name: B200EntityRankingJob` selects the entity-ranking job below (eval.py:36-48); the
+training jobs' validation (`valid.every`) is created by the same factory and picks it up too.
 """
 from __future__ import annotations
 
+import math
+import sys
 import time
 
 import torch
 
+from kge.job.eval_entity_ranking import EntityRankingJob
 from kge.job.train_1vsAll import TrainingJob1vsAll
 from kge.job.train_KvsAll import TrainingJobKvsAll
 from kge.job.train_negative_sampling import TrainingJobNegativeSampling
@@ -479,3 +485,223 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
                 loss_value = self.loss(scores, labels[slot], num_negatives=num_samples) / batch_size
             result.avg_loss += loss_value.item()
             result.forward_time += time.time()
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Entity-ranking evaluation
+
+#: precision modes b200kge_rank_sp_po_eval serves (the in-kernel split modes keep the reference's _evaluate)
+_EVAL_PRECISIONS = ("auto", "fp32", "f16x3")
+
+
+def _row_keys(offsets, cols, row0, E):
+    """row * E + col for every entry of a CSR (rows numbered from row0)."""
+    n = offsets.numel() - 1
+    rows = torch.repeat_interleave(torch.arange(row0, row0 + n), offsets[1:] - offsets[:-1])
+    return rows * E + cols
+
+
+def eval_filter_csr(batch, E, sp_index, po_index, exclude=None):
+    """(offsets [2n+1], cols, keys) over the stacked rows of an evaluation batch [n, 3]: row i lists the known objects of
+    (s_i, p_i, ?), row n+i the known subjects of (?, p_i, o_i), as entity ids, sorted and unique per row — the
+    coordinates get_sp_po_coords_from_spo_batch (kge/job/util.py:6-29) yields, with the _po block moved from columns
+    [E, 2E) to rows [n, 2n).  keys = row * E + col (sorted); entries whose key is in `exclude` (sorted) are dropped."""
+    n = batch.shape[0]
+    o_sp, c_sp = sp_index.get_all_csr(batch[:, [S, P]])
+    o_po, c_po = po_index.get_all_csr(batch[:, [P, O]])
+    keys = torch.unique(torch.cat((_row_keys(o_sp, c_sp, 0, E), _row_keys(o_po, c_po, n, E))))
+    if exclude is not None and exclude.numel() and keys.numel():
+        keys = keys[~torch.isin(keys, exclude)]
+    offsets = torch.zeros(2 * n + 1, dtype=torch.int64)
+    torch.cumsum(torch.bincount(keys // E, minlength=2 * n), 0, out=offsets[1:])
+    return offsets, keys % E, keys
+
+
+class B200EntityRankingJob(EntityRankingJob):
+    """`EntityRankingJob` (eval_entity_ranking.py:12-487) whose batch is ranked by ONE library call
+    (b200kge_rank_sp_po_eval) against the whole entity table: the raw, filtered and filtered-with-test counts come from a
+    single scoring pass, with the filters as CSR built on the host by the DataLoader workers (kge_b200.indexing).  No
+    [n, 2E] score, label or coordinate tensor exists.  The counts are additive over the table and nothing of size [n, E]
+    is allocated, so `entity_ranking.chunk_size` is not needed and not read.
+
+    The true scores are taken as the reference takes them (score_sp / score_po on the unique targets, :192-203) and the
+    reference's tie-handling consistency check (:240-274) compares them with the scores the kernel computed at the true
+    answers.  Final ranks, histograms (every `metrics_per.*` hook), metrics, hooks and trace entries are the reference
+    job's own (`_get_ranks`, `hist_hooks`, `_compute_metrics`).
+
+    The fused route needs a b200 model whose tables can be read in place (or a ReciprocalRelationsModel over one) and
+    a precision the library's ranking entry serves; everything else, collate included, is the reference's."""
+
+    def __init__(self, config, dataset, parent_job, model):
+        super().__init__(config, dataset, parent_job, model)
+        self._b200_route = None
+        if self.__class__ == B200EntityRankingJob:
+            for f in Job.job_created_hooks:
+                f(self)
+
+    def _b200_select_route(self):
+        """(b200 model, R or None) when the fused route serves this job's model, else None."""
+        base, recip = _reciprocal_base(self.model)
+        target = self.model if base is None else base
+        if getattr(target, "_b200_name", None) is None or not hasattr(target, "b200_fusable"):
+            return None
+        was = target.training
+        try:
+            target.train(False)             # evaluation runs in eval mode: embedding dropout is inactive there
+            ok = target.b200_fusable()
+        finally:
+            target.train(was)
+        if not ok or target._b200_args()[1] not in _EVAL_PRECISIONS:
+            return None
+        return target, recip
+
+    def _prepare(self):
+        super()._prepare()
+        self._b200_route = self._b200_select_route()
+        if self._b200_route is None:
+            return
+        from ..indexing import index_KvsAll
+
+        # the reference appended the evaluation split to filter_splits (:27-29)
+        known = torch.cat([self.dataset.split(sp) for sp in self.filter_splits])
+        self._b200_index = (index_KvsAll(known, "sp"), index_KvsAll(known, "po"))
+        self._b200_test_index = None
+        if "test" not in self.filter_splits and self.filter_with_test:
+            test = self.dataset.split("test")
+            self._b200_test_index = (index_KvsAll(test, "sp"), index_KvsAll(test, "po"))
+
+    def _collate(self, batch):
+        if self._b200_route is None:
+            return super()._collate(batch)
+        batch = torch.cat(batch).reshape((-1, 3))
+        E = self.dataset.num_entities()
+        tri = batch.long()
+        f_off, f_col, f_keys = eval_filter_csr(tri, E, *self._b200_index)
+        test = ()
+        if self._b200_test_index is not None:
+            t_off, t_col, _ = eval_filter_csr(tri, E, *self._b200_test_index, exclude=f_keys)
+            test = (t_off, t_col)
+        own = torch.cat((tri[:, O], tri[:, S]))
+        return batch, (f_off, f_col), test, own
+
+    def _b200_tie_check(self, own_score, true2n):
+        """The reference's check that the ranking pass scored the true answers as score_sp / score_po did (:240-274):
+        on failure log the mean and max difference, then raise or (tie_handling.warn_only) print and go on."""
+        if torch.allclose(own_score, true2n, rtol=self.tie_rtol, atol=self.tie_atol):
+            return
+        diff = torch.abs(own_score - true2n)
+        self.config.log(f"Tie-handling: mean difference between scores was: {diff.mean()}.")
+        self.config.log(f"Tie-handling: max difference between scores was: {diff.max()}.")
+        msg = ("Error in tie-handling: the ranking pass and score_sp / score_po scored a true answer differently beyond "
+               "entity_ranking.tie_handling.rtol / atol. Verify the model's scoring implementations or consider "
+               "increasing the tie-handling tolerances.")
+        if self.config.get("entity_ranking.tie_handling.warn_only"):
+            print(msg, file=sys.stderr)
+        else:
+            raise ValueError(msg)
+
+    def _b200_true_scores(self, s, p, o):
+        """[2n]: o's score of each sp_ row, then s's score of each _po row, from the model's score_sp / score_po on the
+        unique targets (:192-203)."""
+        uo, io = torch.unique(o, return_inverse=True)
+        o_true = torch.gather(self.model.score_sp(s, p, uo), 1, io.view(-1, 1)).view(-1)
+        us, is_ = torch.unique(s, return_inverse=True)
+        s_true = torch.gather(self.model.score_po(p, o, us), 1, is_.view(-1, 1)).view(-1)
+        return torch.cat((o_true, s_true))
+
+    @torch.no_grad()
+    def _evaluate(self):
+        if self._b200_route is None:
+            return super()._evaluate()
+        model, recip = self._b200_route
+        with_test = "test" not in self.filter_splits and self.filter_with_test
+        suffixes = ["", "_filtered"] + (["_filtered_with_test"] if with_test else [])
+        hists = [dict() for _ in suffixes]
+        nb = len(self.loader)
+        common = dict(type="entity_ranking", split=self.eval_split, filter_splits=self.filter_splits)
+        self.current_trace["epoch"] = dict(common, scope="epoch", epoch=self.epoch, batches=nb,
+                                           size=len(self.triples))
+        for f in self.pre_epoch_hooks:
+            f(self)
+
+        metrics = {}
+        epoch_time = -time.time()
+        for batch_number, (batch, filt, test, own) in enumerate(self.loader):
+            self.current_trace["batch"] = dict(common, scope="batch", epoch=self.epoch, batch=batch_number,
+                                               size=len(batch), batches=nb)
+            for f in self.pre_batch_hooks:
+                f(self)
+
+            batch = batch.to(self.device)
+            s, p, o = batch[:, 0], batch[:, 1], batch[:, 2]
+            n = len(batch)
+            filt = tuple(t.to(self.device, non_blocking=True) for t in filt)
+            test = tuple(t.to(self.device, non_blocking=True) for t in test) if with_test else None
+            own = own.to(self.device, non_blocking=True)
+            true2n = self._b200_true_scores(s, p, o)
+            rank, ties, own_score = model.rank_eval(s, p, o, true2n, filt, test, self.tie_rtol, self.tie_atol,
+                                                    reciprocal=recip, own_col=own)
+            self._b200_tie_check(own_score, true2n)
+
+            # per ranking: (s ranks, o ranks); stacked rows 0..n-1 rank the objects, n..2n-1 the subjects
+            ranks = []
+            for k in range(len(suffixes)):
+                r = self._get_ranks(rank[k], ties[k])
+                ranks.append((r[n:], r[:n]))
+            batch_hists = [dict() for _ in suffixes]
+            for f in self.hist_hooks:
+                for k in (0, 1):
+                    f(batch_hists[k], s, p, o, ranks[k][0], ranks[k][1], job=self)
+            if with_test:
+                for f in self.hist_hooks:
+                    f(batch_hists[2], s, p, o, ranks[2][0], ranks[2][1], job=self)
+
+            if self.trace_examples:
+                self._b200_trace_examples(s, p, o, ranks, with_test, nb)
+
+            metrics = {}
+            for k, suffix in enumerate(suffixes):
+                metrics.update(self._compute_metrics(batch_hists[k]["all"], suffix=suffix))
+            self.current_trace["batch"].update(metrics)
+            for f in self.post_batch_hooks:
+                f(self)
+            if self.trace_batch:
+                self.trace(**self.current_trace["batch"])
+            self.current_trace["batch"] = None
+            self._b200_print_progress(batch_number, nb, metrics)
+
+            for k in range(len(suffixes)):
+                for key, h in batch_hists[k].items():
+                    hists[k][key] = hists[k][key] + h if key in hists[k] else h
+
+        self.config.print("\033[2K\r", end="", flush=True)
+        for key in hists[0]:
+            name = "_" + key if key != "all" else ""
+            for k, suffix in enumerate(suffixes):
+                metrics.update(self._compute_metrics(hists[k][key], suffix=suffix + name))
+        epoch_time += time.time()
+        self.current_trace["epoch"].update(dict(epoch_time=epoch_time, event="eval_completed", **metrics))
+
+    def _b200_trace_examples(self, s, p, o, ranks, with_test, nb):
+        """One `example_rank` entry per task and triple, as the reference writes them (:364-403)."""
+        entry = dict(type="entity_ranking", scope="example", split=self.eval_split, filter_splits=self.filter_splits,
+                     size=len(s), batches=nb, epoch=self.epoch)
+        for i in range(len(s)):
+            entry["batch"] = i
+            entry["s"], entry["p"], entry["o"] = s[i].item(), p[i].item(), o[i].item()
+            for task, side in (("sp", 1), ("po", 0)):
+                if with_test:
+                    entry["rank_filtered_with_test"] = ranks[2][side][i].item() + 1
+                self.trace(event="example_rank", task=task, rank=ranks[0][side][i].item() + 1,
+                           rank_filtered=ranks[1][side][i].item() + 1, **entry)
+
+    def _b200_print_progress(self, batch_number, nb, metrics):
+        """The reference's console progress line (:429-453)."""
+        k = self.hits_at_k_s[-1]
+        width = 1 + int(math.ceil(math.log10(nb)))
+        self.config.print(
+            f"\r{self.config.log_prefix}  batch:{batch_number: {width}d}/{nb - 1}, "
+            f"mrr (filt.): {metrics['mean_reciprocal_rank']:4.3f} ({metrics['mean_reciprocal_rank_filtered']:4.3f}), "
+            f"hits@1: {metrics['hits_at_1']:4.3f} ({metrics['hits_at_1_filtered']:4.3f}), "
+            f"hits@{k}: {metrics[f'hits_at_{k}']:4.3f} ({metrics[f'hits_at_{k}_filtered']:4.3f})\033[K",
+            end="", flush=True)
