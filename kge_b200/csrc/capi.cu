@@ -83,6 +83,53 @@ int validate_norm(int model, float l_norm) {
   return 0;
 }
 
+// ent / rel of the entry points that take whole tables: present, plain (idx == NULL), a model and norm they fit
+int check_tables(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel) {
+  if (!ent || !rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables (idx == NULL)"); return B200KGE_ERR_INVALID; }
+  int rc = validate_model(model, to_rows(ent), to_rows(rel));
+  return rc ? rc : validate_norm(model, l_norm);
+}
+
+int check_loss_kind(int loss_kind) {
+  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  return 0;
+}
+
+int check_grad_ld(const b200kge_rows_t* ent, int64_t lde, const b200kge_rows_t* rel, int64_t ldr) {
+  if (lde < ent->dim || ldr < rel->dim) { set_error("gradient leading dimensions are smaller than the table widths"); return B200KGE_ERR_INVALID; }
+  return 0;
+}
+
+EpiParams empty_epi() {
+  EpiParams P;
+  memset(&P, 0, sizeof(P));
+  return P;
+}
+
+bool take_planes(Arena& ws, SplitSet& S) {
+  S.hi = ws.take((size_t)S.rows * S.Kp * 2);
+  S.lo = ws.take((size_t)S.rows * S.Kp * 2);
+  S.inv_scale = (float*)ws.take((size_t)S.rows_pad * 4);
+  return S.hi && S.lo && S.inv_scale;
+}
+size_t planes_bytes(int64_t rows, int64_t rows_pad, int64_t Kp) {
+  return 2 * ((size_t)rows * Kp * 2 + 256) + (size_t)rows_pad * 4 + 256;
+}
+
+// C[M,N] = A B^T on planes: A = "queries" (rows M), B = "table" (rows N, inv_scale padded to N+32)
+// Long reductions are split into 512-element segments accumulated in fp32 (C is zeroed here first).
+int gemm_planes(const SplitSet& A, const SplitSet& B, float* C, int64_t ldc, cudaStream_t st) {
+  EpiParams P = empty_epi();
+  P.out = C; P.ldo = ldc;
+  if (A.Kp > 512) {
+    P.accumulate_out = 1;
+    cudaError_t e = cudaMemset2DAsync(C, (size_t)ldc * 4, 0, (size_t)B.rows * 4, (size_t)A.rows, st);
+    if (e != cudaSuccess) return check_cuda(e, "cudaMemset2DAsync(gemm output)");
+  }
+  return launch_pairwise_tc3(EPI_STORE, A, B, P, st);
+}
+
 // One direction (or the stacked sp+po pair) of a 1-vs-N problem, with any epilogue.
 struct Block {
   int model, combine;     // combine of the first n rows; stacked => second n rows use the other one
@@ -93,6 +140,34 @@ struct Block {
   const float* Qpre = nullptr;   // already-folded queries [nq, round_up(K,32)] (skips the fold launches)
   bool same_fold = false;        // stacked halves BOTH use `combine` (the reciprocal-relations step)
 };
+
+// The block's folded queries [nq, ldq]: B.Qpre, or both halves folded into the workspace.
+int fold_block(const Block& B, int64_t ldq, Arena& ws, cudaStream_t st, const float** Q) {
+  *Q = B.Qpre;
+  if (*Q) return 0;
+  const int64_t n = B.n;
+  float* Qw = (float*)ws.take((size_t)(B.q1 ? 2 * n : n) * ldq * 4);
+  if (!Qw) { set_error("workspace too small for folded queries"); return B200KGE_ERR_WORKSPACE; }
+  int rc = launch_fold_queries(B.model, B.combine, *B.q0, *B.p, n, 0, Qw, ldq, st);
+  if (rc) return rc;
+  if (B.q1 && (rc = launch_fold_queries(B.model, B.same_fold ? B.combine : 1 - B.combine, *B.q1, *B.p, n, n, Qw, ldq, st)))
+    return rc;
+  *Q = Qw;
+  return 0;
+}
+
+// The scorer's nch chunks per row, and for the BCE/KL epilogues their loss partials [nq, nch, F].
+int take_partials(int epi_kind, int64_t nq, int nch, EpiParams& P, Arena& ws, int* nchunks_out, float** part_out) {
+  if (epi_kind == EPI_BCE || epi_kind == EPI_KL) {
+    const int F = (epi_kind == EPI_BCE) ? 2 : 5;
+    P.part = (float*)ws.take((size_t)nq * nch * F * 4);
+    if (!P.part) { set_error("workspace too small for loss partials"); return B200KGE_ERR_WORKSPACE; }
+    if (part_out) *part_out = P.part;
+  }
+  P.nchunks = nch;
+  if (nchunks_out) *nchunks_out = nch;
+  return 0;
+}
 
 // nchunks_out / part_out (optional): number of per-row partial chunks and the partial buffer the loss
 // epilogues wrote (input of launch_loss_finalize).
@@ -128,11 +203,6 @@ int run_block(const Block& B, float l_norm, int precision, int epi_kind, EpiPara
   } else if (precision != B200KGE_PREC_AUTO && precision != B200KGE_PREC_FP32) {
     if (f0.pair_op != PAIR_DOT) { set_error("tensor-core precision modes apply to dot-product scorers only"); return B200KGE_ERR_UNSUPPORTED; }
   }
-  { const char* env_v = getenv("B200KGE_TC_VERSION");      // experiments: 1 forces the in-kernel split
-    if (env_v && atoi(env_v) == 1 && tc_kind == 3 && epi_kind != EPI_RANK_EVAL &&
-        tc_supported(f0.pair_op, K, *B.cand, f0.col_off)) {
-      tc_kind = 1; precision = B200KGE_PREC_TF32_BF16X2;
-    } }
 
   if (epi_kind == EPI_RANK_EVAL) {
     // every ranking in one pass: the pre-split tensor-core kernel and the CUDA-core kernel; CP runs per direction below
@@ -166,91 +236,38 @@ int run_block(const Block& B, float l_norm, int precision, int epi_kind, EpiPara
     return run_block(h1, l_norm, precision, epi_kind, P1, ws, st, nchunks_out);
   }
 
-  if (tc_kind) {
-    int rc = 0;
-    const float* Q = B.Qpre;
-    if (!Q) {
-      float* Qw = (float*)ws.take((size_t)nq * ldq * 4);
-      if (!Qw) { set_error("workspace too small for folded queries"); return B200KGE_ERR_WORKSPACE; }
-      rc = launch_fold_queries(B.model, B.combine, *B.q0, *B.p, n, 0, Qw, ldq, st);
-      if (rc) return rc;
-      if (B.q1) { rc = launch_fold_queries(B.model, B.same_fold ? B.combine : 1 - B.combine, *B.q1, *B.p, n, n, Qw, ldq, st); if (rc) return rc; }
-      Q = Qw;
+  const float* Q = nullptr;
+  int rc = fold_block(B, ldq, ws, st, &Q);
+  if (rc) return rc;
+  if (tc_kind == 3) {
+    // pre-split fp16 path (presplit.cu + pairwise_tc.cu): one launch derives the hi/lo planes of the folded queries
+    // and of the (gathered) candidate rows, one launch scores them.
+    const int Kp = (int)round_up(K, 64);
+    SplitSet SQ{Q, ldq, nullptr, 0, nq, nq, K, Kp, nullptr, nullptr, nullptr};
+    SplitSet ST{B.cand->base, B.cand->ld, B.cand->idx, f0.col_off, m, m + 32, K, Kp, nullptr, nullptr, nullptr};
+    if (!take_planes(ws, SQ) || !take_planes(ws, ST)) {
+      set_error("workspace too small for the pre-split operand planes");
+      return B200KGE_ERR_WORKSPACE;
     }
-    if (tc_kind == 3) {
-      // pre-split fp16 path (presplit.cu + pairwise_tc.cu): one launch derives the hi/lo planes of the folded queries
-      // and of the (gathered) candidate rows, one launch scores them.
-      const int Kp = (int)round_up(K, 64);
-      SplitSet SQ{Q, ldq, nullptr, 0, nq, nq, K, Kp, nullptr, nullptr, nullptr};
-      SplitSet ST{B.cand->base, B.cand->ld, B.cand->idx, f0.col_off, m, m + 32, K, Kp, nullptr, nullptr, nullptr};
-      SQ.hi = ws.take((size_t)nq * Kp * 2); SQ.lo = ws.take((size_t)nq * Kp * 2);
-      SQ.inv_scale = (float*)ws.take((size_t)nq * 4);
-      ST.hi = ws.take((size_t)m * Kp * 2); ST.lo = ws.take((size_t)m * Kp * 2);
-      ST.inv_scale = (float*)ws.take((size_t)(m + 32) * 4);
-      if (!SQ.hi || !SQ.lo || !SQ.inv_scale || !ST.hi || !ST.lo || !ST.inv_scale) {
-        set_error("workspace too small for the pre-split operand planes");
-        return B200KGE_ERR_WORKSPACE;
-      }
-      const int nch3 = tc_nchunks(nq, m);
-      if (epi_kind == EPI_BCE || epi_kind == EPI_KL) {
-        const int F = (epi_kind == EPI_BCE) ? 2 : 5;
-        P.part = (float*)ws.take((size_t)nq * nch3 * F * 4);
-        if (!P.part) { set_error("workspace too small for loss partials"); return B200KGE_ERR_WORKSPACE; }
-        if (part_out) *part_out = P.part;
-      }
-      P.nchunks = nch3;
-      if (nchunks_out) *nchunks_out = nch3;
-      if ((rc = launch_presplit(ST, SQ, st))) return rc;
-      return launch_pairwise_tc3(epi_kind, SQ, ST, P, st);
-    }
+    if ((rc = take_partials(epi_kind, nq, tc_nchunks(nq, m), P, ws, nchunks_out, part_out))) return rc;
+    if ((rc = launch_presplit(ST, SQ, st))) return rc;
+    return launch_pairwise_tc3(epi_kind, SQ, ST, P, st);
+  }
+  if (tc_kind == 1) {
     const int passes = (precision == B200KGE_PREC_TF32) ? 1 : (precision == B200KGE_PREC_3XTF32 ? 3 : 2);
     const float* T = B.cand->base + f0.col_off;
     int64_t ldt = B.cand->ld;
     if (B.cand->idx) {
       float* G = (float*)ws.take((size_t)m * ldq * 4);
       if (!G) { set_error("workspace too small to gather the candidate subset"); return B200KGE_ERR_WORKSPACE; }
-      rc = launch_gather_rows(*B.cand, f0.col_off, K, G, ldq, st);
-      if (rc) return rc;
+      if ((rc = launch_gather_rows(*B.cand, f0.col_off, K, G, ldq, st))) return rc;
       T = G; ldt = ldq;
     }
-    const int nch = tc_nchunks(nq, m);
-    if (epi_kind == EPI_BCE || epi_kind == EPI_KL) {
-      const int F = (epi_kind == EPI_BCE) ? 2 : 5;
-      P.part = (float*)ws.take((size_t)nq * nch * F * 4);
-      if (!P.part) { set_error("workspace too small for loss partials"); return B200KGE_ERR_WORKSPACE; }
-      if (part_out) *part_out = P.part;
-    }
-    P.nchunks = nch;
-    if (nchunks_out) *nchunks_out = nch;
+    if ((rc = take_partials(epi_kind, nq, tc_nchunks(nq, m), P, ws, nchunks_out, part_out))) return rc;
     return launch_pairwise_tc(epi_kind, passes, Q, ldq, nq, T, ldt, m, K, P, st);
   }
-
-  int rc = 0;
-  const float* Q = B.Qpre;
-  if (!Q) {
-    float* Qw = (float*)ws.take((size_t)nq * ldq * 4);
-    if (!Qw) { set_error("workspace too small for folded queries"); return B200KGE_ERR_WORKSPACE; }
-    rc = launch_fold_queries(B.model, B.combine, *B.q0, *B.p, n, 0, Qw, ldq, st);
-    if (rc) return rc;
-    if (B.q1) { rc = launch_fold_queries(B.model, B.same_fold ? B.combine : 1 - B.combine, *B.q1, *B.p, n, n, Qw, ldq, st); if (rc) return rc; }
-    Q = Qw;
-  }
-  const int nch = pairwise_simt_nchunks(nq, m);
-  if (epi_kind == EPI_BCE || epi_kind == EPI_KL) {
-    const int F = (epi_kind == EPI_BCE) ? 2 : 5;
-    P.part = (float*)ws.take((size_t)nq * nch * F * 4);
-    if (!P.part) { set_error("workspace too small for loss partials"); return B200KGE_ERR_WORKSPACE; }
-    if (part_out) *part_out = P.part;
-  }
-  P.nchunks = nch;
-  if (nchunks_out) *nchunks_out = nch;
+  if ((rc = take_partials(epi_kind, nq, pairwise_simt_nchunks(nq, m), P, ws, nchunks_out, part_out))) return rc;
   return launch_pairwise_simt(epi_kind, f0.pair_op, l_norm, Q, ldq, nq, *B.cand, f0.col_off, K, P, st);
-}
-
-EpiParams empty_epi() {
-  EpiParams P;
-  memset(&P, 0, sizeof(P));
-  return P;
 }
 
 int check_1vsN_args(int model, int combine, const b200kge_rows_t* q, const b200kge_rows_t* p,
@@ -274,6 +291,17 @@ __global__ void unpack_triples_kernel(const int64_t* __restrict__ tri, int64_t n
     labels2n[i] = c;       // sp_ rows are labelled with the object      train_1vsAll.py:64-65
     labels2n[n + i] = a;   // _po rows are labelled with the subject     train_1vsAll.py:75-76
   }
+}
+
+// s/p/o and the [2n] labels of [n, 3] triples into the caller's buffers; S, O (rows of E) and P (rows of R) index them
+int unpack_triples(const int64_t* triples, int64_t n, int64_t* sidx, int64_t* pidx, int64_t* oidx, int64_t* lab,
+                   const Rows& E, const Rows& R, Rows& S, Rows& O, Rows& P, cudaStream_t st) {
+  unpack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(triples, n, sidx, pidx, oidx, lab);
+  B2K_LAUNCH_CHECK("unpack_triples_kernel");
+  S = E; S.idx = sidx; S.rows = n;
+  O = E; O.idx = oidx; O.rows = n;
+  P = R; P.idx = pidx; P.rows = n;
+  return 0;
 }
 
 __global__ void pack_triples_kernel(const int64_t* __restrict__ q, const int64_t* __restrict__ p, int64_t n, int combine,
@@ -436,7 +464,7 @@ int b200kge_score_1vsN_loss(int model, int combine, float l_norm, int precision,
   int rc = check_1vsN_args(model, combine, q, p, cand, n); if (rc) return rc;
   if ((rc = validate_norm(model, l_norm))) return rc;
   if (!labels || (!labels->idx) == (!labels->dense)) { set_error("exactly one of labels.idx / labels.dense must be given"); return B200KGE_ERR_INVALID; }
-  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  if ((rc = check_loss_kind(loss_kind))) return rc;
   if (!loss_out) { set_error("loss_out is null"); return B200KGE_ERR_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
   Rows Q = to_rows(q), Pr = to_rows(p), C = to_rows(cand);
@@ -521,15 +549,13 @@ int b200kge_rank_sp_po_eval(int model, float l_norm, int precision, const b200kg
                             const int64_t* filter_off, const int64_t* filter_col, const int64_t* test_off,
                             const int64_t* test_col, float rtol, float atol, int64_t* rank, int64_t* ties,
                             float* own_score, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
-  if (!ent || !rel || !s || !p || !o || !true_score || !own_col || !filter_off || !rank || !ties || !own_score) {
+  if (!s || !p || !o || !true_score || !own_col || !filter_off || !rank || !ties || !own_score) {
     set_error("null rank operand");
     return B200KGE_ERR_INVALID;
   }
-  if (ent->idx || rel->idx) { set_error("ent and rel must be plain tables (idx == NULL)"); return B200KGE_ERR_INVALID; }
   if (n < 0) { set_error("negative batch size"); return B200KGE_ERR_INVALID; }
   if (num_relations < 0) { set_error("num_relations must be >= 0"); return B200KGE_ERR_INVALID; }
-  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
-  if ((rc = validate_norm(model, l_norm))) return rc;
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
   if (num_relations > 0 && (rc = check_reciprocal(rel, num_relations))) return rc;
   if (precision == B200KGE_PREC_TF32 || precision == B200KGE_PREC_3XTF32 || precision == B200KGE_PREC_TF32_BF16X2) {
     set_error("the evaluation ranking does not run the in-kernel split precision modes");
@@ -587,7 +613,7 @@ int b200kge_loss_dense(const float* scores, int64_t lds, int64_t n, int64_t m,
   if (!scores || !labels || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if ((!labels->idx) == (!labels->dense)) { set_error("exactly one of labels.idx / labels.dense must be given"); return B200KGE_ERR_INVALID; }
   if (loss_kind >= B200KGE_LOSS_BCE_MEAN && loss_kind <= B200KGE_LOSS_SE) { set_error("loss kind %d is row-wise with one positive per row: use b200kge_ns_loss", loss_kind); return B200KGE_ERR_UNSUPPORTED; }
-  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  int rc = check_loss_kind(loss_kind); if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   if (n == 0 || m == 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
   Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
@@ -601,8 +627,7 @@ int b200kge_loss_dense(const float* scores, int64_t lds, int64_t n, int64_t m,
   if (!P.part) { set_error("workspace too small for loss partials (need %zu bytes)", (size_t)n * nch * F * 4); return B200KGE_ERR_WORKSPACE; }
   void* scratch = ws.take(1024);
   if (!scratch) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
-  int rc = launch_loss_dense(loss_kind, scores, lds, n, m, P, st);
-  if (rc) return rc;
+  if ((rc = launch_loss_dense(loss_kind, scores, lds, n, m, P, st))) return rc;
   return launch_loss_finalize(loss_kind, P.part, nch, n, loss_out, row_loss_out, 1.0f, 0, scratch, 0, st);
 }
 
@@ -651,11 +676,9 @@ static int train_1vsall_forward_impl(int model, float l_norm, int precision,
                                      const int64_t* triples, int64_t n, int loss_kind, float offset,
                                      float* loss_out, void* workspace, size_t workspace_bytes,
                                      b200kge_stream_t stream, int64_t num_rel) {
-  if (!ent || !rel || !triples || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
-  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
-  if ((rc = validate_norm(model, l_norm))) return rc;
-  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  if (!triples || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
+  if ((rc = check_loss_kind(loss_kind))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   if (n <= 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
   Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
@@ -665,44 +688,34 @@ static int train_1vsall_forward_impl(int model, float l_norm, int precision,
   // reciprocal: both halves are sp_ queries
   Folded f0 = folded_problem(model, B200KGE_SP_, E.dim, l_norm),
          f1 = folded_problem(model, num_rel > 0 ? B200KGE_SP_ : B200KGE__PO, E.dim, l_norm);
-  {
-    // Pre-split tensor-core path (dot family except CP, whose directions read different table columns — CP joins in
-    // the reciprocal step): the whole step is THREE launches — prologue (gather + both folds + operand split of queries
-    // and table + labels), the scorer with the loss reduction in its epilogue, and the fixed-order finaliser.
-    const char* env_v = getenv("B200KGE_TC_VERSION");
-    const int tcv = (env_v && atoi(env_v) == 1) ? 1 : 3;
-    const int K = f0.K;
-    const bool presplit = f0.col_off == f1.col_off && f0.pair_op == PAIR_DOT && (model != B200KGE_CP || num_rel > 0) &&
-                          (precision == B200KGE_PREC_AUTO || precision == B200KGE_PREC_F16X3) && K >= 32 && K <= 1024 &&
-                          n >= 16 && E.rows < (1ll << 31) && tcv == 3 &&
-                          ((size_t)round_up(K, 64) + (model == B200KGE_RESCAL ? E.dim : 0)) * 4 <= 48 * 1024;
-    if (presplit) {
-      const int64_t nq = 2 * n, m = E.rows;
-      const int Kp = (int)round_up(K, 64);
-      SplitSet SQ{nullptr, 0, nullptr, 0, nq, nq, K, Kp, nullptr, nullptr, nullptr};
-      SplitSet ST{E.base, E.ld, nullptr, f0.col_off, m, m + 32, K, Kp, nullptr, nullptr, nullptr};
-      SQ.hi = ws.take((size_t)nq * Kp * 2); SQ.lo = ws.take((size_t)nq * Kp * 2);
-      SQ.inv_scale = (float*)ws.take((size_t)nq * 4);
-      ST.hi = ws.take((size_t)m * Kp * 2); ST.lo = ws.take((size_t)m * Kp * 2);
-      ST.inv_scale = (float*)ws.take((size_t)(m + 32) * 4);
-      int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
-      uint8_t* scratch = (uint8_t*)ws.take(1024);
-      const int nch = tc_nchunks(nq, m);
-      const int F = (loss_kind == B200KGE_LOSS_BCE) ? 2 : 5;
-      float* part = (float*)ws.take((size_t)nq * nch * F * 4);
-      if (!SQ.hi || !SQ.lo || !SQ.inv_scale || !ST.hi || !ST.lo || !ST.inv_scale || !lab || !scratch || !part) {
-        set_error("workspace too small");
-        return B200KGE_ERR_WORKSPACE;
-      }
-      unsigned int* ticket = reinterpret_cast<unsigned int*>(scratch + 512);
-      if ((rc = launch_prep_split_1vsall(model, E, R, triples, n, SQ, ST, lab, ticket, st, num_rel))) return rc;
-      EpiParams P = empty_epi();
-      P.label_idx = lab;
-      P.offset = (loss_kind == B200KGE_LOSS_BCE) ? offset : 0.f;
-      P.part = part; P.nchunks = nch;
-      if ((rc = launch_pairwise_tc3(epi, SQ, ST, P, st))) return rc;
-      return launch_loss_finalize(loss_kind, part, nch, nq, loss_out, nullptr, scale, 0, scratch, 1, st);
-    }
+  // Pre-split tensor-core path (dot family except CP, whose directions read different table columns — CP joins in
+  // the reciprocal step): the whole step is THREE launches — prologue (gather + both folds + operand split of queries
+  // and table + labels), the scorer with the loss reduction in its epilogue, and the fixed-order finaliser.
+  const int K = f0.K;
+  const bool presplit = f0.col_off == f1.col_off && f0.pair_op == PAIR_DOT && (model != B200KGE_CP || num_rel > 0) &&
+                        (precision == B200KGE_PREC_AUTO || precision == B200KGE_PREC_F16X3) && K >= 32 && K <= 1024 &&
+                        n >= 16 && E.rows < (1ll << 31) &&
+                        ((size_t)round_up(K, 64) + (model == B200KGE_RESCAL ? E.dim : 0)) * 4 <= 48 * 1024;
+  if (presplit) {
+    const int64_t nq = 2 * n, m = E.rows;
+    const int Kp = (int)round_up(K, 64);
+    SplitSet SQ{nullptr, 0, nullptr, 0, nq, nq, K, Kp, nullptr, nullptr, nullptr};
+    SplitSet ST{E.base, E.ld, nullptr, f0.col_off, m, m + 32, K, Kp, nullptr, nullptr, nullptr};
+    const bool planes = take_planes(ws, SQ) && take_planes(ws, ST);
+    int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
+    uint8_t* scratch = (uint8_t*)ws.take(1024);
+    const int nch = tc_nchunks(nq, m);
+    const int F = (loss_kind == B200KGE_LOSS_BCE) ? 2 : 5;
+    float* part = (float*)ws.take((size_t)nq * nch * F * 4);
+    if (!planes || !lab || !scratch || !part) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
+    unsigned int* ticket = reinterpret_cast<unsigned int*>(scratch + 512);
+    if ((rc = launch_prep_split_1vsall(model, E, R, triples, n, SQ, ST, lab, ticket, st, num_rel))) return rc;
+    EpiParams P = empty_epi();
+    P.label_idx = lab;
+    P.offset = (loss_kind == B200KGE_LOSS_BCE) ? offset : 0.f;
+    P.part = part; P.nchunks = nch;
+    if ((rc = launch_pairwise_tc3(epi, SQ, ST, P, st))) return rc;
+    return launch_loss_finalize(loss_kind, part, nch, nq, loss_out, nullptr, scale, 0, scratch, 1, st);
   }
   if (f0.col_off == f1.col_off) {
     // sp_ and _po rows stacked into ONE problem of 2n query rows against the same table:
@@ -734,11 +747,8 @@ static int train_1vsall_forward_impl(int model, float l_norm, int precision,
   int64_t* oidx = (int64_t*)ws.take((size_t)n * 8);
   int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
   if (!sidx || !pidx || !oidx || !lab) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
-  unpack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(triples, n, sidx, pidx, oidx, lab);
-  B2K_LAUNCH_CHECK("unpack_triples_kernel");
-  Rows S = E; S.idx = sidx; S.rows = n;
-  Rows O = E; O.idx = oidx; O.rows = n;
-  Rows Pr = R; Pr.idx = pidx; Pr.rows = n;
+  Rows S, O, Pr;
+  if ((rc = unpack_triples(triples, n, sidx, pidx, oidx, lab, E, R, S, O, Pr, st))) return rc;
   EpiParams P = empty_epi();
   P.label_idx = lab;
   P.offset = (loss_kind == B200KGE_LOSS_BCE) ? offset : 0.f;
@@ -799,82 +809,82 @@ int b200kge_train_1vsall_forward_host(int model, float l_norm, int precision,
 // normalisation, negative-sampling backward, CSR-label losses: SURVEY 8f rows.
 namespace {
 
-bool take_planes(Arena& ws, SplitSet& S) {
-  S.hi = ws.take((size_t)S.rows * S.Kp * 2);
-  S.lo = ws.take((size_t)S.rows * S.Kp * 2);
-  S.inv_scale = (float*)ws.take((size_t)S.rows_pad * 4);
-  return S.hi && S.lo && S.inv_scale;
-}
-size_t planes_bytes(int64_t rows, int64_t rows_pad, int64_t Kp) {
-  return 2 * ((size_t)rows * Kp * 2 + 256) + (size_t)rows_pad * 4 + 256;
+// Where dL/dz of a backward comes from: one-hot labels lab [nq] (1vsAll, scaled 1/n), the CSR labels of a KvsAll
+// query type (target a * y + b, scaled inv_batch), or the caller's dense G [nq, ldg] (autograd through a dense score
+// matrix).  lab also serves as the placeholder index vector of the pre-folded operands.
+struct GradSpec {
+  const int64_t* lab = nullptr;
+  int loss_kind = B200KGE_LOSS_BCE;
+  float offset = 0.f;
+  const int64_t* csr_off = nullptr;
+  const int64_t* csr_col = nullptr;
+  float csr_a = 1.f, csr_b = 0.f, inv_batch = 0.f;
+  const float* G = nullptr;
+  int64_t ldg = 0;
+};
+
+// the CSR labels of a KvsAll query type over m candidates, label smoothing as in KvsAll (y (1 - ls) + ls / m)
+GradSpec csr_grad(const int64_t* q_idx, const int64_t* csr_off, const int64_t* csr_col, float label_smoothing, int64_t m,
+                  int64_t batch_size, int loss_kind, float offset) {
+  GradSpec g;
+  g.lab = q_idx;
+  g.loss_kind = loss_kind; g.offset = offset;
+  g.csr_off = csr_off; g.csr_col = csr_col;
+  g.csr_a = 1.0f - label_smoothing; g.csr_b = label_smoothing > 0.f ? 1.0f / (float)m : 0.f;
+  g.inv_batch = 1.0f / (float)batch_size;
+  return g;
 }
 
-// C[M,N] = A B^T on planes: A = "queries" (rows M), B = "table" (rows N, inv_scale padded to N+32)
-// Long reductions are split into 512-element segments accumulated in fp32 (C is zeroed here first).
-int gemm_planes(const SplitSet& A, const SplitSet& B, float* C, int64_t ldc, cudaStream_t st) {
-  EpiParams P = empty_epi();
-  P.out = C; P.ldo = ldc;
-  if (A.Kp > 512) {
-    P.accumulate_out = 1;
-    cudaError_t e = cudaMemset2DAsync(C, (size_t)ldc * 4, 0, (size_t)B.rows * 4, (size_t)A.rows, st);
-    if (e != cudaSuccess) return check_cuda(e, "cudaMemset2DAsync(gemm output)");
-  }
-  return launch_pairwise_tc3(EPI_STORE, A, B, P, st);
-}
-
-// One block of the backward up to dQ: nq folded query rows Q [nq, ldq] with one-hot labels lab [nq] against
-// the candidate columns [off, off+K) of the entity table; stores dT into those columns of d_ent and dQ
-// [nq, ldq] into the caller's buffer.  dir as in launch_unfold.
-int backward_block(int model, const Rows& E, const Rows& R, const int64_t* triples, int64_t n, int dir,
-                   const float* Q, int64_t ldq, const int64_t* lab, int col_off, int K, int loss_kind, float offset,
-                   float* d_ent, int64_t lde, float* dQ, Arena ws, cudaStream_t st,
-                   const float* Gdense = nullptr, int64_t ldg = 0, const int64_t* csr_off = nullptr,
-                   const int64_t* csr_col = nullptr, float csr_a = 1.f, float csr_b = 0.f, float inv_batch = 0.f,
-                   bool same_fold = false) {
+// One block of the backward up to dQ: nq folded query rows Q [nq, ldq] against the candidate columns [off, off+K)
+// of the entity table; stores dT into those columns of d_ent and dQ [nq, ldq] into the caller's buffer.  dir as in
+// launch_unfold.
+int backward_block(int model, const Rows& E, const Rows& R, int64_t n, int dir, bool same_fold, const float* Q,
+                   int64_t ldq, int col_off, int K, const GradSpec& g, float* d_ent, int64_t lde, float* dQ, Arena ws,
+                   cudaStream_t st) {
   const int64_t nq = dir < 0 ? 2 * n : n, m = E.rows;
   const int64_t ldz = round_up(m, 4), Ep = round_up(m, 64), Np = round_up(nq, 64);
   const int64_t ldE = round_up(m, 4), ldN = round_up(nq, 4);
   int rc;
   SplitSet SG{nullptr, 0, nullptr, 0, nq, nq, (int)m, (int)Ep, nullptr, nullptr, nullptr};
   SplitSet SGT{nullptr, 0, nullptr, 0, m, m, (int)nq, (int)Np, nullptr, nullptr, nullptr};
-  if (Gdense) {
-    // the caller's dL/dz (autograd through a dense score matrix): planes of G and of its transpose, row scaled
+  if (g.G) {
+    // planes of G and of its transpose, row scaled
     float* Gt = (float*)ws.take((size_t)m * ldN * 4);
     if (!Gt) { set_error("workspace too small for the transposed gradient"); return B200KGE_ERR_WORKSPACE; }
-    if ((rc = launch_transpose(Gdense, ldg, nq, m, Gt, ldN, st))) return rc;
-    SG.src = Gdense; SG.ld = ldg;
+    if ((rc = launch_transpose(g.G, g.ldg, nq, m, Gt, ldN, st))) return rc;
+    SG.src = g.G; SG.ld = g.ldg;
     SGT.src = Gt; SGT.ld = ldN;
     if (!take_planes(ws, SG) || !take_planes(ws, SGT)) { set_error("workspace too small for the gradient planes"); return B200KGE_ERR_WORKSPACE; }
     if ((rc = launch_presplit(SGT, SG, st))) return rc;
   } else {
-  // 1. scores through the validated scorer (plain-store epilogue)
-  float* z = (float*)ws.take((size_t)nq * ldz * 4);
-  if (!z) { set_error("workspace too small for the score matrix"); return B200KGE_ERR_WORKSPACE; }
-  {
-    Rows S = E; S.idx = lab; S.rows = n;      // placeholders: operands are pre-folded
-    Rows Pr = R; Pr.idx = lab; Pr.rows = n;
-    EpiParams P = empty_epi();
-    P.out = z; P.ldo = ldz;
-    Block B{model, dir <= 0 ? B200KGE_SP_ : B200KGE__PO, &S, dir < 0 ? &S : nullptr, &Pr, &E, n};
-    B.Qpre = Q;
-    B.same_fold = same_fold;
-    if ((rc = run_block(B, 1.0f, B200KGE_PREC_AUTO, EPI_STORE, P, ws, st, nullptr))) return rc;
-  }
-  // 2. G = sigmoid(z + off) - y as planes, both layouts
-  if (!take_planes(ws, SG) || !take_planes(ws, SGT)) { set_error("workspace too small for the gradient planes"); return B200KGE_ERR_WORKSPACE; }
-  float* row_stat = nullptr;
-  if (loss_kind == B200KGE_LOSS_KL) {
-    row_stat = (float*)ws.take((size_t)nq * 2 * 4);
-    if (!row_stat) { set_error("workspace too small for the row statistics"); return B200KGE_ERR_WORKSPACE; }
-  }
-  if (csr_off) {
-    if ((rc = launch_grad_planes_csr(z, ldz, nq, m, csr_off, csr_col, csr_a, csr_b, row_stat,
-                                     loss_kind == B200KGE_LOSS_KL ? 0.f : offset, inv_batch, SG.hi, SG.lo, Ep, SGT.hi,
-                                     SGT.lo, Np, SG.inv_scale, SGT.inv_scale, st))) return rc;
-  } else
-  if ((rc = launch_grad_planes(z, ldz, nq, m, lab, nullptr, 0, row_stat, loss_kind == B200KGE_LOSS_KL ? 0.f : offset,
-                               1.0f / (float)n, SG.hi, SG.lo, Ep, SGT.hi, SGT.lo, Np, SG.inv_scale, SGT.inv_scale,
-                               st))) return rc;
+    // 1. scores through the validated scorer (plain-store epilogue)
+    float* z = (float*)ws.take((size_t)nq * ldz * 4);
+    if (!z) { set_error("workspace too small for the score matrix"); return B200KGE_ERR_WORKSPACE; }
+    {
+      Rows S = E; S.idx = g.lab; S.rows = n;      // placeholders: operands are pre-folded
+      Rows Pr = R; Pr.idx = g.lab; Pr.rows = n;
+      EpiParams P = empty_epi();
+      P.out = z; P.ldo = ldz;
+      Block B{model, dir <= 0 ? B200KGE_SP_ : B200KGE__PO, &S, dir < 0 ? &S : nullptr, &Pr, &E, n};
+      B.Qpre = Q;
+      B.same_fold = same_fold;
+      if ((rc = run_block(B, 1.0f, B200KGE_PREC_AUTO, EPI_STORE, P, ws, st, nullptr))) return rc;
+    }
+    // 2. G = sigmoid(z + off) - y as planes, both layouts
+    if (!take_planes(ws, SG) || !take_planes(ws, SGT)) { set_error("workspace too small for the gradient planes"); return B200KGE_ERR_WORKSPACE; }
+    float* row_stat = nullptr;
+    if (g.loss_kind == B200KGE_LOSS_KL) {
+      row_stat = (float*)ws.take((size_t)nq * 2 * 4);
+      if (!row_stat) { set_error("workspace too small for the row statistics"); return B200KGE_ERR_WORKSPACE; }
+    }
+    const float off = g.loss_kind == B200KGE_LOSS_KL ? 0.f : g.offset;
+    if (g.csr_off)
+      rc = launch_grad_planes_csr(z, ldz, nq, m, g.csr_off, g.csr_col, g.csr_a, g.csr_b, row_stat, off, g.inv_batch,
+                                  SG.hi, SG.lo, Ep, SGT.hi, SGT.lo, Np, SG.inv_scale, SGT.inv_scale, st);
+    else
+      rc = launch_grad_planes(z, ldz, nq, m, g.lab, nullptr, 0, row_stat, off, 1.0f / (float)n, SG.hi, SG.lo, Ep,
+                              SGT.hi, SGT.lo, Np, SG.inv_scale, SGT.inv_scale, st);
+    if (rc) return rc;
   }
   // 3. transposed operands T^T [K, E] and Q^T [K, nq], then their planes
   float* Tt = (float*)ws.take((size_t)K * ldE * 4);
@@ -890,6 +900,50 @@ int backward_block(int model, const Rows& E, const Rows& R, const int64_t* tripl
   if ((rc = gemm_planes(SGT, SQt, d_ent + col_off, lde, st))) return rc;
   return gemm_planes(SG, STt, dQ, ldq, st);
   // 5. (caller) unfold dQ into the rows of the batch — after EVERY block has stored its dT columns
+}
+
+// The two row-gradient passes of the distance family (grad_distance.cu) with weights W = dL/dz [nq, m]: Wt = W^T,
+// dQ [nq, ldq] from the queries Q against the table T, dT [m, ldt] from T against Q.  Each pass reads its weights
+// transposed ([column, row]): the other pass's orientation.
+int distance_rowgrads(int pair_op, const float* Q, int64_t ldq, int64_t nq, const Rows& T, int K, const float* W,
+                      int64_t ldw, float* Wt, float* dQ, float* dT, int64_t ldt, cudaStream_t st) {
+  const int64_t m = T.rows, ldN = round_up(nq, 4);
+  int rc;
+  if ((rc = launch_transpose(W, ldw, nq, m, Wt, ldN, st))) return rc;
+  if ((rc = launch_pair_rowgrad(pair_op, Q, ldq, nq, T.base, T.ld, m, K, Wt, ldN, dQ, ldq, st))) return rc;
+  return launch_pair_rowgrad(pair_op, T.base, T.ld, m, Q, ldq, nq, K, W, ldw, dT, ldt, st);
+}
+
+// The distance-family backward of the pre-folded queries B.Qpre (nq rows) against the plain table B.cand, one-hot
+// labels: scores by the CUDA-core scorer, the KL row statistics, dense G, then both row-gradient passes into dQ and
+// dT.  The caller unfolds dQ.
+int distance_backward(const Block& B, float l_norm, const GradSpec& g, float* dQ, float* dT, int64_t ldt, Arena& ws,
+                      cudaStream_t st) {
+  const Folded f = folded_problem(B.model, B.combine, B.cand->dim, l_norm);
+  const int64_t nq = B.q1 ? 2 * B.n : B.n, m = B.cand->rows, ldz = round_up(m, 4), ldN = round_up(nq, 4);
+  const bool kl = g.loss_kind == B200KGE_LOSS_KL;
+  float* z = (float*)ws.take((size_t)nq * ldz * 4);
+  float* G = (float*)ws.take((size_t)nq * ldz * 4);
+  float* Gt = (float*)ws.take((size_t)m * ldN * 4);
+  float* row_stat = kl ? (float*)ws.take((size_t)nq * 2 * 4) : nullptr;
+  if (!z || !G || !Gt || (kl && !row_stat)) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
+  EpiParams P = empty_epi();
+  P.out = z; P.ldo = ldz;
+  int rc;
+  if ((rc = run_block(B, l_norm, B200KGE_PREC_AUTO, EPI_STORE, P, ws, st, nullptr))) return rc;
+  if (kl && (rc = launch_row_lse(z, ldz, nq, m, g.lab, row_stat, st))) return rc;
+  if ((rc = launch_grad_dense(z, ldz, nq, m, g.lab, row_stat, kl ? 0.f : g.offset, 1.0f / (float)B.n,
+                              f.pair_op == PAIR_L2, G, ldz, st))) return rc;
+  return distance_rowgrads(f.pair_op, B.Qpre, round_up(f.K, 32), nq, *B.cand, f.K, G, ldz, Gt, dQ, dT, ldt, st);
+}
+
+// the distance-family backward covers these pairings only
+int check_distance_pair(int pair_op) {
+  if (pair_op != PAIR_L1 && pair_op != PAIR_L2 && pair_op != PAIR_CMOD_L1) {
+    set_error("the distance-family backward covers l_norm 1 and 2 (TransE) and 1 (RotatE)");
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  return 0;
 }
 
 size_t backward_block_bytes(int64_t nq, int64_t m, int64_t K, int64_t ldq) {
@@ -941,59 +995,39 @@ static int train_1vsall_backward_impl(int model, float l_norm, const b200kge_row
                                       const int64_t* triples, int64_t n, int loss_kind, float offset, float* d_ent,
                                       int64_t lde, float* d_rel, int64_t ldr, void* workspace, size_t workspace_bytes,
                                       b200kge_stream_t stream, int64_t num_rel) {
-  if (!ent || !rel || !triples || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
-  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
-  if ((rc = validate_norm(model, l_norm))) return rc;
-  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
-  if (lde < ent->dim || ldr < rel->dim) { set_error("gradient leading dimensions are smaller than the table widths"); return B200KGE_ERR_INVALID; }
+  if (!triples || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
+  if ((rc = check_loss_kind(loss_kind))) return rc;
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   Rows E = to_rows(ent), R = to_rows(rel);
   B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
   if (n <= 0) { B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st)); return 0; }
   Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
   if (model == B200KGE_TRANSE || model == B200KGE_ROTATE) {
-    // distance family (grad_distance.cu): scores by the CUDA-core scorer, dense G, two row-gradient passes, unfold
     Folded f = folded_problem(model, B200KGE_SP_, E.dim, l_norm);
-    if (f.pair_op != PAIR_L1 && f.pair_op != PAIR_L2 && f.pair_op != PAIR_CMOD_L1) {
-      set_error("the distance-family backward covers l_norm 1 and 2 (TransE) and 1 (RotatE)");
-      return B200KGE_ERR_UNSUPPORTED;
-    }
-    const int64_t nq = 2 * n, m = E.rows, ldq = round_up(f.K, 32), ldz = round_up(m, 4), ldN = round_up(nq, 4);
+    if ((rc = check_distance_pair(f.pair_op))) return rc;
+    const int64_t nq = 2 * n, ldq = round_up(f.K, 32);
     float* Q = (float*)ws.take((size_t)nq * ldq * 4);
     float* dQ = (float*)ws.take((size_t)nq * ldq * 4);
     int64_t* lab = (int64_t*)ws.take((size_t)nq * 8);
-    float* z = (float*)ws.take((size_t)nq * ldz * 4);
-    float* G = (float*)ws.take((size_t)nq * ldz * 4);
-    float* Gt = (float*)ws.take((size_t)m * ldN * 4);
-    float* row_stat = loss_kind == B200KGE_LOSS_KL ? (float*)ws.take((size_t)nq * 2 * 4) : nullptr;
-    if (!Q || !dQ || !lab || !z || !G || !Gt || (loss_kind == B200KGE_LOSS_KL && !row_stat)) {
-      set_error("workspace too small");
-      return B200KGE_ERR_WORKSPACE;
-    }
+    if (!Q || !dQ || !lab) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
     if ((rc = launch_prep_1vsall(model, E, R, triples, n, Q, ldq, lab, nullptr, st, num_rel))) return rc;
-    {
-      Rows S = E; S.idx = lab; S.rows = n;      // placeholders: operands are pre-folded
-      Rows Pr = R; Pr.idx = lab; Pr.rows = n;
-      EpiParams P = empty_epi();
-      P.out = z; P.ldo = ldz;
-      Block B{model, B200KGE_SP_, &S, &S, &Pr, &E, n};
-      B.Qpre = Q;
-      B.same_fold = num_rel > 0;
-      if ((rc = run_block(B, l_norm, B200KGE_PREC_AUTO, EPI_STORE, P, ws, st, nullptr))) return rc;
-    }
-    if (row_stat && (rc = launch_row_lse(z, ldz, nq, m, lab, row_stat, st))) return rc;
-    if ((rc = launch_grad_dense(z, ldz, nq, m, lab, row_stat, loss_kind == B200KGE_LOSS_KL ? 0.f : offset, 1.0f / (float)n,
-                                f.pair_op == PAIR_L2, G, ldz, st))) return rc;
-    if ((rc = launch_transpose(G, ldz, nq, m, Gt, ldN, st))) return rc;
-    // each pass reads its weights transposed ([column, row]): the other pass's orientation
-    if ((rc = launch_pair_rowgrad(f.pair_op, Q, ldq, nq, E.base, E.ld, m, f.K, Gt, ldN, dQ, ldq, st))) return rc;
-    if ((rc = launch_pair_rowgrad(f.pair_op, E.base, E.ld, m, Q, ldq, nq, f.K, G, ldz, d_ent, lde, st))) return rc;
+    Rows S = E; S.idx = lab; S.rows = n;      // placeholders: operands are pre-folded
+    Rows Pr = R; Pr.idx = lab; Pr.rows = n;
+    Block B{model, B200KGE_SP_, &S, &S, &Pr, &E, n};
+    B.Qpre = Q;
+    B.same_fold = num_rel > 0;
+    GradSpec g;
+    g.lab = lab; g.loss_kind = loss_kind; g.offset = offset;
+    if ((rc = distance_backward(B, l_norm, g, dQ, d_ent, lde, ws, st))) return rc;
     return launch_unfold_distance(model, E, R, triples, n, -1, dQ, ldq, d_ent, lde, d_rel, ldr, st, num_rel);
   }
   Folded f0 = folded_problem(model, B200KGE_SP_, E.dim, 1.0f),
          f1 = folded_problem(model, num_rel > 0 ? B200KGE_SP_ : B200KGE__PO, E.dim, 1.0f);
   const int64_t ldq = round_up(f0.K, 32);
+  GradSpec g;
+  g.loss_kind = loss_kind; g.offset = offset;
   if (f0.col_off == f1.col_off) {
     float* Q = (float*)ws.take((size_t)(2 * n) * ldq * 4);
     int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
@@ -1003,8 +1037,8 @@ static int train_1vsall_backward_impl(int model, float l_norm, const b200kge_row
     if ((rc = launch_prep_1vsall(model, E, R, triples, n, Q, ldq, lab, nullptr, st, num_rel))) return rc;
     // reciprocal CP: the table GEMM stores columns [h, D) only; the unfold adds the rows' [0, h) into zeros
     if (f0.col_off > 0) B2K_CUDA(cudaMemset2DAsync(d_ent, (size_t)lde * 4, 0, (size_t)f0.col_off * 4, (size_t)E.rows, st));
-    if ((rc = backward_block(model, E, R, triples, n, -1, Q, ldq, lab, f0.col_off, f0.K, loss_kind, offset, d_ent, lde, dQ, ws, st,
-                             nullptr, 0, nullptr, nullptr, 1.f, 0.f, 0.f, num_rel > 0))) return rc;
+    g.lab = lab;
+    if ((rc = backward_block(model, E, R, n, -1, num_rel > 0, Q, ldq, f0.col_off, f0.K, g, d_ent, lde, dQ, ws, st))) return rc;
     return launch_unfold(model, E, R, triples, n, -1, dQ, ldq, d_ent, lde, d_rel, ldr, st, num_rel);
   }
   // CP: the two directions pair with different halves of the candidate columns
@@ -1015,16 +1049,14 @@ static int train_1vsall_backward_impl(int model, float l_norm, const b200kge_row
   float* Q = (float*)ws.take((size_t)n * ldq * 4);
   float* dQ2 = (float*)ws.take((size_t)(2 * n) * ldq * 4);
   if (!sidx || !pidx || !oidx || !lab || !Q || !dQ2) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
-  unpack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(triples, n, sidx, pidx, oidx, lab);
-  B2K_LAUNCH_CHECK("unpack_triples_kernel");
-  Rows S = E; S.idx = sidx; S.rows = n;
-  Rows O = E; O.idx = oidx; O.rows = n;
-  Rows Pr = R; Pr.idx = pidx; Pr.rows = n;
+  Rows S, O, Pr;
+  if ((rc = unpack_triples(triples, n, sidx, pidx, oidx, lab, E, R, S, O, Pr, st))) return rc;
   for (int dir = 0; dir < 2; ++dir) {
     const Folded& f = dir == 0 ? f0 : f1;
     if ((rc = launch_fold_queries(model, dir, dir == 0 ? S : O, Pr, n, 0, Q, ldq, st))) return rc;
-    if ((rc = backward_block(model, E, R, triples, n, dir, Q, ldq, lab + dir * n, f.col_off, f.K, loss_kind, offset, d_ent,
-                             lde, dQ2 + (size_t)dir * n * ldq, ws, st))) return rc;
+    g.lab = lab + dir * n;
+    if ((rc = backward_block(model, E, R, n, dir, false, Q, ldq, f.col_off, f.K, g, d_ent, lde,
+                             dQ2 + (size_t)dir * n * ldq, ws, st))) return rc;
   }
   // both halves of the dense column gradient are stored: now add the batch rows' own gradients
   for (int dir = 0; dir < 2; ++dir)
@@ -1054,20 +1086,16 @@ int b200kge_score_1vsN_backward(int model, int combine, float l_norm, const b200
                                 const int64_t* q_idx, const int64_t* p_idx, int64_t n, const float* grad_scores,
                                 int64_t ldg, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
                                 size_t workspace_bytes, b200kge_stream_t stream) {
-  if (!ent || !rel || !q_idx || !p_idx || !grad_scores || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
+  if (!q_idx || !p_idx || !grad_scores || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
-  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
-  if ((rc = validate_norm(model, l_norm))) return rc;
-  if (lde < ent->dim || ldr < rel->dim || ldg < ent->rows) { set_error("leading dimensions too small"); return B200KGE_ERR_INVALID; }
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
+  if (ldg < ent->rows) { set_error("grad_scores is narrower than the entity table"); return B200KGE_ERR_INVALID; }
   const bool distance = (model == B200KGE_TRANSE || model == B200KGE_ROTATE);
   cudaStream_t st = (cudaStream_t)stream;
   Rows E = to_rows(ent), R = to_rows(rel);
   Folded f = folded_problem(model, combine, E.dim, l_norm);
-  if (distance && f.pair_op != PAIR_L1 && f.pair_op != PAIR_L2 && f.pair_op != PAIR_CMOD_L1) {
-    set_error("the distance-family backward covers l_norm 1 and 2 (TransE) and 1 (RotatE)");
-    return B200KGE_ERR_UNSUPPORTED;
-  }
+  if (distance && (rc = check_distance_pair(f.pair_op))) return rc;
   B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
   B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st));
   if (n <= 0) return 0;
@@ -1084,7 +1112,7 @@ int b200kge_score_1vsN_backward(int model, int combine, float l_norm, const b200
   Rows Pr = R; Pr.idx = p_idx; Pr.rows = n;
   if ((rc = launch_fold_queries(model, combine, A, Pr, n, 0, Q, ldq, st))) return rc;
   if (distance) {
-    // grad_distance.cu: W = dL/dscores (L2: divided by the recomputed scores), then the two row-gradient passes
+    // W = dL/dscores (L2: divided by the recomputed scores), then the two row-gradient passes
     const int64_t m = E.rows, ldz = round_up(m, 4), ldN = round_up(n, 4);
     const float* W = grad_scores;
     int64_t ldw = ldg;
@@ -1102,13 +1130,12 @@ int b200kge_score_1vsN_backward(int model, int combine, float l_norm, const b200
     }
     float* Wt = (float*)ws.take((size_t)m * ldN * 4);
     if (!Wt) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
-    if ((rc = launch_transpose(W, ldw, n, m, Wt, ldN, st))) return rc;
-    if ((rc = launch_pair_rowgrad(f.pair_op, Q, ldq, n, E.base, E.ld, m, f.K, Wt, ldN, dQ, ldq, st))) return rc;
-    if ((rc = launch_pair_rowgrad(f.pair_op, E.base, E.ld, m, Q, ldq, n, f.K, W, ldw, d_ent, lde, st))) return rc;
+    if ((rc = distance_rowgrads(f.pair_op, Q, ldq, n, E, f.K, W, ldw, Wt, dQ, d_ent, lde, st))) return rc;
     return launch_unfold_distance(model, E, R, tri, n, combine, dQ, ldq, d_ent, lde, d_rel, ldr, st);
   }
-  if ((rc = backward_block(model, E, R, tri, n, combine, Q, ldq, nullptr, f.col_off, f.K, B200KGE_LOSS_BCE, 0.f, d_ent, lde, dQ,
-                           ws, st, grad_scores, ldg))) return rc;
+  GradSpec g;
+  g.G = grad_scores; g.ldg = ldg;
+  if ((rc = backward_block(model, E, R, n, combine, false, Q, ldq, f.col_off, f.K, g, d_ent, lde, dQ, ws, st))) return rc;
   return launch_unfold(model, E, R, tri, n, combine, dQ, ldq, d_ent, lde, d_rel, ldr, st);
 }
 
@@ -1117,14 +1144,13 @@ int b200kge_score_1vsN_loss_csr_backward(int model, int combine, const b200kge_r
                                          const int64_t* csr_col, float label_smoothing, int loss_kind, float offset,
                                          int64_t batch_size, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
                                          void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
-  if (!ent || !rel || !q_idx || !p_idx || !csr_off || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
+  if (!q_idx || !p_idx || !csr_off || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
-  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
+  int rc = check_tables(model, 1.0f, ent, rel); if (rc) return rc;      // the dot family folds with l_norm 1
   if (model > B200KGE_RESCAL) { set_error("the tensor-core backward covers the dot family only (model %d)", model); return B200KGE_ERR_UNSUPPORTED; }
-  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  if ((rc = check_loss_kind(loss_kind))) return rc;
   if (batch_size <= 0 || !(label_smoothing >= 0.f && label_smoothing < 1.f)) { set_error("bad batch_size / label_smoothing"); return B200KGE_ERR_INVALID; }
-  if (lde < ent->dim || ldr < rel->dim) { set_error("leading dimensions too small"); return B200KGE_ERR_INVALID; }
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   Rows E = to_rows(ent), R = to_rows(rel);
   B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
@@ -1142,9 +1168,8 @@ int b200kge_score_1vsN_loss_csr_backward(int model, int combine, const b200kge_r
   Rows A = E; A.idx = q_idx; A.rows = n;
   Rows Pr = R; Pr.idx = p_idx; Pr.rows = n;
   if ((rc = launch_fold_queries(model, combine, A, Pr, n, 0, Q, ldq, st))) return rc;
-  const float a = 1.0f - label_smoothing, b = label_smoothing > 0.f ? 1.0f / (float)E.rows : 0.f;
-  if ((rc = backward_block(model, E, R, tri, n, combine, Q, ldq, q_idx /* placeholder index vector */, f.col_off, f.K, loss_kind,
-                           offset, d_ent, lde, dQ, ws, st, nullptr, 0, csr_off, csr_col, a, b, 1.0f / (float)batch_size))) return rc;
+  const GradSpec g = csr_grad(q_idx, csr_off, csr_col, label_smoothing, E.rows, batch_size, loss_kind, offset);
+  if ((rc = backward_block(model, E, R, n, combine, false, Q, ldq, f.col_off, f.K, g, d_ent, lde, dQ, ws, st))) return rc;
   return launch_unfold(model, E, R, tri, n, combine, dQ, ldq, d_ent, lde, d_rel, ldr, st);
 }
 
@@ -1167,12 +1192,10 @@ int b200kge_ns_backward(int model, float l_norm, const b200kge_rows_t* ent, cons
                           const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, float offset,
                           int64_t batch_size, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
                           size_t workspace_bytes, b200kge_stream_t stream) {
-  if (!ent || !rel || !triples || (!neg && n * K > 0) || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
-  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
-  if ((rc = validate_norm(model, l_norm))) return rc;
+  if (!triples || (!neg && n * K > 0) || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
   if (batch_size <= 0) { set_error("batch_size must be positive"); return B200KGE_ERR_INVALID; }
-  if (lde < ent->dim || ldr < rel->dim) { set_error("gradient leading dimensions are smaller than the table widths"); return B200KGE_ERR_INVALID; }
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
   Rows E = to_rows(ent), R = to_rows(rel);
   Folded f = folded_problem(model, B200KGE_SP_, E.dim, l_norm);
   const int64_t ldq = round_up(f.K, 32);
@@ -1187,12 +1210,10 @@ int b200kge_ns_backward_grad(int model, float l_norm, const b200kge_rows_t* ent,
                              const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K,
                              const float* grad_scores, int64_t ldg, float* d_ent, int64_t lde, float* d_rel,
                              int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
-  if (!ent || !rel || !triples || (!neg && n * K > 0) || (!grad_scores && n > 0) || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
-  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
-  if ((rc = validate_norm(model, l_norm))) return rc;
+  if (!triples || (!neg && n * K > 0) || (!grad_scores && n > 0) || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
   if (ldg < K + 1) { set_error("grad_scores is narrower than the 1 + K columns of the block"); return B200KGE_ERR_INVALID; }
-  if (lde < ent->dim || ldr < rel->dim) { set_error("gradient leading dimensions are smaller than the table widths"); return B200KGE_ERR_INVALID; }
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
   Rows E = to_rows(ent), R = to_rows(rel);
   Folded f = folded_problem(model, B200KGE_SP_, E.dim, l_norm);
   const int64_t ldq = round_up(f.K, 32);
@@ -1245,7 +1266,7 @@ int b200kge_score_1vsN_loss_csr(int model, int combine, float l_norm, int precis
   if ((rc = validate_norm(model, l_norm))) return rc;
   if (!csr_off || (!csr_col && nnz > 0) || !loss_out || nnz < 0) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (cand->idx) { set_error("CSR labels address the columns of a plain candidate table (cand.idx must be NULL)"); return B200KGE_ERR_INVALID; }
-  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  if ((rc = check_loss_kind(loss_kind))) return rc;
   if (!(label_smoothing >= 0.f && label_smoothing < 1.f)) { set_error("label_smoothing must be in [0, 1)"); return B200KGE_ERR_INVALID; }
   const bool dot = model <= B200KGE_RESCAL;
   if (label_smoothing > 0.f && !dot) { set_error("label smoothing with CSR labels is available for the dot family"); return B200KGE_ERR_UNSUPPORTED; }
@@ -1400,62 +1421,6 @@ size_t masked_bytes(int model, int64_t n, int64_t E, int32_t D) {
          + (size_t)n * 2 * 4 + 4096;                           // KL row statistics, scalars
 }
 
-// One direction of the masked backward: gather, fold, dT and dQ (tensor-core GEMMs or the distance row-gradient
-// passes), unfold into the per-row buffers, then d_ent[:, cols] += mask_t * dT, d_ent[q] += mask_q * dQe,
-// d_rel[p] += mask_r * dPr.  Labels: lab (one per row, 1vsAll, scaled 1/n) or the CSR of a KvsAll query type.
-struct DirGrad {
-  const int64_t* lab;
-  const int64_t* csr_off; const int64_t* csr_col; float csr_a, csr_b, inv_batch;
-  int loss_kind; float offset;
-};
-// `dir` is the fold (query type); `mask_dir` picks the draws (they differ for the reciprocal direction: sp_ fold, _po
-// draws).
-int dropout_backward_dir(int model, float l_norm, int dir, int mask_dir, const Rows& E, const Rows& R, const int64_t* q_idx,
-                         const int64_t* p_idx, int64_t n, const b200kge_dropout_t& d, const DirGrad& g,
-                         const MaskedOps& o, float* Q, float* dQ, float* dT, float* dQe, float* dPr, const int64_t* tri,
-                         Arena ws, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, cudaStream_t st) {
-  const DirMasks m = dir_masks(d, mask_dir);
-  const Folded f = folded_problem(model, dir, E.dim, l_norm);
-  const int64_t ldq = round_up(f.K, 32), mE = E.rows;
-  const int D = E.dim, Dr = R.dim;
-  Rows Qr, Pr, Tr;
-  int rc = gather_masked(m, E, R, q_idx, p_idx, n, o, Qr, Pr, Tr, st);
-  if (rc) return rc;
-  if ((rc = launch_fold_queries(model, dir, Qr, Pr, n, 0, Q, ldq, st))) return rc;
-  B2K_CUDA(cudaMemsetAsync(dQe, 0, (size_t)n * D * 4, st));
-  B2K_CUDA(cudaMemsetAsync(dPr, 0, (size_t)n * Dr * 4, st));
-  if (f.pair_op == PAIR_DOT) {
-    if ((rc = backward_block(model, Tr, Pr, tri, n, dir, Q, ldq, g.lab, f.col_off, f.K, g.loss_kind, g.offset, dT, D, dQ,
-                             ws, st, nullptr, 0, g.csr_off, g.csr_col, g.csr_a, g.csr_b, g.inv_batch))) return rc;
-    if ((rc = launch_unfold(model, Qr, Pr, tri, n, dir, dQ, ldq, dQe, D, dPr, Dr, st))) return rc;
-  } else {
-    // distance family: scores by the CUDA-core scorer, dense G, the two row-gradient passes (as the stacked step)
-    const int64_t ldz = round_up(mE, 4), ldN = round_up(n, 4);
-    float* z = (float*)ws.take((size_t)n * ldz * 4);
-    float* G = (float*)ws.take((size_t)n * ldz * 4);
-    float* Gt = (float*)ws.take((size_t)mE * ldN * 4);
-    float* row_stat = g.loss_kind == B200KGE_LOSS_KL ? (float*)ws.take((size_t)n * 2 * 4) : nullptr;
-    if (!z || !G || !Gt || (g.loss_kind == B200KGE_LOSS_KL && !row_stat)) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
-    {
-      EpiParams P = empty_epi();
-      P.out = z; P.ldo = ldz;
-      Block B{model, dir, &Qr, nullptr, &Pr, &Tr, n};
-      B.Qpre = Q;
-      if ((rc = run_block(B, l_norm, B200KGE_PREC_AUTO, EPI_STORE, P, ws, st, nullptr))) return rc;
-    }
-    if (row_stat && (rc = launch_row_lse(z, ldz, n, mE, g.lab, row_stat, st))) return rc;
-    if ((rc = launch_grad_dense(z, ldz, n, mE, g.lab, row_stat, g.loss_kind == B200KGE_LOSS_KL ? 0.f : g.offset,
-                                1.0f / (float)n, f.pair_op == PAIR_L2, G, ldz, st))) return rc;
-    if ((rc = launch_transpose(G, ldz, n, mE, Gt, ldN, st))) return rc;
-    if ((rc = launch_pair_rowgrad(f.pair_op, Q, ldq, n, Tr.base, Tr.ld, mE, f.K, Gt, ldN, dQ, ldq, st))) return rc;
-    if ((rc = launch_pair_rowgrad(f.pair_op, Tr.base, Tr.ld, mE, Q, ldq, n, f.K, G, ldz, dT, D, st))) return rc;
-    if ((rc = launch_unfold_distance(model, Qr, Pr, tri, n, dir, dQ, ldq, dQe, D, dPr, Dr, st))) return rc;
-  }
-  if ((rc = launch_dropout_add_cols(m.t, dT, D, mE, D, f.col_off, f.col_off + f.K, d_ent, lde, st))) return rc;
-  if ((rc = launch_dropout_scatter(m.q, dQe, D, n, D, q_idx, d_ent, lde, st))) return rc;
-  return launch_dropout_scatter(m.r, dPr, Dr, n, Dr, p_idx, d_rel, ldr, st);
-}
-
 // the per-direction buffers of the backward
 struct BackBufs { MaskedOps o; float *Q, *dQ, *dT, *dQe, *dPr; int64_t* tri; };
 bool take_back(Arena& ws, int64_t n, int64_t E, int D, int Dr, int64_t ldq, BackBufs& b) {
@@ -1467,6 +1432,37 @@ bool take_back(Arena& ws, int64_t n, int64_t E, int D, int Dr, int64_t ldq, Back
   b.dPr = (float*)ws.take((size_t)n * Dr * 4);
   b.tri = (int64_t*)ws.take((size_t)n * 3 * 8);
   return b.Q && b.dQ && b.dT && b.dQe && b.dPr && b.tri;
+}
+
+// One direction of the masked backward: gather, fold, dT and dQ (tensor-core GEMMs or the distance row-gradient
+// passes), unfold into the per-row buffers, then d_ent[:, cols] += mask_t * dT, d_ent[q] += mask_q * dQe,
+// d_rel[p] += mask_r * dPr.  `dir` is the fold (query type); `mask_dir` picks the draws (they differ for the
+// reciprocal direction: sp_ fold, _po draws).
+int dropout_backward_dir(int model, float l_norm, int dir, int mask_dir, const Rows& E, const Rows& R, const int64_t* q_idx,
+                         const int64_t* p_idx, int64_t n, const b200kge_dropout_t& d, const GradSpec& g,
+                         const BackBufs& b, Arena ws, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, cudaStream_t st) {
+  const DirMasks m = dir_masks(d, mask_dir);
+  const Folded f = folded_problem(model, dir, E.dim, l_norm);
+  const int64_t ldq = round_up(f.K, 32), mE = E.rows;
+  const int D = E.dim, Dr = R.dim;
+  Rows Qr, Pr, Tr;
+  int rc = gather_masked(m, E, R, q_idx, p_idx, n, b.o, Qr, Pr, Tr, st);
+  if (rc) return rc;
+  if ((rc = launch_fold_queries(model, dir, Qr, Pr, n, 0, b.Q, ldq, st))) return rc;
+  B2K_CUDA(cudaMemsetAsync(b.dQe, 0, (size_t)n * D * 4, st));
+  B2K_CUDA(cudaMemsetAsync(b.dPr, 0, (size_t)n * Dr * 4, st));
+  if (f.pair_op == PAIR_DOT) {
+    if ((rc = backward_block(model, Tr, Pr, n, dir, false, b.Q, ldq, f.col_off, f.K, g, b.dT, D, b.dQ, ws, st))) return rc;
+    if ((rc = launch_unfold(model, Qr, Pr, b.tri, n, dir, b.dQ, ldq, b.dQe, D, b.dPr, Dr, st))) return rc;
+  } else {
+    Block B{model, dir, &Qr, nullptr, &Pr, &Tr, n};
+    B.Qpre = b.Q;
+    if ((rc = distance_backward(B, l_norm, g, b.dQ, b.dT, D, ws, st))) return rc;
+    if ((rc = launch_unfold_distance(model, Qr, Pr, b.tri, n, dir, b.dQ, ldq, b.dQe, D, b.dPr, Dr, st))) return rc;
+  }
+  if ((rc = launch_dropout_add_cols(m.t, b.dT, D, mE, D, f.col_off, f.col_off + f.K, d_ent, lde, st))) return rc;
+  if ((rc = launch_dropout_scatter(m.q, b.dQe, D, n, D, q_idx, d_ent, lde, st))) return rc;
+  return launch_dropout_scatter(m.r, b.dPr, Dr, n, Dr, p_idx, d_rel, ldr, st);
 }
 
 Arena rest_of(const Arena& ws) {
@@ -1493,169 +1489,116 @@ size_t b200kge_train_1vsall_dropout_workspace_bytes(int model, int64_t n, int64_
   return masked_bytes(model, n, E, D) + (dir > fwd ? dir : fwd);
 }
 
-int b200kge_train_1vsall_forward_dropout(int model, float l_norm, int precision, const b200kge_rows_t* ent,
-                                         const b200kge_rows_t* rel, const int64_t* triples, int64_t n, int loss_kind,
-                                         float offset, const b200kge_dropout_t* drop, float* loss_out, void* workspace,
-                                         size_t workspace_bytes, b200kge_stream_t stream) {
-  if (!ent || !rel || !triples || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
-  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
-  if ((rc = validate_norm(model, l_norm))) return rc;
-  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+// The 1vsAll step under embedding dropout; the masks of direction dir are drawn on dir's streams.  num_rel > 0: the
+// reciprocal-relations step (reciprocal_relations_model.py:85-92): both directions are sp_ queries against the table;
+// the second one, (o, p + R) labelled s, is score_po and draws its masks on the _po streams in the reference's call
+// order (embed_all: B200KGE_DROP_PO_TABLE, embed(p + R): B200KGE_DROP_PO_REL, embed(o): B200KGE_DROP_PO_ENT).
+static int train_1vsall_forward_dropout_impl(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                                             const b200kge_rows_t* rel, const int64_t* triples, int64_t n,
+                                             int loss_kind, float offset, const b200kge_dropout_t* drop,
+                                             float* loss_out, void* workspace, size_t workspace_bytes,
+                                             cudaStream_t st, int64_t num_rel) {
+  if (!triples || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
+  if ((rc = check_loss_kind(loss_kind))) return rc;
   if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
   if (n <= 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
   Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
   Rows E = to_rows(ent), R = to_rows(rel);
   int64_t* sidx = (int64_t*)ws.take((size_t)n * 8);
   int64_t* pidx = (int64_t*)ws.take((size_t)n * 8);
   int64_t* oidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* pinv = num_rel > 0 ? (int64_t*)ws.take((size_t)n * 8) : nullptr;
   int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
   float* dir_loss = (float*)ws.take(256);
   MaskedOps o;
-  if (!sidx || !pidx || !oidx || !lab || !dir_loss || !take_masked(ws, n, E.rows, E.dim, R.dim, o)) {
-    set_error("workspace too small (see b200kge_train_1vsall_dropout_workspace_bytes)");
+  if (!sidx || !pidx || !oidx || (num_rel > 0 && !pinv) || !lab || !dir_loss ||
+      !take_masked(ws, n, E.rows, E.dim, R.dim, o)) {
+    set_error("workspace too small (see b200kge_train_1vsall_%s_workspace_bytes)", num_rel > 0 ? "reciprocal" : "dropout");
     return B200KGE_ERR_WORKSPACE;
   }
-  unpack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(triples, n, sidx, pidx, oidx, lab);
-  B2K_LAUNCH_CHECK("unpack_triples_kernel");
+  Rows S, O, P;
+  if ((rc = unpack_triples(triples, n, sidx, pidx, oidx, lab, E, R, S, O, P, st))) return rc;
+  if (num_rel > 0) {
+    offset_index_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pidx, n, num_rel, pinv);
+    B2K_LAUNCH_CHECK("offset_index_kernel");
+  }
   const Arena rest = rest_of(ws);
   for (int dir = 0; dir < 2; ++dir) {
     Rows Qr, Pr, Tr;
-    if ((rc = gather_masked(dir_masks(*drop, dir), E, R, dir == 0 ? sidx : oidx, pidx, n, o, Qr, Pr, Tr, st))) return rc;
+    if ((rc = gather_masked(dir_masks(*drop, dir), E, R, dir == 0 ? sidx : oidx, dir == 1 && pinv ? pinv : pidx, n, o,
+                            Qr, Pr, Tr, st))) return rc;
     const b200kge_rows_t q{Qr.base, nullptr, n, Qr.ld, Qr.dim}, p{Pr.base, nullptr, n, Pr.ld, Pr.dim},
         c{Tr.base, nullptr, Tr.rows, Tr.ld, Tr.dim};
     const b200kge_labels_t labels{lab + dir * n, nullptr, 0};
-    if ((rc = b200kge_score_1vsN_loss(model, dir, l_norm, precision, &q, &p, &c, n, &labels, loss_kind, offset,
-                                      dir_loss + dir, nullptr, rest.base, rest.cap, stream))) return rc;
+    if ((rc = b200kge_score_1vsN_loss(model, num_rel > 0 ? B200KGE_SP_ : dir, l_norm, precision, &q, &p, &c, n, &labels,
+                                      loss_kind, offset, dir_loss + dir, nullptr, rest.base, rest.cap, st))) return rc;
   }
   return launch_rows_sum(dir_loss, 2, 1.0f / (float)n, loss_out, st);    // (loss_sp + loss_po) / n
+}
+
+// the backward of train_1vsall_forward_dropout_impl
+static int train_1vsall_backward_dropout_impl(int model, float l_norm, const b200kge_rows_t* ent,
+                                              const b200kge_rows_t* rel, const int64_t* triples, int64_t n,
+                                              int loss_kind, float offset, const b200kge_dropout_t* drop, float* d_ent,
+                                              int64_t lde, float* d_rel, int64_t ldr, void* workspace,
+                                              size_t workspace_bytes, cudaStream_t st, int64_t num_rel) {
+  if (!triples || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
+  if ((rc = check_loss_kind(loss_kind))) return rc;
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
+  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
+  const Folded f = folded_problem(model, B200KGE_SP_, ent->dim, l_norm);
+  if (f.pair_op != PAIR_DOT && (rc = check_distance_pair(f.pair_op))) return rc;
+  Rows E = to_rows(ent), R = to_rows(rel);
+  B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
+  B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st));
+  if (n <= 0) return 0;
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  int64_t* sidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* pidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* oidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* pinv = num_rel > 0 ? (int64_t*)ws.take((size_t)n * 8) : nullptr;
+  int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
+  BackBufs b;
+  if (!sidx || !pidx || !oidx || (num_rel > 0 && !pinv) || !lab ||
+      !take_back(ws, n, E.rows, E.dim, R.dim, round_up(f.K, 32), b)) {
+    set_error("workspace too small (see b200kge_train_1vsall_%s_workspace_bytes)", num_rel > 0 ? "reciprocal" : "dropout");
+    return B200KGE_ERR_WORKSPACE;
+  }
+  Rows S, O, P;
+  if ((rc = unpack_triples(triples, n, sidx, pidx, oidx, lab, E, R, S, O, P, st))) return rc;
+  if (num_rel > 0) {
+    offset_index_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pidx, n, num_rel, pinv);
+    B2K_LAUNCH_CHECK("offset_index_kernel");
+  }
+  if ((rc = launch_identity_triples(n, b.tri, st))) return rc;
+  const Arena rest = rest_of(ws);
+  GradSpec g;
+  g.loss_kind = loss_kind; g.offset = offset;
+  for (int dir = 0; dir < 2; ++dir) {
+    g.lab = lab + dir * n;
+    if ((rc = dropout_backward_dir(model, l_norm, num_rel > 0 ? B200KGE_SP_ : dir, dir, E, R, dir == 0 ? sidx : oidx,
+                                   dir == 1 && pinv ? pinv : pidx, n, *drop, g, b, rest, d_ent, lde, d_rel, ldr, st)))
+      return rc;
+  }
+  return 0;
+}
+
+int b200kge_train_1vsall_forward_dropout(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                                         const b200kge_rows_t* rel, const int64_t* triples, int64_t n, int loss_kind,
+                                         float offset, const b200kge_dropout_t* drop, float* loss_out, void* workspace,
+                                         size_t workspace_bytes, b200kge_stream_t stream) {
+  return train_1vsall_forward_dropout_impl(model, l_norm, precision, ent, rel, triples, n, loss_kind, offset, drop,
+                                           loss_out, workspace, workspace_bytes, (cudaStream_t)stream, 0);
 }
 
 int b200kge_train_1vsall_backward_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
                                           const int64_t* triples, int64_t n, int loss_kind, float offset,
                                           const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
                                           int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
-  if (!ent || !rel || !triples || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
-  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
-  if ((rc = validate_norm(model, l_norm))) return rc;
-  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
-  if (lde < ent->dim || ldr < rel->dim) { set_error("gradient leading dimensions are smaller than the table widths"); return B200KGE_ERR_INVALID; }
-  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
-  const Folded f = folded_problem(model, B200KGE_SP_, ent->dim, l_norm);
-  if (f.pair_op != PAIR_DOT && f.pair_op != PAIR_L1 && f.pair_op != PAIR_L2 && f.pair_op != PAIR_CMOD_L1) {
-    set_error("the distance-family backward covers l_norm 1 and 2 (TransE) and 1 (RotatE)");
-    return B200KGE_ERR_UNSUPPORTED;
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  Rows E = to_rows(ent), R = to_rows(rel);
-  B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
-  B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st));
-  if (n <= 0) return 0;
-  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
-  int64_t* sidx = (int64_t*)ws.take((size_t)n * 8);
-  int64_t* pidx = (int64_t*)ws.take((size_t)n * 8);
-  int64_t* oidx = (int64_t*)ws.take((size_t)n * 8);
-  int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
-  BackBufs b;
-  if (!sidx || !pidx || !oidx || !lab || !take_back(ws, n, E.rows, E.dim, R.dim, round_up(f.K, 32), b)) {
-    set_error("workspace too small (see b200kge_train_1vsall_dropout_workspace_bytes)");
-    return B200KGE_ERR_WORKSPACE;
-  }
-  unpack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(triples, n, sidx, pidx, oidx, lab);
-  B2K_LAUNCH_CHECK("unpack_triples_kernel");
-  if ((rc = launch_identity_triples(n, b.tri, st))) return rc;
-  const Arena rest = rest_of(ws);
-  for (int dir = 0; dir < 2; ++dir) {
-    DirGrad g{lab + dir * n, nullptr, nullptr, 1.f, 0.f, 0.f, loss_kind, offset};
-    if ((rc = dropout_backward_dir(model, l_norm, dir, dir, E, R, dir == 0 ? sidx : oidx, pidx, n, *drop, g, b.o, b.Q,
-                                   b.dQ, b.dT, b.dQe, b.dPr, b.tri, rest, d_ent, lde, d_rel, ldr, st))) return rc;
-  }
-  return 0;
-}
-
-// ---- reciprocal relations (reciprocal_relations_model.py:85-92): both directions are sp_ queries against the table;
-// the second one, (o, p + R) labelled s, is score_po and draws its masks on the _po streams in the reference's call
-// order (embed_all: B200KGE_DROP_PO_TABLE, embed(p + R): B200KGE_DROP_PO_REL, embed(o): B200KGE_DROP_PO_ENT).
-
-static int recip_forward_dropout(int model, float l_norm, int precision, const b200kge_rows_t* ent,
-                                 const b200kge_rows_t* rel, int64_t num_rel, const int64_t* triples, int64_t n,
-                                 int loss_kind, float offset, const b200kge_dropout_t* drop, float* loss_out,
-                                 void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  int rc;
-  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
-  if (n <= 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
-  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
-  Rows E = to_rows(ent), R = to_rows(rel);
-  int64_t* sidx = (int64_t*)ws.take((size_t)n * 8);
-  int64_t* pidx = (int64_t*)ws.take((size_t)n * 8);
-  int64_t* oidx = (int64_t*)ws.take((size_t)n * 8);
-  int64_t* pinv = (int64_t*)ws.take((size_t)n * 8);
-  int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
-  float* dir_loss = (float*)ws.take(256);
-  MaskedOps o;
-  if (!sidx || !pidx || !oidx || !pinv || !lab || !dir_loss || !take_masked(ws, n, E.rows, E.dim, R.dim, o)) {
-    set_error("workspace too small (see b200kge_train_1vsall_reciprocal_workspace_bytes)");
-    return B200KGE_ERR_WORKSPACE;
-  }
-  unpack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(triples, n, sidx, pidx, oidx, lab);
-  B2K_LAUNCH_CHECK("unpack_triples_kernel");
-  offset_index_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pidx, n, num_rel, pinv);
-  B2K_LAUNCH_CHECK("offset_index_kernel");
-  const Arena rest = rest_of(ws);
-  for (int dir = 0; dir < 2; ++dir) {
-    Rows Qr, Pr, Tr;
-    if ((rc = gather_masked(dir_masks(*drop, dir), E, R, dir == 0 ? sidx : oidx, dir == 0 ? pidx : pinv, n, o, Qr, Pr,
-                            Tr, st))) return rc;
-    const b200kge_rows_t q{Qr.base, nullptr, n, Qr.ld, Qr.dim}, p{Pr.base, nullptr, n, Pr.ld, Pr.dim},
-        c{Tr.base, nullptr, Tr.rows, Tr.ld, Tr.dim};
-    const b200kge_labels_t labels{lab + dir * n, nullptr, 0};
-    if ((rc = b200kge_score_1vsN_loss(model, B200KGE_SP_, l_norm, precision, &q, &p, &c, n, &labels, loss_kind, offset,
-                                      dir_loss + dir, nullptr, rest.base, rest.cap, st))) return rc;
-  }
-  return launch_rows_sum(dir_loss, 2, 1.0f / (float)n, loss_out, st);
-}
-
-static int recip_backward_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                  int64_t num_rel, const int64_t* triples, int64_t n, int loss_kind, float offset,
-                                  const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                                  void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  int rc;
-  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
-  const Folded f = folded_problem(model, B200KGE_SP_, ent->dim, l_norm);
-  if (f.pair_op != PAIR_DOT && f.pair_op != PAIR_L1 && f.pair_op != PAIR_L2 && f.pair_op != PAIR_CMOD_L1) {
-    set_error("the distance-family backward covers l_norm 1 and 2 (TransE) and 1 (RotatE)");
-    return B200KGE_ERR_UNSUPPORTED;
-  }
-  Rows E = to_rows(ent), R = to_rows(rel);
-  B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
-  B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st));
-  if (n <= 0) return 0;
-  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
-  int64_t* sidx = (int64_t*)ws.take((size_t)n * 8);
-  int64_t* pidx = (int64_t*)ws.take((size_t)n * 8);
-  int64_t* oidx = (int64_t*)ws.take((size_t)n * 8);
-  int64_t* pinv = (int64_t*)ws.take((size_t)n * 8);
-  int64_t* lab = (int64_t*)ws.take((size_t)n * 2 * 8);
-  BackBufs b;
-  if (!sidx || !pidx || !oidx || !pinv || !lab || !take_back(ws, n, E.rows, E.dim, R.dim, round_up(f.K, 32), b)) {
-    set_error("workspace too small (see b200kge_train_1vsall_reciprocal_workspace_bytes)");
-    return B200KGE_ERR_WORKSPACE;
-  }
-  unpack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(triples, n, sidx, pidx, oidx, lab);
-  B2K_LAUNCH_CHECK("unpack_triples_kernel");
-  offset_index_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pidx, n, num_rel, pinv);
-  B2K_LAUNCH_CHECK("offset_index_kernel");
-  if ((rc = launch_identity_triples(n, b.tri, st))) return rc;
-  const Arena rest = rest_of(ws);
-  for (int dir = 0; dir < 2; ++dir) {
-    DirGrad g{lab + dir * n, nullptr, nullptr, 1.f, 0.f, 0.f, loss_kind, offset};
-    if ((rc = dropout_backward_dir(model, l_norm, B200KGE_SP_, dir, E, R, dir == 0 ? sidx : oidx, dir == 0 ? pidx : pinv,
-                                   n, *drop, g, b.o, b.Q, b.dQ, b.dT, b.dQe, b.dPr, b.tri, rest, d_ent, lde, d_rel, ldr,
-                                   st))) return rc;
-  }
-  return 0;
+  return train_1vsall_backward_dropout_impl(model, l_norm, ent, rel, triples, n, loss_kind, offset, drop, d_ent, lde,
+                                            d_rel, ldr, workspace, workspace_bytes, (cudaStream_t)stream, 0);
 }
 
 size_t b200kge_train_1vsall_reciprocal_workspace_bytes(int model, int64_t n, int64_t E, int32_t D) {
@@ -1676,12 +1619,8 @@ int b200kge_train_1vsall_reciprocal_forward(int model, float l_norm, int precisi
   if (!drop)
     return train_1vsall_forward_impl(model, l_norm, precision, ent, rel, triples, n, loss_kind, offset, loss_out,
                                      workspace, workspace_bytes, stream, num_relations);
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
-  if ((rc = validate_model(model, to_rows(ent), to_rows(rel)))) return rc;
-  if ((rc = validate_norm(model, l_norm))) return rc;
-  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
-  return recip_forward_dropout(model, l_norm, precision, ent, rel, num_relations, triples, n, loss_kind, offset, drop,
-                               loss_out, workspace, workspace_bytes, (cudaStream_t)stream);
+  return train_1vsall_forward_dropout_impl(model, l_norm, precision, ent, rel, triples, n, loss_kind, offset, drop,
+                                           loss_out, workspace, workspace_bytes, (cudaStream_t)stream, num_relations);
 }
 
 int b200kge_train_1vsall_reciprocal_backward(int model, float l_norm, const b200kge_rows_t* ent,
@@ -1694,13 +1633,8 @@ int b200kge_train_1vsall_reciprocal_backward(int model, float l_norm, const b200
   if (!drop)
     return train_1vsall_backward_impl(model, l_norm, ent, rel, triples, n, loss_kind, offset, d_ent, lde, d_rel, ldr,
                                       workspace, workspace_bytes, stream, num_relations);
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
-  if ((rc = validate_model(model, to_rows(ent), to_rows(rel)))) return rc;
-  if ((rc = validate_norm(model, l_norm))) return rc;
-  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
-  if (lde < ent->dim || ldr < rel->dim) { set_error("gradient leading dimensions are smaller than the table widths"); return B200KGE_ERR_INVALID; }
-  return recip_backward_dropout(model, l_norm, ent, rel, num_relations, triples, n, loss_kind, offset, drop, d_ent, lde,
-                                d_rel, ldr, workspace, workspace_bytes, (cudaStream_t)stream);
+  return train_1vsall_backward_dropout_impl(model, l_norm, ent, rel, triples, n, loss_kind, offset, drop, d_ent, lde,
+                                            d_rel, ldr, workspace, workspace_bytes, (cudaStream_t)stream, num_relations);
 }
 
 size_t b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(int model, int64_t n, int64_t E, int32_t D, int64_t nnz) {
@@ -1716,11 +1650,11 @@ int b200kge_score_1vsN_loss_csr_dropout_dir(int model, int combine, int mask_dir
                                             float offset, const b200kge_dropout_t* drop, float* loss_out,
                                             float* row_loss_out, void* workspace, size_t workspace_bytes,
                                             b200kge_stream_t stream) {
-  if (!ent || !rel || (!q_idx && n > 0) || (!p_idx && n > 0) || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
+  if ((!q_idx && n > 0) || (!p_idx && n > 0) || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
   if (mask_dir != B200KGE_SP_ && mask_dir != B200KGE__PO) { set_error("bad mask direction %d", mask_dir); return B200KGE_ERR_INVALID; }
-  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
+  // l_norm is checked by b200kge_score_1vsN_loss_csr below
+  int rc = check_tables(model, 1.0f, ent, rel); if (rc) return rc;
   if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   if (n <= 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
@@ -1759,15 +1693,14 @@ int b200kge_score_1vsN_loss_csr_backward_dropout_dir(int model, int combine, int
                                                      float offset, int64_t batch_size, const b200kge_dropout_t* drop,
                                                      float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
                                                      void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
-  if (!ent || !rel || !q_idx || !p_idx || !csr_off || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
+  if (!q_idx || !p_idx || !csr_off || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
   if (mask_dir != B200KGE_SP_ && mask_dir != B200KGE__PO) { set_error("bad mask direction %d", mask_dir); return B200KGE_ERR_INVALID; }
-  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
+  int rc = check_tables(model, 1.0f, ent, rel); if (rc) return rc;      // the dot family folds with l_norm 1
   if (model > B200KGE_RESCAL) { set_error("the tensor-core backward covers the dot family only (model %d)", model); return B200KGE_ERR_UNSUPPORTED; }
-  if (loss_kind != B200KGE_LOSS_BCE && loss_kind != B200KGE_LOSS_KL) { set_error("unknown loss kind %d", loss_kind); return B200KGE_ERR_INVALID; }
+  if ((rc = check_loss_kind(loss_kind))) return rc;
   if (batch_size <= 0 || !(label_smoothing >= 0.f && label_smoothing < 1.f)) { set_error("bad batch_size / label_smoothing"); return B200KGE_ERR_INVALID; }
-  if (lde < ent->dim || ldr < rel->dim) { set_error("leading dimensions too small"); return B200KGE_ERR_INVALID; }
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
   if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   Rows E = to_rows(ent), R = to_rows(rel);
@@ -1782,10 +1715,9 @@ int b200kge_score_1vsN_loss_csr_backward_dropout_dir(int model, int combine, int
     return B200KGE_ERR_WORKSPACE;
   }
   if ((rc = launch_identity_triples(n, b.tri, st))) return rc;
-  const float a = 1.0f - label_smoothing, bb = label_smoothing > 0.f ? 1.0f / (float)E.rows : 0.f;
-  DirGrad g{q_idx /* placeholder index vector */, csr_off, csr_col, a, bb, 1.0f / (float)batch_size, loss_kind, offset};
-  return dropout_backward_dir(model, 1.0f, combine, mask_dir, E, R, q_idx, p_idx, n, *drop, g, b.o, b.Q, b.dQ, b.dT,
-                              b.dQe, b.dPr, b.tri, rest_of(ws), d_ent, lde, d_rel, ldr, st);
+  const GradSpec g = csr_grad(q_idx, csr_off, csr_col, label_smoothing, E.rows, batch_size, loss_kind, offset);
+  return dropout_backward_dir(model, 1.0f, combine, mask_dir, E, R, q_idx, p_idx, n, *drop, g, b, rest_of(ws), d_ent, lde,
+                              d_rel, ldr, st);
 }
 
 int b200kge_score_1vsN_loss_csr_backward_dropout(int model, int combine, const b200kge_rows_t* ent,
@@ -1809,11 +1741,9 @@ namespace {
 int validate_ns_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
                         const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
                         const b200kge_dropout_t* drop) {
-  if (!ent || !rel || (!triples && n > 0) || (!neg && n * K > 0)) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if ((!triples && n > 0) || (!neg && n * K > 0)) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (n < 0 || K < 0) { set_error("negative sizes"); return B200KGE_ERR_INVALID; }
-  if (ent->idx || rel->idx) { set_error("ent/rel must be plain tables"); return B200KGE_ERR_INVALID; }
-  int rc = validate_model(model, to_rows(ent), to_rows(rel)); if (rc) return rc;
-  if ((rc = validate_norm(model, l_norm))) return rc;
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
   if (impl != B200KGE_NS_TRIPLE && impl != B200KGE_NS_BATCH) { set_error("impl must be B200KGE_NS_TRIPLE or B200KGE_NS_BATCH"); return B200KGE_ERR_INVALID; }
   if (slot != 0 && slot != 2) { set_error("negative-sampling dropout covers the S and O slots"); return B200KGE_ERR_UNSUPPORTED; }
   if ((model == B200KGE_TRANSE && l_norm != 1.0f && l_norm != 2.0f) || (model == B200KGE_ROTATE && l_norm != 1.0f)) {
@@ -1879,7 +1809,7 @@ int b200kge_ns_backward_dropout(int model, float l_norm, const b200kge_rows_t* e
   if (n == 0) return 0;
   if (!grad_scores || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (ldg < K + 1) { set_error("grad_scores is narrower than the 1 + K columns of the block"); return B200KGE_ERR_INVALID; }
-  if (lde < ent->dim || ldr < rel->dim) { set_error("gradient leading dimensions are smaller than the table widths"); return B200KGE_ERR_INVALID; }
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
   return launch_ns_dropout(model, l_norm, to_rows(ent), to_rows(rel), triples, slot, neg, n, K, impl, ns_drop_keys(*drop),
                            grad_scores, ldg, nullptr, 0, d_ent, lde, d_rel, ldr, workspace, workspace_bytes,
                            (cudaStream_t)stream);

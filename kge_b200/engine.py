@@ -703,19 +703,12 @@ def score_1vsN_loss_csr_backward(model: str, combine: str, ent, rel, q, p, csr_o
     if dropout is not None:
         ws = torch.empty(lib.b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(
             MODELS[model], n, ent.shape[0], ent.shape[1], int(cols.numel())), dtype=torch.uint8, device=dev)
-        if dropout_streams is not None:
-            _lib.check(lib.b200kge_score_1vsN_loss_csr_backward_dropout_dir(
-                MODELS[model], SP_ if combine == "sp_" else _PO, SP_ if dropout_streams == "sp_" else _PO,
-                C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(),
-                cols.data_ptr() if cols.numel() else None, label_smoothing, LOSS[loss], offset, batch_size or n,
-                C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0),
-                ws.data_ptr(), ws.numel(), _stream(dev)))
-            return d_ent, d_rel
-        _lib.check(lib.b200kge_score_1vsN_loss_csr_backward_dropout(
-            MODELS[model], SP_ if combine == "sp_" else _PO, C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n,
-            offs.data_ptr(), cols.data_ptr() if cols.numel() else None, label_smoothing, LOSS[loss], offset,
-            batch_size or n, C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(),
-            d_rel.stride(0), ws.data_ptr(), ws.numel(), _stream(dev)))
+        _lib.check(lib.b200kge_score_1vsN_loss_csr_backward_dropout_dir(
+            MODELS[model], SP_ if combine == "sp_" else _PO, SP_ if (dropout_streams or combine) == "sp_" else _PO,
+            C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(),
+            cols.data_ptr() if cols.numel() else None, label_smoothing, LOSS[loss], offset, batch_size or n,
+            C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0),
+            ws.data_ptr(), ws.numel(), _stream(dev)))
         return d_ent, d_rel
     ws = torch.empty(lib.b200kge_score_1vsN_backward_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1]),
                      dtype=torch.uint8, device=dev)
@@ -889,18 +882,11 @@ def score_1vsN_loss_csr(model: str, combine: str, q_tab, rel, cand_tab, csr_offs
         k.refs += [qi, pi]
         ws = torch.empty(lib.b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(MODELS[model], n, m, rq.dim, nnz),
                          dtype=torch.uint8, device=dev)
-        if dropout_streams is not None:
-            _lib.check(lib.b200kge_score_1vsN_loss_csr_dropout_dir(
-                MODELS[model], SP_ if combine == "sp_" else _PO, SP_ if dropout_streams == "sp_" else _PO, l_norm,
-                PREC[precision], C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(),
-                cols.data_ptr() if nnz else None, nnz, label_smoothing, LOSS[loss], offset, C.byref(dropout.struct()),
-                out.data_ptr(), rows.data_ptr() if rows is not None else None, ws.data_ptr(), ws.numel(), _stream(dev)))
-            return (out, rows) if return_rows else out
-        _lib.check(lib.b200kge_score_1vsN_loss_csr_dropout(
-            MODELS[model], SP_ if combine == "sp_" else _PO, l_norm, PREC[precision], C.byref(re_), C.byref(rr),
-            qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(), cols.data_ptr() if nnz else None, nnz, label_smoothing,
-            LOSS[loss], offset, C.byref(dropout.struct()), out.data_ptr(), rows.data_ptr() if rows is not None else None,
-            ws.data_ptr(), ws.numel(), _stream(dev)))
+        _lib.check(lib.b200kge_score_1vsN_loss_csr_dropout_dir(
+            MODELS[model], SP_ if combine == "sp_" else _PO, SP_ if (dropout_streams or combine) == "sp_" else _PO,
+            l_norm, PREC[precision], C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(),
+            cols.data_ptr() if nnz else None, nnz, label_smoothing, LOSS[loss], offset, C.byref(dropout.struct()),
+            out.data_ptr(), rows.data_ptr() if rows is not None else None, ws.data_ptr(), ws.numel(), _stream(dev)))
         return (out, rows) if return_rows else out
     nbytes = lib.b200kge_score_1vsN_loss_csr_workspace_bytes(MODELS[model], n, m, rq.dim, nnz)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)

@@ -38,21 +38,7 @@ def _assert_close(got, ref, what, tol=TOL):
     assert err <= tol * rms, f"{what}: max|d|={err:.3e} rms={rms:.3e} ratio={err / rms:.2e}"
 
 
-VARIANTS = ["3"]   # B200KGE_TC_VERSION
-
-
-@pytest.fixture(params=VARIANTS, ids=["tc3"])
-def variant(request, monkeypatch):
-    """Selects the kernel for the duration of a test (the default path is restored afterwards)."""
-    ver = request.param
-
-    def select():
-        monkeypatch.setenv("B200KGE_TC_VERSION", ver)
-    return select
-
-
-def test_presplit_fp16_golden(eng, variant):
-    variant()
+def test_presplit_fp16_golden(eng):
     for fname, model in (("scores_complex.npz", "complex"), ("scores_distmult.npz", "distmult"),
                          ("scores_simple.npz", "simple"), ("scores_complex_sigma01.npz", "complex")):
         g = _load(fname)
@@ -66,11 +52,10 @@ def test_presplit_fp16_golden(eng, variant):
 
 
 @pytest.mark.parametrize("sigma", [1.0, 1e-3])
-def test_presplit_fp16_medium(eng, variant, sigma):
+def test_presplit_fp16_medium(eng, sigma):
     """Dense scores, gathered candidate subsets, fused BCE/KL, fused rank counting at ragged sizes (tiles cut in
     both dimensions, K not a multiple of the 64-wide chunk for RESCAL/CP), including tiny-valued tables that a
     fixed fp16 scale would flush."""
-    variant()
     for model, D in (("complex", 192), ("distmult", 64), ("simple", 128), ("rescal", 40), ("cp", 200)):
         E, R, n = 6007, 7, 389
         ent, rel = orc.make_tables(model, E, R, D, sigma=sigma)
@@ -95,14 +80,13 @@ def test_presplit_fp16_medium(eng, variant, sigma):
         assert torch.equal(r.cpu(), rr) and torch.equal(t.cpu(), tt)
 
 
-def test_presplit_fp16_headline_shape(eng, variant):
-    """BASELINE configs[1] shape: loss of the experimental path == loss of the default path to 1e-5."""
+def test_presplit_fp16_headline_shape(eng):
+    """BASELINE configs[1] shape: the loss repeats to 1e-5 and the scores match the oracle."""
     E, R, D, n = 14541, 237, 512, 1024
     ent, rel = orc.make_tables("complex", E, R, D)
     tri = orc.make_triples(E, R, n)
     ce, cr, ct = ent.cuda(), rel.cuda(), tri.cuda()
     base = float(eng.train_1vsall_forward("complex", ce, cr, ct, "bce"))
-    variant()
     got = float(eng.train_1vsall_forward("complex", ce, cr, ct, "bce"))
     assert abs(got - base) <= 1e-5 * abs(base), (got, base)
     ref = orc.score_sp("complex", ent, rel, tri[:64, S], tri[:64, P])
