@@ -366,16 +366,29 @@ int b200kge_score_1vsN_backward(int model, int combine, float l_norm, const b200
                                 int64_t ldg, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
                                 size_t workspace_bytes, b200kge_stream_t stream);
 
-/* Backward of b200kge_score_1vsN_loss_csr / batch_size (loss_value.backward() at kge/job/train_KvsAll.py:294) for the
- * dot family: dense gradients d_ent [E, lde], d_rel [R, ldr] (OVERWRITTEN) of  sum_i loss(score row i, y_i) / batch_size
- * with y = (1 - eps) * count + (eps > 0 ? 1/E : 0) from the CSR labels — recompute, G planes written with the label-free
- * value everywhere and patched at the nnz listed entries, two split-K tensor-core GEMMs, unfold.  Workspace:
- * b200kge_score_1vsN_backward_workspace_bytes. */
+/* Backward of b200kge_score_1vsN_loss_csr / batch_size (loss_value.backward() at kge/job/train_KvsAll.py:294): dense
+ * gradients d_ent [E, lde], d_rel [R, ldr] (OVERWRITTEN) of  sum_i loss(score row i, y_i) / batch_size with
+ * y = (1 - eps) * count + (eps > 0 ? 1/E : 0) from the CSR labels (sorted per row; a repeated column counts as often as
+ * it appears).
+ *   dot family: recompute, G planes written with the label-free value everywhere and patched at the nnz listed
+ *     entries, two split-K tensor-core GEMMs, unfold.
+ *   TransE (l_norm 1, 2) / RotatE (l_norm 1): recompute on the CUDA-core scorer, dense fp32 G (label-free value, then
+ *     each row's listed columns by the row's own thread block; KL: row log-sum-exp first), the two row-gradient passes
+ *     of b200kge_train_1vsall_backward, unfold.  Other norms: B200KGE_ERR_UNSUPPORTED before any launch.
+ * The plain entry is the _norm entry with l_norm = 1.  Workspace: b200kge_score_1vsN_backward_workspace_bytes (the
+ * distance family: Q, dQ [n, round_up(D, 32)] each, triples [3n] and the KL row statistics [2n floats] in its n * 4 * 8
+ * bytes, scores and G [n, round_up(E, 4)] each, G^T [E, round_up(n, 4)], the scorer's workspace). */
 int b200kge_score_1vsN_loss_csr_backward(int model, int combine, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
                                          const int64_t* q_idx, const int64_t* p_idx, int64_t n, const int64_t* csr_off,
                                          const int64_t* csr_col, float label_smoothing, int loss_kind, float offset,
                                          int64_t batch_size, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
                                          void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+int b200kge_score_1vsN_loss_csr_backward_norm(int model, int combine, float l_norm, const b200kge_rows_t* ent,
+                                              const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx,
+                                              int64_t n, const int64_t* csr_off, const int64_t* csr_col,
+                                              float label_smoothing, int loss_kind, float offset, int64_t batch_size,
+                                              float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
+                                              size_t workspace_bytes, b200kge_stream_t stream);
 
 /* KvsAll loss with CSR multi-hot labels (kge/job/train_KvsAll.py:242-300 without the densified label matrix):
  * row i's labels are the columns csr_col[csr_off[i] .. csr_off[i+1]) (sorted; a repeated column counts as often
@@ -383,7 +396,9 @@ int b200kge_score_1vsN_loss_csr_backward(int model, int combine, const b200kge_r
  * *loss_out = sum_i loss(score row i, y_i) (BCE with offset | KL), row_loss_out (optional) the per-row terms.
  * On the pre-split tensor-core path (dot family) ONE fused pass scores, reduces the label-free loss terms and emits
  * the nnz listed scores from its epilogue (per-thread cursor into the row's sorted segment); elsewhere the listed
- * scores come from the row-wise triple kernel.  cand must be a plain table; eps > 0 needs a dot-family model.  Sizes: b200kge_score_1vsN_loss_csr_workspace_bytes. */
+ * scores come from the row-wise triple kernel.  cand must be a plain table.  With eps > 0 the row sums sum_j z_ij come
+ * from Q_i . colsum(T) (dot family) or from the CUDA-core scoring pass itself (TransE, RotatE: one partial per row and
+ * column chunk, no second pass over the table).  Sizes: b200kge_score_1vsN_loss_csr_workspace_bytes. */
 size_t b200kge_score_1vsN_loss_csr_workspace_bytes(int model, int64_t n, int64_t m, int32_t D, int64_t nnz);
 int b200kge_score_1vsN_loss_csr(int model, int combine, float l_norm, int precision,
                                   const b200kge_rows_t* q, const b200kge_rows_t* p,
@@ -496,9 +511,11 @@ int b200kge_train_1vsall_backward_dropout(int model, float l_norm, const b200kge
                                           int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
 
 /* b200kge_score_1vsN_loss_csr / _backward with dropout for one KvsAll query type: queries ent[q_idx] (stream 0 | 5),
- * relations rel[p_idx] (1 | 4) and the candidate table ent (2 | 3) for combine sp_ | _po.  The backward covers the dot
- * family (as b200kge_score_1vsN_loss_csr_backward) and OVERWRITES d_ent / d_rel.
- * Workspace (either call): b200kge_score_1vsN_loss_csr_dropout_workspace_bytes. */
+ * relations rel[p_idx] (1 | 4) and the candidate table ent (2 | 3) for combine sp_ | _po.  The backward covers the models
+ * and norms of b200kge_score_1vsN_loss_csr_backward (the plain dropout backward entries: l_norm 1; the _norm entry
+ * below takes it) and OVERWRITES d_ent / d_rel.
+ * Workspace (either call): b200kge_score_1vsN_loss_csr_dropout_workspace_bytes (the masked copies and per-direction
+ * buffers, then the larger of the forward's and the backward's workspace). */
 size_t b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(int model, int64_t n, int64_t E, int32_t D, int64_t nnz);
 int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, float l_norm, int precision, const b200kge_rows_t* ent,
                                         const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx, int64_t n,
@@ -531,6 +548,16 @@ int b200kge_score_1vsN_loss_csr_backward_dropout_dir(int model, int combine, int
                                                      float offset, int64_t batch_size, const b200kge_dropout_t* drop,
                                                      float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
                                                      void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+/* b200kge_score_1vsN_loss_csr_backward_dropout_dir with the model's l_norm: TransE 1 | 2, RotatE 1 (else
+ * B200KGE_ERR_UNSUPPORTED before any launch); ignored by the dot family.  Same workspace. */
+int b200kge_score_1vsN_loss_csr_backward_dropout_norm(int model, int combine, int mask_dir, float l_norm,
+                                                      const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                                      const int64_t* q_idx, const int64_t* p_idx, int64_t n,
+                                                      const int64_t* csr_off, const int64_t* csr_col,
+                                                      float label_smoothing, int loss_kind, float offset,
+                                                      int64_t batch_size, const b200kge_dropout_t* drop, float* d_ent,
+                                                      int64_t lde, float* d_rel, int64_t ldr, void* workspace,
+                                                      size_t workspace_bytes, b200kge_stream_t stream);
 
 /* ---- The 1vsAll step of a reciprocal-relations model ----------------------------------------------------------------
  * LibKGE's ReciprocalRelationsModel (reciprocal_relations_model.py:85-92) keeps 2R relation rows and answers score_po

@@ -105,6 +105,10 @@ SIGNATURES = {
                                                        C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_float, C.c_int64,
                                                        C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t,
                                                        C.c_void_p]),
+    "b200kge_score_1vsN_loss_csr_backward_norm": (C.c_int, [C.c_int, C.c_int, C.c_float, _RP, _RP, C.c_void_p,
+                                                            C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float,
+                                                            C.c_int, C.c_float, C.c_int64, C.c_void_p, C.c_int64,
+                                                            C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_score_1vsN_loss_csr_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32, C.c_int64]),
     "b200kge_score_1vsN_loss_csr": (C.c_int, [C.c_int, C.c_int, C.c_float, C.c_int, _RP, _RP, _RP, C.c_int64,
                                                 C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_int, C.c_float,
@@ -151,6 +155,11 @@ SIGNATURES = {
                                                                    C.c_float, C.c_int, C.c_float, C.c_int64, _DP,
                                                                    C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
                                                                    C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_score_1vsN_loss_csr_backward_dropout_norm": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_float, _RP, _RP,
+                                                                    C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                                                    C.c_void_p, C.c_float, C.c_int, C.c_float, C.c_int64,
+                                                                    _DP, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                                                    C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_train_1vsall_reciprocal_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32]),
     "b200kge_train_1vsall_reciprocal_forward": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_int64, C.c_void_p,
                                                           C.c_int64, C.c_int, C.c_float, _DP, C.c_void_p, C.c_void_p,

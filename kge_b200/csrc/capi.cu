@@ -158,8 +158,9 @@ int fold_block(const Block& B, int64_t ldq, Arena& ws, cudaStream_t st, const fl
 
 // The scorer's nch chunks per row, and for the BCE/KL epilogues their loss partials [nq, nch, F].
 int take_partials(int epi_kind, int64_t nq, int nch, EpiParams& P, Arena& ws, int* nchunks_out, float** part_out) {
-  if (epi_kind == EPI_BCE || epi_kind == EPI_KL) {
-    const int F = (epi_kind == EPI_BCE) ? 2 : 5;
+  const int loss_epi = epi_loss_base(epi_kind);
+  if (loss_epi == EPI_BCE || loss_epi == EPI_KL) {
+    const int F = (loss_epi == EPI_BCE) ? 2 : 5;
     P.part = (float*)ws.take((size_t)nq * nch * F * 4);
     if (!P.part) { set_error("workspace too small for loss partials"); return B200KGE_ERR_WORKSPACE; }
     if (part_out) *part_out = P.part;
@@ -914,9 +915,9 @@ int distance_rowgrads(int pair_op, const float* Q, int64_t ldq, int64_t nq, cons
   return launch_pair_rowgrad(pair_op, T.base, T.ld, m, Q, ldq, nq, K, W, ldw, dT, ldt, st);
 }
 
-// The distance-family backward of the pre-folded queries B.Qpre (nq rows) against the plain table B.cand, one-hot
-// labels: scores by the CUDA-core scorer, the KL row statistics, dense G, then both row-gradient passes into dQ and
-// dT.  The caller unfolds dQ.
+// The distance-family backward of the pre-folded queries B.Qpre (nq rows) against the plain table B.cand, one-hot or
+// CSR labels: scores by the CUDA-core scorer, the KL row statistics, dense G, then both row-gradient passes into dQ
+// and dT.  The caller unfolds dQ.
 int distance_backward(const Block& B, float l_norm, const GradSpec& g, float* dQ, float* dT, int64_t ldt, Arena& ws,
                       cudaStream_t st) {
   const Folded f = folded_problem(B.model, B.combine, B.cand->dim, l_norm);
@@ -931,9 +932,15 @@ int distance_backward(const Block& B, float l_norm, const GradSpec& g, float* dQ
   P.out = z; P.ldo = ldz;
   int rc;
   if ((rc = run_block(B, l_norm, B200KGE_PREC_AUTO, EPI_STORE, P, ws, st, nullptr))) return rc;
-  if (kl && (rc = launch_row_lse(z, ldz, nq, m, g.lab, row_stat, st))) return rc;
-  if ((rc = launch_grad_dense(z, ldz, nq, m, g.lab, row_stat, kl ? 0.f : g.offset, 1.0f / (float)B.n,
-                              f.pair_op == PAIR_L2, G, ldz, st))) return rc;
+  const int64_t* lab = g.csr_off ? nullptr : g.lab;       // CSR: only the log-sum-exp, grad_csr_kernel has the label mass
+  if (kl && (rc = launch_row_lse(z, ldz, nq, m, lab, row_stat, st))) return rc;
+  if (g.csr_off)
+    rc = launch_grad_csr(z, ldz, nq, m, g.csr_off, g.csr_col, g.csr_a, g.csr_b, row_stat, kl ? 0.f : g.offset,
+                         g.inv_batch, f.pair_op == PAIR_L2, G, ldz, st);
+  else
+    rc = launch_grad_dense(z, ldz, nq, m, g.lab, row_stat, kl ? 0.f : g.offset, 1.0f / (float)B.n,
+                           f.pair_op == PAIR_L2, G, ldz, st);
+  if (rc) return rc;
   return distance_rowgrads(f.pair_op, B.Qpre, round_up(f.K, 32), nq, *B.cand, f.K, G, ldz, Gt, dQ, dT, ldt, st);
 }
 
@@ -1076,7 +1083,9 @@ int b200kge_train_1vsall_backward(int model, float l_norm, const b200kge_rows_t*
 size_t b200kge_score_1vsN_backward_workspace_bytes(int model, int64_t n, int64_t E, int32_t D) {
   const int64_t K = (model == B200KGE_CP) ? D / 2 : D;
   const int64_t ldq = round_up(K, 32);
-  if (model == B200KGE_TRANSE || model == B200KGE_ROTATE)   // Q, dQ, triples, z + W (L2), W^T, scorer workspace
+  // distance family: Q, dQ, triples [3n] + the KL row statistics of the CSR-label backward [2n floats] (n * 4 * 8 bytes),
+  // z + W (L2) or z + G (CSR labels), W^T / G^T, scorer workspace
+  if (model == B200KGE_TRANSE || model == B200KGE_ROTATE)
     return 2 * (size_t)n * ldq * 4 + (size_t)n * 4 * 8 + 2 * (size_t)n * round_up(E, 4) * 4 + (size_t)E * round_up(n, 4) * 4 +
            16 * 256 + b200kge_workspace_bytes(model, n, E, D, 0);
   return 2 * (size_t)n * ldq * 4 + (size_t)n * 4 * 8 + (size_t)E * round_up(n, 4) * 4 + 8192 + backward_block_bytes(n, E, K, ldq);
@@ -1139,15 +1148,18 @@ int b200kge_score_1vsN_backward(int model, int combine, float l_norm, const b200
   return launch_unfold(model, E, R, tri, n, combine, dQ, ldq, d_ent, lde, d_rel, ldr, st);
 }
 
-int b200kge_score_1vsN_loss_csr_backward(int model, int combine, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                         const int64_t* q_idx, const int64_t* p_idx, int64_t n, const int64_t* csr_off,
-                                         const int64_t* csr_col, float label_smoothing, int loss_kind, float offset,
-                                         int64_t batch_size, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                                         void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+int b200kge_score_1vsN_loss_csr_backward_norm(int model, int combine, float l_norm, const b200kge_rows_t* ent,
+                                              const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx,
+                                              int64_t n, const int64_t* csr_off, const int64_t* csr_col,
+                                              float label_smoothing, int loss_kind, float offset, int64_t batch_size,
+                                              float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
+                                              size_t workspace_bytes, b200kge_stream_t stream) {
   if (!q_idx || !p_idx || !csr_off || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
-  int rc = check_tables(model, 1.0f, ent, rel); if (rc) return rc;      // the dot family folds with l_norm 1
-  if (model > B200KGE_RESCAL) { set_error("the tensor-core backward covers the dot family only (model %d)", model); return B200KGE_ERR_UNSUPPORTED; }
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
+  const bool distance = (model == B200KGE_TRANSE || model == B200KGE_ROTATE);
+  Folded f = folded_problem(model, combine, ent->dim, distance ? l_norm : 1.0f);     // the dot family folds with l_norm 1
+  if (distance && (rc = check_distance_pair(f.pair_op))) return rc;
   if ((rc = check_loss_kind(loss_kind))) return rc;
   if (batch_size <= 0 || !(label_smoothing >= 0.f && label_smoothing < 1.f)) { set_error("bad batch_size / label_smoothing"); return B200KGE_ERR_INVALID; }
   if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
@@ -1157,7 +1169,6 @@ int b200kge_score_1vsN_loss_csr_backward(int model, int combine, const b200kge_r
   B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st));
   if (n <= 0) return 0;
   Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
-  Folded f = folded_problem(model, combine, E.dim, 1.0f);
   const int64_t ldq = round_up(f.K, 32);
   float* Q = (float*)ws.take((size_t)n * ldq * 4);
   float* dQ = (float*)ws.take((size_t)n * ldq * 4);
@@ -1169,8 +1180,24 @@ int b200kge_score_1vsN_loss_csr_backward(int model, int combine, const b200kge_r
   Rows Pr = R; Pr.idx = p_idx; Pr.rows = n;
   if ((rc = launch_fold_queries(model, combine, A, Pr, n, 0, Q, ldq, st))) return rc;
   const GradSpec g = csr_grad(q_idx, csr_off, csr_col, label_smoothing, E.rows, batch_size, loss_kind, offset);
+  if (distance) {
+    Block B{model, combine, &A, nullptr, &Pr, &E, n};
+    B.Qpre = Q;
+    if ((rc = distance_backward(B, l_norm, g, dQ, d_ent, lde, ws, st))) return rc;
+    return launch_unfold_distance(model, E, R, tri, n, combine, dQ, ldq, d_ent, lde, d_rel, ldr, st);
+  }
   if ((rc = backward_block(model, E, R, n, combine, false, Q, ldq, f.col_off, f.K, g, d_ent, lde, dQ, ws, st))) return rc;
   return launch_unfold(model, E, R, tri, n, combine, dQ, ldq, d_ent, lde, d_rel, ldr, st);
+}
+
+int b200kge_score_1vsN_loss_csr_backward(int model, int combine, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                         const int64_t* q_idx, const int64_t* p_idx, int64_t n, const int64_t* csr_off,
+                                         const int64_t* csr_col, float label_smoothing, int loss_kind, float offset,
+                                         int64_t batch_size, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
+                                         void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+  return b200kge_score_1vsN_loss_csr_backward_norm(model, combine, 1.0f, ent, rel, q_idx, p_idx, n, csr_off, csr_col,
+                                                   label_smoothing, loss_kind, offset, batch_size, d_ent, lde, d_rel,
+                                                   ldr, workspace, workspace_bytes, stream);
 }
 
 int b200kge_lookup_penalty(const b200kge_rows_t* rows, const float* counts, float p, int complex_abs, float scale,
@@ -1254,6 +1281,8 @@ size_t b200kge_score_1vsN_loss_csr_workspace_bytes(int model, int64_t n, int64_t
   size_t b = b200kge_workspace_bytes(model, n, m, D, 0);
   b += (size_t)n * 8 + 3 * ((size_t)tot * 8 + 256) + (size_t)tot * 4 + 4 * ((size_t)n * 4 + 256) + 2048;
   b += (size_t)n * ldq * 4 + ((size_t)((m + 1023) / 1024) + 1) * ldq * 4 + 512;
+  if (model == B200KGE_TRANSE || model == B200KGE_ROTATE)    // label smoothing: the scorer's partial row score sums
+    b += (size_t)n * pairwise_simt_nchunks(n, m) * 4 + 256;
   return b;
 }
 
@@ -1269,7 +1298,6 @@ int b200kge_score_1vsN_loss_csr(int model, int combine, float l_norm, int precis
   if ((rc = check_loss_kind(loss_kind))) return rc;
   if (!(label_smoothing >= 0.f && label_smoothing < 1.f)) { set_error("label_smoothing must be in [0, 1)"); return B200KGE_ERR_INVALID; }
   const bool dot = model <= B200KGE_RESCAL;
-  if (label_smoothing > 0.f && !dot) { set_error("label smoothing with CSR labels is available for the dot family"); return B200KGE_ERR_UNSUPPORTED; }
   cudaStream_t st = (cudaStream_t)stream;
   if (n == 0 || cand->rows == 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
   Rows Q = to_rows(q), Pr = to_rows(p), C = to_rows(cand);
@@ -1284,7 +1312,11 @@ int b200kge_score_1vsN_loss_csr(int model, int combine, float l_norm, int precis
   float* rows = row_loss_out ? row_loss_out : (float*)ws.take((size_t)n * 4);
   float* total = (float*)ws.take(256);
   void* scratch = ws.take(1024);
-  if (!lab || !qsel || !psel || !esel || !zpos || !fused || !rows || !total || !scratch) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
+  // label smoothing needs sum_j z_ij: the distance family's CUDA-core pass below sums it per row and column chunk
+  const bool zsum_fused = label_smoothing > 0.f && !dot;
+  const int zch = zsum_fused ? pairwise_simt_nchunks(n, m) : 1;
+  float* zsum = zsum_fused ? (float*)ws.take((size_t)n * zch * 4) : nullptr;
+  if (!lab || !qsel || !psel || !esel || !zpos || !fused || !rows || !total || !scratch || (zsum_fused && !zsum)) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
   // 1. label-free fused pass: BCE with no label (index -1) -> sum_j softplus;  KL with the one-hot label at
   //    column 0 -> lse_i - z_i0.  On the pre-split tensor-core path the SAME pass also emits the scores of the listed
   //    columns (and z_i0) from its epilogue (per-thread cursor into the row's sorted CSR segment, tc_common.cuh):
@@ -1292,11 +1324,13 @@ int b200kge_score_1vsN_loss_csr(int model, int combine, float l_norm, int precis
   B2K_CUDA(cudaMemsetAsync(lab, loss_kind == B200KGE_LOSS_BCE ? 0xFF : 0, (size_t)n * 8, st));
   bool emitted = false;
   {
-    const int epi = (loss_kind == B200KGE_LOSS_BCE) ? EPI_BCE : EPI_KL;
+    const int epi = (loss_kind == B200KGE_LOSS_BCE) ? (zsum_fused ? EPI_BCE_ZSUM : EPI_BCE)
+                                                    : (zsum_fused ? EPI_KL_ZSUM : EPI_KL);
     for (int attempt = 0; attempt < 2; ++attempt) {
       EpiParams P = empty_epi();
       P.label_idx = lab;
       P.offset = (loss_kind == B200KGE_LOSS_BCE) ? offset : 0.f;
+      P.zsum_part = zsum;
       if (attempt == 0) {
         P.csr_off = csr_off; P.csr_col = csr_col; P.csr_out = zpos; P.csr_nnz = nnz;
         P.csr_extra = (loss_kind == B200KGE_LOSS_KL) ? 1 : 0;
@@ -1327,8 +1361,7 @@ int b200kge_score_1vsN_loss_csr(int model, int combine, float l_norm, int precis
     }
   }
   // 3. label smoothing: sum_j z_ij = Q_i . colsum(T)   (dot family)
-  float* zsum = nullptr;
-  if (label_smoothing > 0.f) {
+  if (label_smoothing > 0.f && dot) {
     Folded f = folded_problem(model, combine, Q.dim, l_norm);
     const int64_t ldq = round_up(f.K, 32);
     float* Qf = (float*)ws.take((size_t)n * ldq * 4);
@@ -1340,7 +1373,7 @@ int b200kge_score_1vsN_loss_csr(int model, int combine, float l_norm, int precis
   }
   // 4. per-row combination and the scalar
   const float a = 1.0f - label_smoothing, b = label_smoothing > 0.f ? 1.0f / (float)m : 0.f;
-  if ((rc = launch_csr_rows(loss_kind, csr_off, csr_col, zpos, n, nnz, fused, zsum, a, b, (float)m,
+  if ((rc = launch_csr_rows(loss_kind, csr_off, csr_col, zpos, n, nnz, fused, zsum, zch, a, b, (float)m,
                             loss_kind == B200KGE_LOSS_BCE ? offset : 0.f, rows, st))) return rc;
   return launch_rows_sum(rows, n, 1.0f, loss_out, st);
 }
@@ -1686,18 +1719,22 @@ int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, float l_norm, in
                                                  loss_out, row_loss_out, workspace, workspace_bytes, stream);
 }
 
-int b200kge_score_1vsN_loss_csr_backward_dropout_dir(int model, int combine, int mask_dir, const b200kge_rows_t* ent,
-                                                     const b200kge_rows_t* rel, const int64_t* q_idx,
-                                                     const int64_t* p_idx, int64_t n, const int64_t* csr_off,
-                                                     const int64_t* csr_col, float label_smoothing, int loss_kind,
-                                                     float offset, int64_t batch_size, const b200kge_dropout_t* drop,
-                                                     float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                                                     void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+int b200kge_score_1vsN_loss_csr_backward_dropout_norm(int model, int combine, int mask_dir, float l_norm,
+                                                      const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                                      const int64_t* q_idx, const int64_t* p_idx, int64_t n,
+                                                      const int64_t* csr_off, const int64_t* csr_col,
+                                                      float label_smoothing, int loss_kind, float offset,
+                                                      int64_t batch_size, const b200kge_dropout_t* drop, float* d_ent,
+                                                      int64_t lde, float* d_rel, int64_t ldr, void* workspace,
+                                                      size_t workspace_bytes, b200kge_stream_t stream) {
   if (!q_idx || !p_idx || !csr_off || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
   if (mask_dir != B200KGE_SP_ && mask_dir != B200KGE__PO) { set_error("bad mask direction %d", mask_dir); return B200KGE_ERR_INVALID; }
-  int rc = check_tables(model, 1.0f, ent, rel); if (rc) return rc;      // the dot family folds with l_norm 1
-  if (model > B200KGE_RESCAL) { set_error("the tensor-core backward covers the dot family only (model %d)", model); return B200KGE_ERR_UNSUPPORTED; }
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
+  const bool distance = (model == B200KGE_TRANSE || model == B200KGE_ROTATE);
+  if (!distance) l_norm = 1.0f;                                           // the dot family folds with l_norm 1
+  const Folded f = folded_problem(model, combine, ent->dim, l_norm);
+  if (distance && (rc = check_distance_pair(f.pair_op))) return rc;
   if ((rc = check_loss_kind(loss_kind))) return rc;
   if (batch_size <= 0 || !(label_smoothing >= 0.f && label_smoothing < 1.f)) { set_error("bad batch_size / label_smoothing"); return B200KGE_ERR_INVALID; }
   if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
@@ -1708,7 +1745,6 @@ int b200kge_score_1vsN_loss_csr_backward_dropout_dir(int model, int combine, int
   B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st));
   if (n <= 0) return 0;
   Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
-  const Folded f = folded_problem(model, combine, E.dim, 1.0f);
   BackBufs b;
   if (!take_back(ws, n, E.rows, E.dim, R.dim, round_up(f.K, 32), b)) {
     set_error("workspace too small (see b200kge_score_1vsN_loss_csr_dropout_workspace_bytes)");
@@ -1716,8 +1752,21 @@ int b200kge_score_1vsN_loss_csr_backward_dropout_dir(int model, int combine, int
   }
   if ((rc = launch_identity_triples(n, b.tri, st))) return rc;
   const GradSpec g = csr_grad(q_idx, csr_off, csr_col, label_smoothing, E.rows, batch_size, loss_kind, offset);
-  return dropout_backward_dir(model, 1.0f, combine, mask_dir, E, R, q_idx, p_idx, n, *drop, g, b, rest_of(ws), d_ent, lde,
-                              d_rel, ldr, st);
+  return dropout_backward_dir(model, l_norm, combine, mask_dir, E, R, q_idx, p_idx, n, *drop, g, b, rest_of(ws), d_ent,
+                              lde, d_rel, ldr, st);
+}
+
+int b200kge_score_1vsN_loss_csr_backward_dropout_dir(int model, int combine, int mask_dir, const b200kge_rows_t* ent,
+                                                     const b200kge_rows_t* rel, const int64_t* q_idx,
+                                                     const int64_t* p_idx, int64_t n, const int64_t* csr_off,
+                                                     const int64_t* csr_col, float label_smoothing, int loss_kind,
+                                                     float offset, int64_t batch_size, const b200kge_dropout_t* drop,
+                                                     float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
+                                                     void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+  return b200kge_score_1vsN_loss_csr_backward_dropout_norm(model, combine, mask_dir, 1.0f, ent, rel, q_idx, p_idx, n,
+                                                           csr_off, csr_col, label_smoothing, loss_kind, offset,
+                                                           batch_size, drop, d_ent, lde, d_rel, ldr, workspace,
+                                                           workspace_bytes, stream);
 }
 
 int b200kge_score_1vsN_loss_csr_backward_dropout(int model, int combine, const b200kge_rows_t* ent,

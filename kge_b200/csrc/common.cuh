@@ -74,7 +74,13 @@ __host__ __device__ inline int relation_dim(int model, int D) {
 // ---------------------------------------------------------------------------------------------
 // Epilogues.  A kernel computes x = score(row, col) for a tile and hands every valid element to
 // one of these functors; per-row state lives in registers and is flushed once per (row, chunk).
-enum EpiKind : int { EPI_STORE = 0, EPI_BCE = 1, EPI_KL = 2, EPI_RANK = 3, EPI_RANK_EVAL = 4 };
+enum EpiKind : int { EPI_STORE = 0, EPI_BCE = 1, EPI_KL = 2, EPI_RANK = 3, EPI_RANK_EVAL = 4, EPI_BCE_ZSUM = 5, EPI_KL_ZSUM = 6 };
+
+// EPI_BCE_ZSUM / EPI_KL_ZSUM (CUDA-core kernel only): the BCE / KL epilogue plus the row's plain score sum sum_j z_ij,
+// which label smoothing of the CSR-label losses needs (the distance family has no Q . colsum(T) identity for it)
+__host__ __device__ constexpr int epi_loss_base(int kind) {
+  return kind == EPI_BCE_ZSUM ? EPI_BCE : (kind == EPI_KL_ZSUM ? EPI_KL : kind);
+}
 
 struct FinalizeArgs;
 struct EpiParams {
@@ -129,6 +135,8 @@ struct EpiParams {
   int64_t rank_ld;
   int n_rank;
   float* own_score;
+  // EPI_BCE_ZSUM / EPI_KL_ZSUM: zsum_part[row * nchunks + chunk] = the chunk's sum of the row's scores
+  float* zsum_part;
 };
 
 // lower bound of `key` in the sorted segment col[lo, hi)
@@ -181,6 +189,15 @@ template <> struct RowState<EPI_KL> {
     y_sum += o.y_sum; yx += o.yx; ylogy += o.ylogy;
   }
 };
+
+// the loss state of BASE plus the plain score sum
+template <int BASE> struct RowStateZsum : RowState<BASE> {
+  float zs;
+  __device__ __forceinline__ void init() { RowState<BASE>::init(); zs = 0.f; }
+  __device__ __forceinline__ void combine(const RowStateZsum& o) { RowState<BASE>::combine(o); zs += o.zs; }
+};
+template <> struct RowState<EPI_BCE_ZSUM> : RowStateZsum<EPI_BCE> {};
+template <> struct RowState<EPI_KL_ZSUM> : RowStateZsum<EPI_KL> {};
 
 // rank / ties counters     eval_entity_ranking.py:571-596
 template <> struct RowState<EPI_RANK> {
@@ -280,6 +297,9 @@ __device__ __forceinline__ void epi_elem(const EpiParams& P, RowState<KIND>& st,
     const bool c = isclose_f(v, row_aux, P.rtol, P.atol);
     st.close += c ? 1u : 0u;
     st.greater += (!c && v > row_aux) ? 1u : 0u;
+  } else if constexpr (KIND == EPI_BCE_ZSUM || KIND == EPI_KL_ZSUM) {
+    epi_elem<epi_loss_base(KIND)>(P, st, row, col, x, row_aux);
+    st.zs += x;
   }
 }
 
@@ -287,7 +307,7 @@ __device__ __forceinline__ void epi_elem(const EpiParams& P, RowState<KIND>& st,
 // < 2^31 candidates per call) or the NaN-cleaned true score.
 template <int KIND>
 __device__ __forceinline__ float epi_row_aux(const EpiParams& P, int64_t row) {
-  if constexpr (KIND == EPI_BCE || KIND == EPI_KL) {
+  if constexpr (epi_loss_base(KIND) == EPI_BCE || epi_loss_base(KIND) == EPI_KL) {
     return P.label_idx ? __int_as_float((int)P.label_idx[row]) : __int_as_float(-1);
   } else if constexpr (KIND == EPI_RANK || KIND == EPI_RANK_EVAL) {
     float t = P.true_score[row];
@@ -318,6 +338,9 @@ __device__ __forceinline__ void epi_flush(const EpiParams& P, const RowState<KIN
       if (st.greater) atomicAdd(P.rank + k * P.rank_ld + row, (unsigned long long)st.greater);
       if (st.close) atomicAdd(P.ties + k * P.rank_ld + row, (unsigned long long)st.close);
     }
+  } else if constexpr (KIND == EPI_BCE_ZSUM || KIND == EPI_KL_ZSUM) {
+    epi_flush<epi_loss_base(KIND)>(P, st, row, chunk);
+    P.zsum_part[row * P.nchunks + chunk] = st.zs;
   }
 }
 

@@ -12,7 +12,8 @@
 // sum_j softplus: fused BCE kernel with no label (index -1).  lse_i: fused KL kernel with the one-hot label at
 // column 0 returns lse_i - z_i0, and z_i0 rides along with the listed columns.  The listed scores come from the
 // row-wise triple kernel (gather + dot per CSR entry: nnz * D work).  sum_j z_ij (label smoothing only) is
-// Q_i . colsum(T) for the dot family.
+// Q_i . colsum(T) for the dot family; the distance family's CUDA-core scorer sums it in the same pass that reduces the
+// label-free terms (EPI_BCE_ZSUM / EPI_KL_ZSUM, one partial per row and column chunk).
 #include "common.cuh"
 
 namespace b200kge {
@@ -39,11 +40,12 @@ __device__ __forceinline__ float wsum(float v) {
 }
 
 // one warp per row: combine the fused kernel's per-row term with the sparse label terms.
-//   fused[i]: BCE -> sum_j softplus(z + off);  KL -> lse_i - z_i0.   zsum may be null (no smoothing).
+//   fused[i]: BCE -> sum_j softplus(z + off);  KL -> lse_i - z_i0.   zsum may be null (no smoothing); else row i's
+//   sum_j z_ij in zch partial sums zsum[i * zch ..] (the CUDA-core scorer's chunks; 1 for the dot family's Q . colsum).
 template <int LOSS>
 __global__ void __launch_bounds__(256)
 csr_rows_kernel(const int64_t* __restrict__ off, const int64_t* __restrict__ col, const float* __restrict__ zpos,
-                int64_t n, int64_t nnz, const float* __restrict__ fused, const float* __restrict__ zsum, float a,
+                int64_t n, int64_t nnz, const float* __restrict__ fused, const float* __restrict__ zsum, int zch, float a,
                 float b, float E, float offset, float* __restrict__ row_loss) {
   const int lane = threadIdx.x & 31;
   const int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -62,7 +64,11 @@ csr_rows_kernel(const int64_t* __restrict__ off, const int64_t* __restrict__ col
   }
   B = wsum(B);
   const float cnt = (float)(t1 - t0);
-  const float zs = zsum ? zsum[i] : 0.f;
+  float zs = 0.f;
+  if (zsum) {
+    for (int c = lane; c < zch; c += 32) zs += zsum[i * zch + c];
+    zs = wsum(zs);
+  }
   float L;
   if (LOSS == B200KGE_LOSS_BCE) {
     L = fused[i] - a * (B + cnt * offset) - b * (zs + E * offset);
@@ -150,14 +156,16 @@ int launch_csr_expand(const int64_t* off, const int64_t* col, int64_t n, int64_t
 }
 
 int launch_csr_rows(int loss_kind, const int64_t* off, const int64_t* col, const float* zpos, int64_t n, int64_t nnz,
-                    const float* fused, const float* zsum, float a, float b, float E, float offset, float* row_loss,
-                    cudaStream_t st) {
+                    const float* fused, const float* zsum, int zsum_chunks, float a, float b, float E, float offset,
+                    float* row_loss, cudaStream_t st) {
   if (n == 0) return 0;
   const unsigned blocks = (unsigned)((n + 7) / 8);
   if (loss_kind == B200KGE_LOSS_BCE)
-    csr_rows_kernel<B200KGE_LOSS_BCE><<<blocks, 256, 0, st>>>(off, col, zpos, n, nnz, fused, zsum, a, b, E, offset, row_loss);
+    csr_rows_kernel<B200KGE_LOSS_BCE><<<blocks, 256, 0, st>>>(off, col, zpos, n, nnz, fused, zsum, zsum_chunks, a, b, E,
+                                                              offset, row_loss);
   else
-    csr_rows_kernel<B200KGE_LOSS_KL><<<blocks, 256, 0, st>>>(off, col, zpos, n, nnz, fused, zsum, a, b, E, offset, row_loss);
+    csr_rows_kernel<B200KGE_LOSS_KL><<<blocks, 256, 0, st>>>(off, col, zpos, n, nnz, fused, zsum, zsum_chunks, a, b, E,
+                                                             offset, row_loss);
   B2K_LAUNCH_CHECK("csr_rows_kernel");
   return 0;
 }

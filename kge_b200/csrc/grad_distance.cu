@@ -8,7 +8,8 @@
 //   L1      s = -sum_k |d_k|             s'_k = -sign(d_k)
 //   L2      s = -||d||                   s'_k = -d_k / ||d|| = d_k / s        (G is pre-divided by the stored score s)
 //   CMOD L1 s = -sum_k |d_k| (complex)   s'_(re,im),k = -(d_re, d_im)_k / |d_k|   (0 if |d_k| = 0)
-// G = n dL/dz comes from grad_dense_kernel (BCE: sigmoid(z + off) - y; KL: w softmax(z) - y / sum y), fp32, dense.
+// G = n dL/dz comes from grad_dense_kernel (BCE: sigmoid(z + off) - y; KL: w softmax(z) - y / sum y), fp32, dense, or
+// from grad_csr_kernel for the CSR labels of KvsAll (dL/dz / batch_size).
 //
 // Tiling: a CTA owns 64 rows of A x one 64-float chunk of the reduction axis (grid.y; every element of the axis is
 // independent) and walks ALL columns in shared-memory tiles of 64, so dA is written once, without atomics.  A thread
@@ -137,6 +138,38 @@ grad_dense_kernel(const float* __restrict__ z, int64_t ldz, int64_t E, const int
   G[i * ldg + e] = g;
 }
 
+// G for the CSR labels of a KvsAll query type (train_KvsAll.py:242-266), the fp32 counterpart of grad.cu's CSR planes:
+// y_ie = a c_ie + b with c_ie the multiplicity of column e in row i's sorted segment col[off[i], off[i+1]).
+//   BCE  sigmoid(z + off) - y          KL  w softmax(z) - y / yc,  Y = a nnz_i + b E, yc = max(Y, 1e-12), w = Y / yc
+// (row_stat[2i] = lse_i), times inv_n; div_z as in grad_dense_kernel.  One block per row: the label-free value (y = b)
+// everywhere, then, after the block barrier, the row's listed columns overwritten by the same block — no atomics and
+// no [n, E] label matrix.  A row with no labels and no smoothing gets sigmoid(z + off) (BCE) or 0 (KL), as on the
+// tensor-core path.  grid = nq
+__global__ void __launch_bounds__(256)
+grad_csr_kernel(const float* __restrict__ z, int64_t ldz, int64_t E, const int64_t* __restrict__ off,
+                const int64_t* __restrict__ col, float a, float b, const float* __restrict__ row_stat, float offset,
+                float inv_n, int div_z, float* __restrict__ G, int64_t ldg) {
+  const int64_t i = blockIdx.x, t0 = off[i], t1 = off[i + 1];
+  const float* __restrict__ zr = z + i * ldz;
+  float* __restrict__ gr = G + i * ldg;
+  const float ys = a * (float)(t1 - t0) + b * (float)E, yc = fmaxf(ys, 1e-12f);
+  auto grad = [&](float zv, float y) {
+    const float x = zv + offset;
+    float g = row_stat ? (ys / yc) * expf(x - row_stat[2 * i]) - y / yc : 1.0f / (1.0f + expf(-x)) - y;
+    g *= inv_n;
+    return div_z ? ((zv != 0.f) ? g / zv : 0.f) : g;
+  };
+  for (int64_t e = threadIdx.x; e < E; e += blockDim.x) gr[e] = grad(zr[e], b);
+  __syncthreads();
+  for (int64_t t = t0 + threadIdx.x; t < t1; t += blockDim.x) {
+    if (t > t0 && col[t] == col[t - 1]) continue;             // a run of equal columns is handled by its first entry
+    int64_t c = 1;
+    while (t + c < t1 && col[t + c] == col[t]) ++c;
+    const int64_t e = col[t];
+    gr[e] = grad(zr[e], a * (float)c + b);
+  }
+}
+
 // W[i, e] = g[i, e] / z[i, e] (0 where z = 0): the L2 pair op's chain factor for a given dL/dscores.  grid = (ceil(E/256), n)
 __global__ void __launch_bounds__(256)
 div_scores_kernel(const float* __restrict__ g, int64_t ldg, const float* __restrict__ z, int64_t ldz, int64_t E,
@@ -188,6 +221,15 @@ int launch_grad_dense(const float* z, int64_t ldz, int64_t nq, int64_t E, const 
   dim3 grid((unsigned)((E + 255) / 256), (unsigned)nq);
   grad_dense_kernel<<<grid, 256, 0, st>>>(z, ldz, E, label_idx, row_stat, offset, inv_n, div_z, G, ldg);
   B2K_LAUNCH_CHECK("grad_dense_kernel");
+  return 0;
+}
+
+int launch_grad_csr(const float* z, int64_t ldz, int64_t nq, int64_t E, const int64_t* csr_off, const int64_t* csr_col,
+                    float a, float b, const float* row_stat, float offset, float inv_n, int div_z, float* G, int64_t ldg,
+                    cudaStream_t st) {
+  if (nq == 0 || E == 0) return 0;
+  grad_csr_kernel<<<(unsigned)nq, 256, 0, st>>>(z, ldz, E, csr_off, csr_col, a, b, row_stat, offset, inv_n, div_z, G, ldg);
+  B2K_LAUNCH_CHECK("grad_csr_kernel");
   return 0;
 }
 

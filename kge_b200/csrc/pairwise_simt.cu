@@ -2,7 +2,8 @@
 //
 // score(i, j) = pair(Q_i, cand_j[col_off : col_off+K]) for a [128 x 128] tile per CTA, 8x8 register
 // micro-tile per thread, K streamed through shared memory in 16-float chunks (register-prefetch
-// double buffering), fused with the STORE / BCE / KL / RANK epilogues of common.cuh.
+// double buffering), fused with the STORE / BCE / KL / RANK epilogues of common.cuh (distance family: also BCE / KL
+// with the row's score sum, for label smoothing of the CSR-label losses).
 //
 // This is THE kernel for the distance family — TransE (transe.py:20-35, cdist without matmul) and
 // RotatE (rotate.py:42-65, which materialises [n,E,D/2] intermediates in the reference) — whose
@@ -326,6 +327,12 @@ int launch_p(int epi, bool vec, dim3 grid, cudaStream_t st, const float* Q, int6
     case EPI_KL:    return launch_pe<PAIR, EPI_KL>(vec, grid, st, Q, ldq, nq, cand, col_off, K, p, P);
     case EPI_RANK:  return launch_pe<PAIR, EPI_RANK>(vec, grid, st, Q, ldq, nq, cand, col_off, K, p, P);
     case EPI_RANK_EVAL: return launch_pe<PAIR, EPI_RANK_EVAL>(vec, grid, st, Q, ldq, nq, cand, col_off, K, p, P);
+  }
+  if constexpr (PAIR != PAIR_DOT) {      // the dot family sums its scores as Q . colsum(T) instead
+    switch (epi) {
+      case EPI_BCE_ZSUM: return launch_pe<PAIR, EPI_BCE_ZSUM>(vec, grid, st, Q, ldq, nq, cand, col_off, K, p, P);
+      case EPI_KL_ZSUM:  return launch_pe<PAIR, EPI_KL_ZSUM>(vec, grid, st, Q, ldq, nq, cand, col_off, K, p, P);
+    }
   }
   set_error("bad epilogue kind %d", epi);
   return B200KGE_ERR_INVALID;

@@ -418,6 +418,10 @@ int launch_pair_rowgrad(int pair_op, const float* A, int64_t lda, int64_t ra, co
                         const float* Wt, int64_t ldwt, float* dA, int64_t ldda, cudaStream_t st);   // Wt: [rb, >= ra]
 int launch_grad_dense(const float* z, int64_t ldz, int64_t nq, int64_t E, const int64_t* label_idx, const float* row_stat,
                       float offset, float inv_n, int div_z, float* G, int64_t ldg, cudaStream_t st);
+// G for CSR labels y = a * count + b (KvsAll); row_stat: KL row log-sum-exp in row_stat[2 i] (else null)
+int launch_grad_csr(const float* z, int64_t ldz, int64_t nq, int64_t E, const int64_t* csr_off, const int64_t* csr_col,
+                    float a, float b, const float* row_stat, float offset, float inv_n, int div_z, float* G, int64_t ldg,
+                    cudaStream_t st);
 int launch_div_scores(const float* g, int64_t ldg, const float* z, int64_t ldz, int64_t n, int64_t E, float* W, int64_t ldw,
                       cudaStream_t st);
 int launch_row_lse(const float* z, int64_t ldz, int64_t nq, int64_t E, const int64_t* label_idx, float* row_stat,
@@ -433,9 +437,10 @@ int launch_grad_planes_csr(const float* z, int64_t ldz, int64_t nq, int64_t E, c
 // CSR-label losses (csr_loss.cu).
 int launch_csr_expand(const int64_t* off, const int64_t* col, int64_t n, int64_t nnz, int extra, const int64_t* q_idx,
                       const int64_t* p_idx, int64_t* qsel, int64_t* psel, int64_t* esel, cudaStream_t st);
+// zsum (label smoothing, else null): zsum_chunks partial score sums per row, [n, zsum_chunks]
 int launch_csr_rows(int loss_kind, const int64_t* off, const int64_t* col, const float* zpos, int64_t n, int64_t nnz,
-                    const float* fused, const float* zsum, float a, float b, float E, float offset, float* row_loss,
-                    cudaStream_t st);
+                    const float* fused, const float* zsum, int zsum_chunks, float a, float b, float E, float offset,
+                    float* row_loss, cudaStream_t st);
 int launch_rows_sum(const float* rows, int64_t n, float scale, float* out, cudaStream_t st);
 int launch_row_score_sums(const float* Q, int64_t ldq, int64_t n, const float* T, int64_t ldt, int64_t E, int K,
                           float* scratch, float* zsum, cudaStream_t st);

@@ -689,9 +689,11 @@ def score_1vsN_backward(model: str, combine: str, ent, rel, q, p, grad_scores, l
 
 def score_1vsN_loss_csr_backward(model: str, combine: str, ent, rel, q, p, csr_offsets, csr_cols, loss: str = "kl",
                                  offset: float = 0.0, label_smoothing: float = 0.0, batch_size: Optional[int] = None,
-                                 dropout: Optional["DropoutKey"] = None, dropout_streams: Optional[str] = None):
-    """(d_ent, d_rel) of score_1vsN_loss_csr(...) / batch_size over the whole entity table (dot family), with the
-    forward's dropout masks when `dropout` is the forward's key (and `dropout_streams` the forward's)."""
+                                 dropout: Optional["DropoutKey"] = None, dropout_streams: Optional[str] = None,
+                                 l_norm: float = 1.0):
+    """(d_ent, d_rel) of score_1vsN_loss_csr(...) / batch_size over the whole entity table (dot family; TransE with
+    l_norm 1 or 2; RotatE with l_norm 1 — other norms raise NotImplementedError), with the forward's dropout masks when
+    `dropout` is the forward's key (and `dropout_streams` the forward's)."""
     _require_cuda(ent, rel, csr_offsets, csr_cols)
     lib, k = _lib.load(), _Keep()
     re_, rr = k.rows(ent), k.rows(rel)
@@ -703,18 +705,18 @@ def score_1vsN_loss_csr_backward(model: str, combine: str, ent, rel, q, p, csr_o
     if dropout is not None:
         ws = torch.empty(lib.b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(
             MODELS[model], n, ent.shape[0], ent.shape[1], int(cols.numel())), dtype=torch.uint8, device=dev)
-        _lib.check(lib.b200kge_score_1vsN_loss_csr_backward_dropout_dir(
+        _lib.check(lib.b200kge_score_1vsN_loss_csr_backward_dropout_norm(
             MODELS[model], SP_ if combine == "sp_" else _PO, SP_ if (dropout_streams or combine) == "sp_" else _PO,
-            C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(),
+            l_norm, C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(),
             cols.data_ptr() if cols.numel() else None, label_smoothing, LOSS[loss], offset, batch_size or n,
             C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0),
             ws.data_ptr(), ws.numel(), _stream(dev)))
         return d_ent, d_rel
     ws = torch.empty(lib.b200kge_score_1vsN_backward_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1]),
                      dtype=torch.uint8, device=dev)
-    _lib.check(lib.b200kge_score_1vsN_loss_csr_backward(
-        MODELS[model], SP_ if combine == "sp_" else _PO, C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n,
-        offs.data_ptr(), cols.data_ptr() if cols.numel() else None, label_smoothing, LOSS[loss], offset,
+    _lib.check(lib.b200kge_score_1vsN_loss_csr_backward_norm(
+        MODELS[model], SP_ if combine == "sp_" else _PO, l_norm, C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(),
+        n, offs.data_ptr(), cols.data_ptr() if cols.numel() else None, label_smoothing, LOSS[loss], offset,
         batch_size or n, d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0), ws.data_ptr(), ws.numel(),
         _stream(dev)))
     return d_ent, d_rel

@@ -249,6 +249,8 @@ class _KvsAllLossFn(torch.autograd.Function):
         kw = {} if dropout is None else {"dropout": dropout}
         if dropout_streams is not None:
             kw["dropout_streams"] = dropout_streams
+        if model._b200_name in ("transe", "rotate"):
+            kw["l_norm"] = model._b200_args()[0]
         d_ent, d_rel = engine.score_1vsN_loss_csr_backward(model._b200_name, combine, ent_w.detach(), rel_w.detach(), a, p,
                                                            offs, cols, loss, offset, smoothing, batch_size, **kw)
         return (d_ent * g, d_rel * g) + (None,) * 12
@@ -346,7 +348,10 @@ class _B200ModelMixin:
         return rates if max(rates) > 0 else None
 
     def b200_csr_labels_ok(self, label_smoothing):
-        return label_smoothing == 0.0 or self._b200_name in ("complex", "distmult", "simple", "cp", "rescal")
+        """The CSR-label loss takes label smoothing for the dot family (Q . colsum(T)) and for TransE / RotatE (the row
+        score sums of the CUDA-core scoring pass), every norm."""
+        return label_smoothing == 0.0 or self._b200_name in ("complex", "distmult", "simple", "cp", "rescal", "transe",
+                                                             "rotate")
 
     def _b200_weights(self):
         return self.get_s_embedder()._embeddings.weight, self.get_p_embedder()._embeddings.weight
@@ -519,8 +524,16 @@ class _B200ModelMixin:
         return engine.score_1vsN_loss_csr(self._b200_name, combine, ent, rel, ent, csr_offsets, csr_cols, a, p,
                                           loss, offset, label_smoothing, ln, prec, **kw)
 
-    def b200_kvsall_native_backward_ok(self):
-        return self.b200_backward == "native" and self._b200_name in ("complex", "distmult", "simple", "cp", "rescal")
+    def b200_kvsall_native_backward_ok(self, dropout=False):
+        """The KvsAll gradient kernels cover the dot family, TransE with l_norm 1 or 2 and RotatE with l_norm 1.  The
+        distance family's CSR-label backward recomputes the scores on the CUDA cores, where the unmodified step without
+        dropout keeps its stored dense scores and runs the same row-gradient passes on dL/dscores: that step is faster
+        (TransE L1 13.0 vs 14.9 ms, RotatE L1 20.8 vs 23.6 ms, scripts/kvsall_distance_train_bench.py).  So TransE and
+        RotatE take the CSR-label backward under embedding dropout (`dropout`), where the unmodified step recomputes
+        through the reference expression instead."""
+        if self.b200_backward != "native" or not self._b200_native_family():
+            return False
+        return dropout or self._b200_name not in ("transe", "rotate")
 
     def loss_kvsall_train(self, combine, a, p, csr_offsets, csr_cols, loss, offset, label_smoothing, batch_size,
                           dropout=None, dropout_streams=None):

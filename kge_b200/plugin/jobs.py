@@ -273,7 +273,7 @@ class B200TrainingJobKvsAll(_DropoutKeys, _BatchSplit, TrainingJobKvsAll):
             model, rates = _dropout_model(target)
         qtypes = [q for q in self.query_types]
         if (model is None or kind is None or "s_o" in qtypes or not model.b200_csr_labels_ok(self.label_smoothing)
-                or (not self.is_forward_only and not model.b200_kvsall_native_backward_ok())):
+                or (not self.is_forward_only and not model.b200_kvsall_native_backward_ok(rates is not None))):
             return super()._process_subbatch(batch_index, batch, subbatch_slice, result)
         batch_size = result.size
         # one key per sub-batch: the sp_ and _po query types draw disjoint mask streams under it
