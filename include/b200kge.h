@@ -276,9 +276,24 @@ int b200kge_ns_score(int model, float l_norm, const b200kge_rows_t* s, const b20
 /* On-device uniform negative sampling: out[i*K + k] ~ U{0, ..., vocab-1}, the device counterpart of
  * KgeUniformSampler._sample (kge/util/sampler.py:588-596: torch.randint on the CPU + a host->device copy of the ids).
  * Counter-based Philox4x32-10: the result depends on (seed, offset, position) only; use a fresh `offset` per call
- * (e.g. a batch counter) for independent draws.  No filtering of positives (sampler.py default filtering off). */
+ * (e.g. a batch counter) for independent draws.  Positives are not filtered here: b200kge_sample_uniform_filtered
+ * does that. */
 int b200kge_sample_uniform(uint64_t seed, uint64_t offset, int64_t vocab, int64_t n, int64_t K, int64_t* out,
                            b200kge_stream_t stream);
+
+/* Filtered uniform negative sampling (negative_sampling.filtering.<slot>, kge/util/sampler.py:108-128,163-196,700-752):
+ * out[i*K + k] ~ U({0..vocab-1} \ P_i), i.i.d., where P_i are the values of row i's key in a filter index.  The key of
+ * row i of triples [n,3] (device, int64) is (p, o) for slot 0 (S), (s, o) for slot 1 (P), (s, p) for slot 2 (O).
+ * The index (device, int64) is a CSR over keys [num_keys,2] in ascending lexicographic order: the values of key j are
+ * values[offsets[j] .. offsets[j+1]), ascending, distinct, in [0, vocab) — what b200kge_filter_index_build returns.
+ * Counter domains: element e = i*K + k first draws x exactly as b200kge_sample_uniform does (block (e/2, offset) under
+ * key seed), so every position whose x is not a positive equals b200kge_sample_uniform's output bit for bit.  A
+ * positive x is replaced by the u-th non-positive id, u = floor(r * (vocab - m) / 2^64) with m = |P_i| and r the same
+ * word pair of block (e/2 | 2^63, offset) under key seed, a counter the first draw never uses.  The result depends on
+ * (seed, offset, i, k) and the index only.  Rows whose key is absent are unfiltered; rows with m >= vocab receive -1. */
+int b200kge_sample_uniform_filtered(uint64_t seed, uint64_t offset, int64_t vocab, int64_t n, int64_t K,
+                                    const int64_t* triples, int slot, const int64_t* keys, const int64_t* offsets,
+                                    const int64_t* values, int64_t num_keys, int64_t* out, b200kge_stream_t stream);
 
 /* One whole 1vsAll forward step (train_1vsAll.py:48-82) for a batch of triples [n,3] (int64,
  * row-major s,p,o): fused score_sp+loss and score_po+loss against the whole entity table, both
@@ -331,6 +346,16 @@ int b200kge_kvsall_lookup(const int64_t* keys, const int64_t* offsets, const int
 int b200kge_kvsall_gather(const int64_t* keys, const int64_t* offsets, const int64_t* values,
                           int64_t num_keys, const int64_t* examples, int64_t nb,
                           int64_t* queries_out, int64_t* offsets_out, int64_t* cols_out);
+
+/* The filter index of b200kge_sample_uniform_filtered from a key -> values index (host arrays: the _keys, _values_offset
+ * and _values of a KvsAllIndex, widened to int64; keys may come in any order and repeat, values may repeat).
+ * keys_out [num_keys,2], offsets_out [num_keys+1] and values_out [offsets[num_keys] - offsets[0]] are caller-allocated
+ * at those capacities.  Keys come out sorted and unique, values sorted and unique per key; keys without values are
+ * dropped.  *num_keys_out receives the number of keys, *max_count the largest number of values of one key.
+ * B200KGE_ERR_INVALID if the offsets decrease or a value lies outside [0, vocab). */
+int b200kge_filter_index_build(const int64_t* keys, const int64_t* offsets, const int64_t* values, int64_t num_keys,
+                               int64_t vocab, int64_t* keys_out, int64_t* offsets_out, int64_t* values_out,
+                               int64_t* num_keys_out, int64_t* max_count);
 
 /* ---- SURVEY 8(f) rows: gradients, penalties, CSR labels -------------
  *

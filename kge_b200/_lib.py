@@ -77,6 +77,11 @@ SIGNATURES = {
     "b200kge_ns_score": (C.c_int, [C.c_int, C.c_float, _RP, _RP, _RP, _RP, C.c_int, C.c_void_p, C.c_int64,
                                    C.c_int64, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]),
     "b200kge_sample_uniform": (C.c_int, [C.c_uint64, C.c_uint64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
+    "b200kge_sample_uniform_filtered": (C.c_int, [C.c_uint64, C.c_uint64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
+                                                  C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                                  C.c_void_p]),
+    "b200kge_filter_index_build": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "b200kge_train_1vsall_forward": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_void_p,
                                                C.c_int64, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
                                                C.c_size_t, C.c_void_p]),

@@ -438,6 +438,10 @@ int launch_ns(int model, float l_norm, const Rows& s, const Rows& p, const Rows&
               const Rows& table, int slot, const int64_t* neg, int64_t n, int64_t K, float* out,
               int64_t ldo, int col0, cudaStream_t st);
 int launch_sample_uniform(uint64_t seed, uint64_t offset, int64_t vocab, int64_t total, int64_t* out, cudaStream_t st);
+// launch_sample_uniform's draws with the positives of each row's key replaced (b200kge_sample_uniform_filtered)
+int launch_sample_uniform_filtered(uint64_t seed, uint64_t offset, int64_t vocab, int64_t n, int64_t K,
+                                   const int64_t* triples, int slot, const int64_t* keys, const int64_t* offsets,
+                                   const int64_t* values, int64_t num_keys, int64_t* out, cudaStream_t st);
 int launch_loss_dense(int loss_kind, const float* scores, int64_t lds, int64_t n, int64_t m,
                       const EpiParams& P, cudaStream_t st);
 int loss_dense_nchunks(int64_t m);

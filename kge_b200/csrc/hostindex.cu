@@ -121,4 +121,57 @@ int b200kge_kvsall_gather(const int64_t* keys, const int64_t* offsets, const int
   return 0;
 }
 
+int b200kge_filter_index_build(const int64_t* keys, const int64_t* offsets, const int64_t* values, int64_t num_keys,
+                               int64_t vocab, int64_t* keys_out, int64_t* offsets_out, int64_t* values_out,
+                               int64_t* num_keys_out, int64_t* max_count) {
+  if (num_keys < 0 || !offsets || !offsets_out || !num_keys_out || !max_count || (num_keys > 0 && !keys)) {
+    set_error("null operand");
+    return B200KGE_ERR_INVALID;
+  }
+  if (vocab <= 0) { set_error("vocabulary size must be positive"); return B200KGE_ERR_INVALID; }
+  // every offset is checked before any value is read: nnz and the values' extent rest on them
+  for (int64_t k = 0; k < num_keys; ++k)
+    if (offsets[k + 1] < offsets[k]) { set_error("offsets must not decrease"); return B200KGE_ERR_INVALID; }
+  const int64_t base = offsets[0], nnz = offsets[num_keys] - base;
+  if (nnz > 0 && (!values || !keys_out || !values_out)) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  // one (key0, key1, value) entry per listed value; sorting and dropping repeats gives sorted unique keys and sorted
+  // distinct values per key whatever order or repeats the input had (a split may repeat a triple)
+  struct Entry { int64_t a, b, v; };
+  std::vector<Entry> ent;
+  ent.reserve((size_t)nnz);
+  for (int64_t k = 0; k < num_keys; ++k) {
+    for (int64_t j = offsets[k]; j < offsets[k + 1]; ++j) {
+      const int64_t v = values[j - base];
+      if (v < 0 || v >= vocab) {
+        set_error("value %lld of key (%lld, %lld) outside [0, %lld)", (long long)v, (long long)keys[2 * k],
+                  (long long)keys[2 * k + 1], (long long)vocab);
+        return B200KGE_ERR_INVALID;
+      }
+      ent.push_back({keys[2 * k], keys[2 * k + 1], v});
+    }
+  }
+  auto lt = [](const Entry& x, const Entry& y) {
+    return x.a != y.a ? x.a < y.a : x.b != y.b ? x.b < y.b : x.v < y.v;
+  };
+  std::sort(ent.begin(), ent.end(), lt);
+  ent.erase(std::unique(ent.begin(), ent.end(),
+                        [](const Entry& x, const Entry& y) { return x.a == y.a && x.b == y.b && x.v == y.v; }),
+            ent.end());
+  int64_t nk = 0, mx = 0;
+  for (size_t i = 0; i < ent.size(); ++i) {
+    if (i == 0 || ent[i].a != ent[i - 1].a || ent[i].b != ent[i - 1].b) {
+      if (nk > 0) mx = std::max(mx, (int64_t)i - offsets_out[nk - 1]);
+      keys_out[2 * nk] = ent[i].a;
+      keys_out[2 * nk + 1] = ent[i].b;
+      offsets_out[nk++] = (int64_t)i;
+    }
+    values_out[i] = ent[i].v;
+  }
+  if (nk > 0) mx = std::max(mx, (int64_t)ent.size() - offsets_out[nk - 1]);
+  offsets_out[nk] = (int64_t)ent.size();
+  *num_keys_out = nk;
+  *max_count = mx;
+  return 0;
+}
+
 }  // extern "C"

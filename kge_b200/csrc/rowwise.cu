@@ -393,7 +393,91 @@ sample_uniform_kernel(uint64_t seed, uint64_t offset, uint64_t vocab, int64_t to
   if (2 * pair + 1 < total) out[2 * pair + 1] = (int64_t)__umul64hi(r1, vocab);
 }
 
+// Filtered uniform sampling (KgeSampler with filtering.<slot>, sampler.py:108-128,163-196,700-752).  Element
+// e = i*K + k first takes sample_uniform_kernel's draw x (block (e/2, offset) under key seed, words (0,1) | (2,3) by the
+// parity of e).  If x is not one of the m sorted, distinct positives of row i's key, the output is x.  Otherwise one
+// second draw u = floor(r' * (vocab - m) / 2^64) picks the u-th non-positive id, where r' is word pair (e & 1) of block
+// (e/2 | 2^63, offset) under the same key: a counter the first draw never reaches (its block index is below 2^62).
+// P(y) = 1/V + (m/V) * 1/(V-m) = 1/(V-m) for every non-positive y: the distribution of the reference's redraw loop, with
+// no loop whose length depends on chance.  The u-th non-positive is u + c, c = #{j : values[j] - j <= u} (values[j] - j
+// counts the non-positives below values[j] and does not decrease in j).  A row whose key is absent has m = 0; a row
+// with m >= vocab has no non-positive and gets -1.
+constexpr uint64_t FILTER_DOMAIN = 1ull << 63;
+
+__device__ __forceinline__ uint64_t philox_u64(uint64_t seed, uint64_t offset, uint64_t block, bool odd) {
+  uint32_t c[4] = {(uint32_t)block, (uint32_t)(block >> 32), (uint32_t)offset, (uint32_t)(offset >> 32)};
+  philox4x32_10(c, seed);
+  return odd ? ((uint64_t)c[3] << 32) | c[2] : ((uint64_t)c[1] << 32) | c[0];
+}
+
+// one CTA per row: thread 0 looks the row's key up once, every thread then takes elements k, k + blockDim.x, ...
+__global__ void __launch_bounds__(256)
+sample_uniform_filtered_kernel(uint64_t seed, uint64_t offset, uint64_t vocab, int64_t K, const int64_t* __restrict__ tri,
+                               int c0, int c1, const int64_t* __restrict__ keys, const int64_t* __restrict__ offsets,
+                               const int64_t* __restrict__ values, int64_t num_keys, int64_t* __restrict__ out) {
+  __shared__ int64_t s_begin, s_m;
+  const int64_t i = blockIdx.x;
+  if (threadIdx.x == 0) {
+    const int64_t a = tri[3 * i + c0], b = tri[3 * i + c1];
+    int64_t lo = 0, hi = num_keys;
+    while (lo < hi) {
+      const int64_t mid = lo + ((hi - lo) >> 1);
+      const int64_t ka = keys[2 * mid], kb = keys[2 * mid + 1];
+      if (ka < a || (ka == a && kb < b)) lo = mid + 1;
+      else hi = mid;
+    }
+    int64_t begin = 0, m = 0;
+    if (lo < num_keys && keys[2 * lo] == a && keys[2 * lo + 1] == b) {
+      begin = offsets[lo];
+      m = offsets[lo + 1] - begin;
+    }
+    s_begin = begin;
+    s_m = m;
+  }
+  __syncthreads();
+  const int64_t* __restrict__ v = values + s_begin;
+  const int64_t m = s_m;
+  int64_t* __restrict__ orow = out + i * K;
+  if ((uint64_t)m >= vocab) {
+    for (int64_t k = threadIdx.x; k < K; k += blockDim.x) orow[k] = -1;
+    return;
+  }
+  for (int64_t k = threadIdx.x; k < K; k += blockDim.x) {
+    const uint64_t e = (uint64_t)(i * K + k);
+    const int64_t x = (int64_t)__umul64hi(philox_u64(seed, offset, e >> 1, e & 1), vocab);
+    int64_t lo = 0, hi = m;                  // lower bound of x among the positives
+    while (lo < hi) {
+      const int64_t mid = lo + ((hi - lo) >> 1);
+      if (__ldg(v + mid) < x) lo = mid + 1;
+      else hi = mid;
+    }
+    if (lo == m || __ldg(v + lo) != x) { orow[k] = x; continue; }
+    const int64_t u = (int64_t)__umul64hi(philox_u64(seed, offset, (e >> 1) | FILTER_DOMAIN, e & 1), vocab - (uint64_t)m);
+    lo = 0; hi = m;                          // c = #{j : v[j] - j <= u}
+    while (lo < hi) {
+      const int64_t mid = lo + ((hi - lo) >> 1);
+      if (__ldg(v + mid) - mid <= u) lo = mid + 1;
+      else hi = mid;
+    }
+    orow[k] = u + lo;
+  }
+}
+
 }  // namespace
+
+int launch_sample_uniform_filtered(uint64_t seed, uint64_t offset, int64_t vocab, int64_t n, int64_t K,
+                                   const int64_t* triples, int slot, const int64_t* keys, const int64_t* offsets,
+                                   const int64_t* values, int64_t num_keys, int64_t* out, cudaStream_t st) {
+  if (n <= 0 || K <= 0) return 0;
+  if (n > 2147483647LL) { set_error("too many rows (%lld)", (long long)n); return B200KGE_ERR_UNSUPPORTED; }
+  // the key pair of each slot: (p, o) for S, (s, o) for P, (s, p) for O (sampler.py:167-173)
+  const int c0 = slot == 0 ? 1 : 0, c1 = slot == 2 ? 1 : 2;
+  const int threads = K >= 256 ? 256 : (int)((K + 31) / 32) * 32;
+  sample_uniform_filtered_kernel<<<(unsigned)n, threads, 0, st>>>(seed, offset, (uint64_t)vocab, K, triples, c0, c1,
+                                                                   keys, offsets, values, num_keys, out);
+  B2K_LAUNCH_CHECK("sample_uniform_filtered_kernel");
+  return 0;
+}
 
 int launch_sample_uniform(uint64_t seed, uint64_t offset, int64_t vocab, int64_t total, int64_t* out, cudaStream_t st) {
   if (total <= 0) return 0;

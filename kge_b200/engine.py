@@ -474,6 +474,40 @@ def sample_uniform(n: int, K: int, vocab: int, seed: int, offset: int, device) -
     return out
 
 
+class FilterIndex:
+    """The positives of one negative-sampling slot, resident on `device`: keys [k,2], offsets [k+1], values [nnz] (int64,
+    include/b200kge.h b200kge_filter_index_build) built once on the host from a KvsAllIndex (`dataset.index(...)` of the
+    reference, or kge_b200.indexing's).  `max_count` is the largest number of distinct positives of one key."""
+
+    def __init__(self, index, vocab: int, device):
+        from .indexing import filter_csr
+
+        keys, offsets, values, self.max_count = filter_csr(index, vocab)
+        self.vocab = int(vocab)
+        self.keys, self.offsets, self.values = (t.to(device) for t in (keys, offsets, values))
+
+    def __len__(self) -> int:
+        return self.keys.shape[0]
+
+
+def sample_uniform_filtered(n: int, K: int, vocab: int, seed: int, offset: int, triples: torch.Tensor, slot: int,
+                            index: FilterIndex) -> torch.Tensor:
+    """[n, K] int64 ids ~ U({0..vocab-1} minus the positives of row i's key) drawn on the device; the key of row i of
+    triples [n,3] is (p, o) for slot S, (s, o) for P, (s, p) for O.  Positions whose first draw is not a positive equal
+    sample_uniform(n, K, vocab, seed, offset); rows whose positives cover the vocabulary get -1."""
+    if index.vocab != vocab:
+        raise ValueError(f"the filter index was built for a vocabulary of {index.vocab}, not {vocab}")
+    _require_cuda(triples, index.keys)
+    tri = triples if (triples.dtype == torch.int64 and triples.is_contiguous()) else triples.long().contiguous()
+    if tri.dim() != 2 or tri.shape[1] != 3 or tri.shape[0] != n:
+        raise ValueError(f"expected triples [{n}, 3], got {tuple(tri.shape)}")
+    out = torch.empty((n, K), dtype=torch.int64, device=tri.device)
+    _lib.check(_lib.load().b200kge_sample_uniform_filtered(
+        seed & (2 ** 64 - 1), offset & (2 ** 64 - 1), vocab, n, K, tri.data_ptr(), int(slot), index.keys.data_ptr(),
+        index.offsets.data_ptr(), index.values.data_ptr(), len(index), out.data_ptr(), _stream(out.device)))
+    return out
+
+
 def train_1vsall_forward(model: str, ent, rel, triples, loss: str = "bce", offset: float = 0.0,
                          l_norm: float = 1.0, precision: str = "auto", out=None, workspace=None,
                          dropout: Optional["DropoutKey"] = None):

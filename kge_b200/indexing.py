@@ -128,6 +128,26 @@ def index_KvsAll(triples: torch.Tensor, key: str) -> KvsAllIndex:
     return KvsAllIndex(triples, cols, val, list)
 
 
+def filter_csr(index, vocab: int) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, int]:
+    """(keys [k,2], offsets [k+1], values [nnz], largest count) int64: the filter index of negative sampling
+    (b200kge_filter_index_build) from a KvsAllIndex — the reference's or this module's, both have `_keys`,
+    `_values_offset` and `_values`.  Keys sorted and unique, values sorted and distinct per key, all in [0, vocab)."""
+    keys, offs, vals = _i64(index._keys).view(-1, 2), _i64(index._values_offset).view(-1), _i64(index._values).view(-1)
+    k = keys.shape[0]
+    cap = max(int(offs[k] - offs[0]), 0)
+    keys_out = torch.empty((k, 2), dtype=torch.int64)
+    offs_out = torch.empty((k + 1,), dtype=torch.int64)
+    vals_out = torch.empty((cap,), dtype=torch.int64)
+    import ctypes as C
+
+    nk, mx = C.c_int64(0), C.c_int64(0)
+    _lib.check(_lib.load().b200kge_filter_index_build(
+        keys.data_ptr(), offs.data_ptr(), vals.data_ptr(), k, int(vocab), keys_out.data_ptr(), offs_out.data_ptr(),
+        vals_out.data_ptr(), C.byref(nk), C.byref(mx)))
+    nk = nk.value
+    return keys_out[:nk].clone(), offs_out[: nk + 1].clone(), vals_out[: int(offs_out[nk])].clone(), mx.value
+
+
 def sp_po_label_csr(triples: torch.Tensor, num_entities: int, sp_index: KvsAllIndex, po_index: KvsAllIndex,
                     ) -> Tuple[torch.Tensor, torch.Tensor]:
     """CSR over the [n, 2E] label / filter matrix of a batch of (s,p,o) triples: known objects of (s,p,?) in

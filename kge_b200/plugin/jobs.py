@@ -340,10 +340,12 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
     rows and scores them, with the positive triple in column 0 — neither `[n*K, D]` gathers (`triple`
     implementation, sampler.py:294-305) nor scoring against all unique targets (`batch`, :306-339).
 
-    With `user.b200_device_sampling: true` (LibKGE's free-form `user.*` option space) and the default sampler
-    settings (uniform, not shared, no filtering) the negatives are also DRAWN on the device (Philox, keyed by the
-    torch seed, counter = batch / slot): the DataLoader workers only slice the triples, and no [n, K] id tensors
-    travel host -> device (KgeUniformSampler._sample, sampler.py:588-596, is a CPU torch.randint)."""
+    With `user.b200_device_sampling: true` (LibKGE's free-form `user.*` option space) and a uniform, not shared
+    sampler the negatives are also DRAWN on the device (Philox, keyed by the torch seed, counter = batch / slot): the
+    DataLoader workers only slice the triples, and no [n, K] id tensors travel host -> device
+    (KgeUniformSampler._sample, sampler.py:588-596, is a CPU torch.randint).  `negative_sampling.filtering.<slot>` is
+    served there too: the sampling kernel replaces positives of the filtering split with uniform non-positives
+    (engine.sample_uniform_filtered), from an index uploaded once when the job is created."""
 
     def __init__(self, config, dataset, parent_job=None, model=None, forward_only=False):
         super().__init__(config, dataset, parent_job, model=model, forward_only=forward_only)
@@ -352,8 +354,8 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
         except KeyError:
             want = False
         sm = self._sampler
-        self._device_sampling = bool(
-            want and type(sm).__name__ == "KgeUniformSampler" and not sm.shared and not any(sm.filter_positives))
+        self._device_sampling = bool(want and type(sm).__name__ == "KgeUniformSampler" and not sm.shared)
+        self._filter_index = self._b200_filter_indexes() if self._device_sampling else {}
         self._sample_calls = 0
         if self.__class__ == B200TrainingJobNegativeSampling:
             for f in Job.job_created_hooks:
@@ -367,15 +369,37 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
             return {"triples": self.dataset.split(self.train_split)[batch, :].long(), "negative_samples": []}
         return collate
 
-    def _device_negatives(self, n, slot, batch_index):
-        from .. import engine
+    def _b200_filter_indexes(self):
+        """{slot: engine.FilterIndex} for every sampled slot with `negative_sampling.filtering.<slot>`: the positives of
+        the sampler's filtering split (the index the sampler created, sampler.py:44-48), uploaded once.  A key whose
+        positives cover the vocabulary is refused here: the reference's redraw loop would never end on it."""
+        sm = self._sampler
+        out = {}
+        for slot in (S, P, O):
+            if not sm.filter_positives[slot] or sm.num_samples[slot] <= 0:
+                continue
+            name = f"{sm.filtering_split}_{['po', 'so', 'sp'][slot]}_to_{SLOT_STR[slot]}"
+            vocab = int(sm.vocabulary_size[slot])
+            index = engine.FilterIndex(self.dataset.index(name), vocab, self.device)
+            if index.max_count >= vocab:
+                raise NotImplementedError(
+                    f"negative_sampling.filtering.{SLOT_STR[slot]}: a key of {name} has all {vocab} ids as positives, "
+                    "so no negative exists for it")
+            out[slot] = index
+        return out
 
+    def _device_negatives(self, n, slot, batch_index, triples):
         sm = self._sampler
         # one independent stream per (epoch, batch, slot); the key follows torch.manual_seed
         offset = ((self.epoch * (1 << 24) + batch_index) << 2) | slot
         self._sample_calls += 1
-        return engine.sample_uniform(n, int(sm.num_samples[slot]), int(sm.vocabulary_size[slot]),
-                                     torch.initial_seed(), offset, self.device)
+        K, vocab = int(sm.num_samples[slot]), int(sm.vocabulary_size[slot])
+        index = self._filter_index.get(slot)
+        if index is None:
+            return engine.sample_uniform(n, K, vocab, torch.initial_seed(), offset, self.device)
+        # the dataset's own triples: with reciprocal relations the S slot is filtered on (p, o), as the reference's
+        # sampler sees them; the (o, p + R, s') rewrite happens only when scoring
+        return engine.sample_uniform_filtered(n, K, vocab, torch.initial_seed(), offset, triples, slot, index)
 
     def _b200_ns_dropout_route(self, kind, slots):
         """(b200 model, (p_ent, p_rel)) if `user.b200_ns_dropout` is on, embedding dropout is active and the dropout
@@ -435,7 +459,13 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
             return super()._process_subbatch(batch_index, batch, subbatch_slice, result)
         batch_size = result.size
         result.prepare_time -= time.time()
-        triples = batch["triples"][subbatch_slice]
+        triples = batch["triples"]
+        if self._filter_index:
+            # one device copy of the batch's triples serves the filtered sampling of every slot and the scoring
+            if "b200_triples" not in batch:
+                batch["b200_triples"] = triples.to(self.device)
+            triples = batch["b200_triples"]
+        triples = triples[subbatch_slice]
         negs = batch["negative_samples"]
         subbatch_size = len(triples)
         labels = batch["labels"]
@@ -450,7 +480,7 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
                 if negs == [] or len(negs) < 3:
                     negs = batch["negative_samples"] = [None, None, None]
                 if negs[slot] is None:          # drawn once per batch and slot, sliced per sub-batch
-                    negs[slot] = self._device_negatives(batch_size, slot, batch_index)
+                    negs[slot] = self._device_negatives(batch_size, slot, batch_index, batch.get("b200_triples"))
                 negatives = negs[slot][subbatch_slice]
             else:
                 negatives = negs[slot].samples(subbatch_slice if (subbatch_size != batch_size) else None)
