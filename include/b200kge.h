@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define B200KGE_VERSION 100
+#define B200KGE_VERSION 101
 
 typedef void* b200kge_stream_t; /* cudaStream_t */
 
@@ -295,18 +295,84 @@ int b200kge_sample_uniform_filtered(uint64_t seed, uint64_t offset, int64_t voca
                                     const int64_t* triples, int slot, const int64_t* keys, const int64_t* offsets,
                                     const int64_t* values, int64_t num_keys, int64_t* out, b200kge_stream_t stream);
 
-/* One whole 1vsAll forward step (train_1vsAll.py:48-82) for a batch of triples [n,3] (int64,
- * row-major s,p,o): fused score_sp+loss and score_po+loss against the whole entity table, both
- * directions stacked into one launch of 2n query rows where the model allows it.  loss_out[0]
- * (device) receives  (loss(score_sp, o) + loss(score_po, s)) / n.  `ent`/`rel` are the
- * device-resident tables (idx must be NULL). */
-int b200kge_train_1vsall_forward(int model, float l_norm, int precision,
-                                 const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                 const int64_t* triples, int64_t n, int loss_kind, float offset,
-                                 float* loss_out, void* workspace, size_t workspace_bytes,
-                                 b200kge_stream_t stream);
+/* ---- Embedding dropout of the 1vsAll / KvsAll training steps ---------------------------------------------------------
+ * LookupEmbedder._postprocess (lookup_embedder.py:96-105) draws a fresh element-wise Bernoulli mask per embed(idx) /
+ * embed_all() call and scales kept values by 1/(1-p).  One sub-batch of 1vsAll training (train_1vsAll.py:64,75 with
+ * kge_model.py:682-721) makes six independent draws, numbered as mask streams:
+ *   score_sp(s, p): 0 = embed(s), 1 = embed(p), 2 = embed_all()       (entity, relation, entity table)
+ *   score_po(p, o): 3 = embed_all(), 4 = embed(p), 5 = embed(o)       (entity table, relation, entity)
+ * so the two directions use different masks on the candidate table and on p.  KvsAll (train_KvsAll.py:274-285) draws
+ * streams 0-2 for its sp_ queries and 3-5 for its _po queries.
+ *
+ * Mask layout (never stored: the backward regenerates the forward's mask from the same key):
+ *   element (row, k) of a draw over rows of width dim has elem = row * dim + k, where row is the GLOBAL row: the entity
+ *   id for the table draws (2, 3), row_base + i for row i of the sub-batch's queries (0, 1, 4, 5);
+ *   Philox4x32-10 with key = seed (64 bits) and counter = ((stream << 46) | (elem >> 2), call), both 64-bit halves
+ *   little-endian as four 32-bit words; the element takes output word elem & 3;
+ *   kept iff word < floor((1 - p) * 2^32), kept value x * (1 / (1 - p)) in fp32.
+ * Requirements (else B200KGE_ERR_INVALID): 0 <= p < 1; row_base >= 0; elem < 2^48 for every element of every draw. */
+#define B200KGE_DROP_SP_ENT 0
+#define B200KGE_DROP_SP_REL 1
+#define B200KGE_DROP_SP_TABLE 2
+#define B200KGE_DROP_PO_TABLE 3
+#define B200KGE_DROP_PO_REL 4
+#define B200KGE_DROP_PO_ENT 5
 
-/* Host-buffer form of the same step (end-to-end measurement, embedding in a host-side loop):
+typedef struct {
+  float p_ent;      /* entity_embedder.dropout   */
+  float p_rel;      /* relation_embedder.dropout */
+  uint64_t seed;    /* Philox key                */
+  uint64_t call;    /* one value per sub-batch (e.g. from epoch, batch index, sub-batch ordinal) */
+  int64_t row_base; /* global index of the sub-batch's first query row */
+} b200kge_dropout_t;
+
+/* The keep mask of one draw: out[i * dim + k] = 1 if element (row_base + i, k) of stream `mask_stream` is kept, else 0,
+ * for i < rows, k < dim (uint8, device). */
+int b200kge_dropout_mask(float p, uint64_t seed, uint64_t call, int mask_stream, int64_t row_base, int64_t rows,
+                         int32_t dim, uint8_t* out, b200kge_stream_t stream);
+
+/* One whole 1vsAll forward step (train_1vsAll.py:48-82) for a batch of triples [n,3] (int64,
+ * row-major s,p,o).  `ent`/`rel` are the device-resident tables (idx must be NULL).
+ *   num_relations = 0: loss_out[0] (device) receives  (loss(score_sp, o) + loss(score_po, s)) / n.  Fused
+ *     score_sp+loss and score_po+loss against the whole entity table, both directions stacked into one launch of 2n
+ *     query rows where the model allows it.
+ *   num_relations = R > 0: the step of a reciprocal-relations model.  LibKGE's ReciprocalRelationsModel
+ *     (reciprocal_relations_model.py:85-92) keeps 2R relation rows and answers score_po as the sp_ query (o, p + R)
+ *     against the same table, so loss_out[0] receives  (loss(score_sp(s, p), o) + loss(score_sp(o, p + R), s)) / n.
+ *     rel->rows must be 2 * num_relations (else B200KGE_ERR_INVALID, as for num_relations < 0).  Without dropout this
+ *     is the stacked problem with the rows [n, 2n) folded as sp_ queries (o_i, p_i + R), labelled s_i — CP included,
+ *     which stacks here because both halves read the table columns [D/2, D).
+ *   drop == NULL: no dropout.  Otherwise the six draws above are applied to gathered copies of the query rows, the
+ *     relation rows and one table copy per direction, and each direction runs the per-direction scorer on those
+ *     copies.  With num_relations > 0, direction 0 draws streams 0-2 as the plain step and direction 1 draws the _po
+ *     streams 3-5 (embed_all, embed(p + R), embed(o)), with the mask rows of the plain step.
+ * Every model and norm.  Workspace: b200kge_train_1vsall_workspace_bytes(model, n, E, D, drop != NULL); without
+ * dropout b200kge_workspace_bytes(model, n, E, D, 0) is enough for the forward. */
+int b200kge_train_1vsall_forward(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                                 const b200kge_rows_t* rel, int64_t num_relations, const int64_t* triples, int64_t n,
+                                 int loss_kind, float offset, const b200kge_dropout_t* drop, float* loss_out,
+                                 void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+
+/* Backward of b200kge_train_1vsall_forward (loss.backward() at kge/job/train_1vsAll.py:70,81) with BCE or KL and the
+ * forward's num_relations and drop: dense gradients of the entity table d_ent [E, lde] and of the relation table d_rel
+ * [R, ldr] (all 2R rows for a reciprocal-relations model) of the forward's loss.  Both buffers are OVERWRITTEN (the
+ * reference accumulates into .grad; add them there).  Models: the dot family (tensor-core GEMMs) and TransE (l_norm 1,
+ * 2) / RotatE (l_norm 1) (CUDA-core row-gradient passes, grad_distance.cu: dQ_i = sum_j G_ij s'(Q_i - T_j),
+ * dT_j = sum_i G_ij s'(T_j - Q_i)).  Recompute-based: scores, G = n dL/dz (sigmoid(z+off) - y | softmax(z) - y), two
+ * split-K tensor-core GEMMs on fp16 hi/lo planes (dT = G^T Q, dQ = G T), row-wise unfold of dQ through the relation
+ * fold (grad.cu); the reciprocal half unfolds into d_ent[o], d_rel[p + R].  With `drop`, each direction runs that
+ * machinery on its masked copies and the table and row gradients are masked with the same draws before they are added
+ * into d_ent / d_rel.  Workspace: b200kge_train_1vsall_workspace_bytes(model, n, E, D, drop != NULL). */
+int b200kge_train_1vsall_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                  int64_t num_relations, const int64_t* triples, int64_t n, int loss_kind, float offset,
+                                  const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
+                                  void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+
+/* Bytes of workspace sufficient for b200kge_train_1vsall_forward and _backward with n triples, E entities of width D,
+ * plain or reciprocal, with dropout (dropout != 0) or without. */
+size_t b200kge_train_1vsall_workspace_bytes(int model, int64_t n, int64_t E, int32_t D, int dropout);
+
+/* Host-buffer form of the plain forward step (end-to-end measurement, embedding in a host-side loop):
  * copies triples_host [n,3] to the device (triples.to(device), train_1vsAll.py:59), runs
  * b200kge_train_1vsall_forward, copies the scalar back to *loss_host (.item(), :66,77) and
  * synchronises the stream. */
@@ -368,18 +434,6 @@ int b200kge_gemm_nt(const float* A, int64_t lda, const float* B, int64_t ldb, in
                       int64_t K, float* C, int64_t ldc, void* workspace, size_t workspace_bytes,
                       b200kge_stream_t stream);
 
-/* Backward of b200kge_train_1vsall_forward (loss.backward() at kge/job/train_1vsAll.py:70,81) with BCE or KL, for the
- * dot family (tensor-core GEMMs, below) and for TransE (l_norm 1, 2) / RotatE (l_norm 1) (CUDA-core row-gradient passes,
- * grad_distance.cu: dQ_i = sum_j G_ij s'(Q_i - T_j), dT_j = sum_i G_ij s'(T_j - Q_i)): dense gradients of the entity table d_ent [E, lde] and of the relation table d_rel
- * [R, ldr] of  (loss(score_sp, o) + loss(score_po, s)) / n.  Both buffers are overwritten (the reference
- * accumulates into .grad; add them there).  Recompute-based: scores, G = n dL/dz (sigmoid(z+off) - y | softmax(z) - y), two tensor-core
- * GEMMs (dT = G^T Q, dQ = G T), row-wise unfold of dQ through the relation fold (grad.cu). */
-size_t b200kge_train_1vsall_backward_workspace_bytes(int model, int64_t n, int64_t E, int32_t D);
-int b200kge_train_1vsall_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                    const int64_t* triples, int64_t n, int loss_kind, float offset,
-                                    float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                                    void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
-
 /* Backward of b200kge_score_1vsN over the whole entity table for the dot family (the unfused route: a job computes a
  * dense [n, E] score matrix, its loss, and autograd hands back grad_scores = dL/dscores [n, ldg]): dense gradients of
  * the entity table d_ent [E, lde] and the relation table d_rel [R, ldr], both OVERWRITTEN.  Fold of the n query rows,
@@ -400,20 +454,19 @@ int b200kge_score_1vsN_backward(int model, int combine, float l_norm, const b200
  *   TransE (l_norm 1, 2) / RotatE (l_norm 1): recompute on the CUDA-core scorer, dense fp32 G (label-free value, then
  *     each row's listed columns by the row's own thread block; KL: row log-sum-exp first), the two row-gradient passes
  *     of b200kge_train_1vsall_backward, unfold.  Other norms: B200KGE_ERR_UNSUPPORTED before any launch.
- * The plain entry is the _norm entry with l_norm = 1.  Workspace: b200kge_score_1vsN_backward_workspace_bytes (the
+ *   l_norm is ignored by the dot family.
+ * drop == NULL: no dropout, and mask_dir is ignored.  Workspace: b200kge_score_1vsN_backward_workspace_bytes (the
  * distance family: Q, dQ [n, round_up(D, 32)] each, triples [3n] and the KL row statistics [2n floats] in its n * 4 * 8
- * bytes, scores and G [n, round_up(E, 4)] each, G^T [E, round_up(n, 4)], the scorer's workspace). */
-int b200kge_score_1vsN_loss_csr_backward(int model, int combine, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                         const int64_t* q_idx, const int64_t* p_idx, int64_t n, const int64_t* csr_off,
-                                         const int64_t* csr_col, float label_smoothing, int loss_kind, float offset,
-                                         int64_t batch_size, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                                         void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
-int b200kge_score_1vsN_loss_csr_backward_norm(int model, int combine, float l_norm, const b200kge_rows_t* ent,
-                                              const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx,
-                                              int64_t n, const int64_t* csr_off, const int64_t* csr_col,
-                                              float label_smoothing, int loss_kind, float offset, int64_t batch_size,
-                                              float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
-                                              size_t workspace_bytes, b200kge_stream_t stream);
+ * bytes, scores and G [n, round_up(E, 4)] each, G^T [E, round_up(n, 4)], the scorer's workspace).
+ * drop != NULL: the backward of b200kge_score_1vsN_loss_csr_dropout under the same key and mask_dir (same models and
+ * norms).  The masks are regenerated, and the table and row gradients of the masked copies are masked with the same
+ * draws before they are added into d_ent / d_rel.  Workspace: b200kge_score_1vsN_loss_csr_dropout_workspace_bytes. */
+int b200kge_score_1vsN_loss_csr_backward(int model, int combine, int mask_dir, float l_norm, const b200kge_rows_t* ent,
+                                         const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx,
+                                         int64_t n, const int64_t* csr_off, const int64_t* csr_col,
+                                         float label_smoothing, int loss_kind, float offset, int64_t batch_size,
+                                         const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
+                                         int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
 
 /* KvsAll loss with CSR multi-hot labels (kge/job/train_KvsAll.py:242-300 without the densified label matrix):
  * row i's labels are the columns csr_col[csr_off[i] .. csr_off[i+1]) (sorted; a repeated column counts as often
@@ -432,16 +485,6 @@ int b200kge_score_1vsN_loss_csr(int model, int combine, float l_norm, int precis
                                   float offset, float* loss_out, float* row_loss_out, void* workspace,
                                   size_t workspace_bytes, b200kge_stream_t stream);
 
-/* Backward of one slot of a negative-sampling batch with BCE (kge/job/train_negative_sampling.py:113-164): the
- * [n, 1+K] block of the slot (column 0 = the positive triple, label 1; columns 1.. = the sampled ids neg [n,K],
- * label 0), loss summed and divided by batch_size.  ADDS into d_ent [E, lde] and d_rel [R, ldr] (zero them before
- * the first slot).  slot 0 (S) or 2 (O); TransE with l_norm 1 or 2, RotatE with l_norm 1, and the dot family.
- * workspace: n * round_up(K_folded, 32) floats. */
-int b200kge_ns_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                          const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K,
-                          float offset, int64_t batch_size, float* d_ent, int64_t lde, float* d_rel,
-                          int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
-
 /* KgeLoss of a negative-sampling block (kge/job/train_negative_sampling.py:126-156 with kge/util/loss.py:139-274):
  * scores [n, m] (row stride lds), one positive per row at column label_idx[i] (NULL: column 0, the layout of
  * b200kge_ns_score with with_positive = 1), every other column a negative (label 0).  Any b200kge_loss kind; `arg` is
@@ -459,16 +502,6 @@ int b200kge_ns_loss(const float* scores, int64_t lds, int64_t n, int64_t m, cons
                     float* row_loss_out, float* grad_out, int64_t ldg, void* workspace,
                     size_t workspace_bytes, b200kge_stream_t stream);
 
-/* b200kge_ns_backward with the gradient of the block given: grad_scores [n, 1+K] (row stride ldg; column 0 the positive,
- * columns 1.. the sampled ids neg [n, K]) holds dL/dz already scaled (e.g. the grad_out of b200kge_ns_loss with
- * scale = 1 / batch_size).  The fold, per-column walk, scatter and unfold are those of b200kge_ns_backward; only the
- * per-column gradient is read instead of computed — so every loss of b200kge_ns_loss trains through the same kernel
- * (loss.backward() at train_negative_sampling.py:164).  ADDS into d_ent / d_rel; same slots, models and workspace. */
-int b200kge_ns_backward_grad(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                             const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K,
-                             const float* grad_scores, int64_t ldg, float* d_ent, int64_t lde, float* d_rel,
-                             int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
-
 /* LookupEmbedder.penalty (kge/model/embedder/lookup_embedder.py:123-177) on the rows view `rows` (the whole
  * table, or the batch's unique rows through rows->idx with their `counts`, NULL = all ones):
  *   *out = scale * sum_r counts[r] * sum_k |x_rk|^p        (complex_abs: x -> sqrt(re^2 + im^2 + 1e-14): "n3",
@@ -484,130 +517,21 @@ int b200kge_lookup_penalty(const b200kge_rows_t* rows, const float* counts, floa
 int b200kge_normalize_rows(float* weight, int64_t ld, int64_t rows, int32_t dim, float p,
                              b200kge_stream_t stream);
 
-/* ---- Embedding dropout of the 1vsAll / KvsAll training steps ---------------------------------------------------------
- * LookupEmbedder._postprocess (lookup_embedder.py:96-105) draws a fresh element-wise Bernoulli mask per embed(idx) /
- * embed_all() call and scales kept values by 1/(1-p).  One sub-batch of 1vsAll training (train_1vsAll.py:64,75 with
- * kge_model.py:682-721) makes six independent draws, numbered as mask streams:
- *   score_sp(s, p): 0 = embed(s), 1 = embed(p), 2 = embed_all()       (entity, relation, entity table)
- *   score_po(p, o): 3 = embed_all(), 4 = embed(p), 5 = embed(o)       (entity table, relation, entity)
- * so the two directions use different masks on the candidate table and on p.  KvsAll (train_KvsAll.py:274-285) draws
- * streams 0-2 for its sp_ queries and 3-5 for its _po queries.
- *
- * Mask layout (never stored: the backward regenerates the forward's mask from the same key):
- *   element (row, k) of a draw over rows of width dim has elem = row * dim + k, where row is the GLOBAL row: the entity
- *   id for the table draws (2, 3), row_base + i for row i of the sub-batch's queries (0, 1, 4, 5);
- *   Philox4x32-10 with key = seed (64 bits) and counter = ((stream << 46) | (elem >> 2), call), both 64-bit halves
- *   little-endian as four 32-bit words; the element takes output word elem & 3;
- *   kept iff word < floor((1 - p) * 2^32), kept value x * (1 / (1 - p)) in fp32.
- * Requirements (else B200KGE_ERR_INVALID): 0 <= p < 1; row_base >= 0; elem < 2^48 for every element of every draw. */
-#define B200KGE_DROP_SP_ENT 0
-#define B200KGE_DROP_SP_REL 1
-#define B200KGE_DROP_SP_TABLE 2
-#define B200KGE_DROP_PO_TABLE 3
-#define B200KGE_DROP_PO_REL 4
-#define B200KGE_DROP_PO_ENT 5
-
-typedef struct {
-  float p_ent;      /* entity_embedder.dropout   */
-  float p_rel;      /* relation_embedder.dropout */
-  uint64_t seed;    /* Philox key                */
-  uint64_t call;    /* one value per sub-batch (e.g. from epoch, batch index, sub-batch ordinal) */
-  int64_t row_base; /* global index of the sub-batch's first query row */
-} b200kge_dropout_t;
-
-/* The keep mask of one draw: out[i * dim + k] = 1 if element (row_base + i, k) of stream `mask_stream` is kept, else 0,
- * for i < rows, k < dim (uint8, device). */
-int b200kge_dropout_mask(float p, uint64_t seed, uint64_t call, int mask_stream, int64_t row_base, int64_t rows,
-                         int32_t dim, uint8_t* out, b200kge_stream_t stream);
-
-/* b200kge_train_1vsall_forward / _backward with dropout: the six draws above, applied to gathered copies of the query
- * rows, the relation rows and one table copy per direction; each direction then runs the per-direction scorer (forward)
- * or gradient machinery (backward, same model coverage as b200kge_train_1vsall_backward) on those copies, and the
- * backward masks the table and row gradients with the same draws before adding them into d_ent / d_rel (OVERWRITTEN).
- * Workspace (either call): b200kge_train_1vsall_dropout_workspace_bytes. */
-size_t b200kge_train_1vsall_dropout_workspace_bytes(int model, int64_t n, int64_t E, int32_t D);
-int b200kge_train_1vsall_forward_dropout(int model, float l_norm, int precision, const b200kge_rows_t* ent,
-                                         const b200kge_rows_t* rel, const int64_t* triples, int64_t n, int loss_kind,
-                                         float offset, const b200kge_dropout_t* drop, float* loss_out, void* workspace,
-                                         size_t workspace_bytes, b200kge_stream_t stream);
-int b200kge_train_1vsall_backward_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                          const int64_t* triples, int64_t n, int loss_kind, float offset,
-                                          const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
-                                          int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
-
-/* b200kge_score_1vsN_loss_csr / _backward with dropout for one KvsAll query type: queries ent[q_idx] (stream 0 | 5),
- * relations rel[p_idx] (1 | 4) and the candidate table ent (2 | 3) for combine sp_ | _po.  The backward covers the models
- * and norms of b200kge_score_1vsN_loss_csr_backward (the plain dropout backward entries: l_norm 1; the _norm entry
- * below takes it) and OVERWRITES d_ent / d_rel.
+/* b200kge_score_1vsN_loss_csr with dropout for one KvsAll query type: queries ent[q_idx], relations rel[p_idx] and the
+ * candidate table ent.  `combine` is the query type's fold; `mask_dir` (B200KGE_SP_ | B200KGE__PO) selects the draws:
+ * streams 0-2 (queries 0, relations 1, table 2) | 3-5 (table 3, relations 4, queries 5).  A plain model's query type
+ * draws with mask_dir = combine; a reciprocal-relations model's _po query type is the sp_ fold of (q_idx = o,
+ * p_idx = p + R) on the _po streams (reciprocal_relations_model.py:85-92).  The backward is
+ * b200kge_score_1vsN_loss_csr_backward with the same drop and mask_dir.
  * Workspace (either call): b200kge_score_1vsN_loss_csr_dropout_workspace_bytes (the masked copies and per-direction
  * buffers, then the larger of the forward's and the backward's workspace). */
 size_t b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(int model, int64_t n, int64_t E, int32_t D, int64_t nnz);
-int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, float l_norm, int precision, const b200kge_rows_t* ent,
-                                        const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx, int64_t n,
-                                        const int64_t* csr_off, const int64_t* csr_col, int64_t nnz,
-                                        float label_smoothing, int loss_kind, float offset,
+int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, int mask_dir, float l_norm, int precision,
+                                        const b200kge_rows_t* ent, const b200kge_rows_t* rel, const int64_t* q_idx,
+                                        const int64_t* p_idx, int64_t n, const int64_t* csr_off, const int64_t* csr_col,
+                                        int64_t nnz, float label_smoothing, int loss_kind, float offset,
                                         const b200kge_dropout_t* drop, float* loss_out, float* row_loss_out,
                                         void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
-int b200kge_score_1vsN_loss_csr_backward_dropout(int model, int combine, const b200kge_rows_t* ent,
-                                                 const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx,
-                                                 int64_t n, const int64_t* csr_off, const int64_t* csr_col,
-                                                 float label_smoothing, int loss_kind, float offset, int64_t batch_size,
-                                                 const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
-                                                 int64_t ldr, void* workspace, size_t workspace_bytes,
-                                                 b200kge_stream_t stream);
-/* The same with the draws picked apart from the fold: `combine` is the query type's fold, `mask_dir` (B200KGE_SP_ |
- * B200KGE__PO) selects streams 0-2 | 3-5.  A reciprocal-relations model's _po query type is the sp_ fold of
- * (q_idx = o, p_idx = p + R) on the _po streams (reciprocal_relations_model.py:85-92); the plain entry points above
- * are these with mask_dir = combine.  Same workspace. */
-int b200kge_score_1vsN_loss_csr_dropout_dir(int model, int combine, int mask_dir, float l_norm, int precision,
-                                            const b200kge_rows_t* ent, const b200kge_rows_t* rel, const int64_t* q_idx,
-                                            const int64_t* p_idx, int64_t n, const int64_t* csr_off,
-                                            const int64_t* csr_col, int64_t nnz, float label_smoothing, int loss_kind,
-                                            float offset, const b200kge_dropout_t* drop, float* loss_out,
-                                            float* row_loss_out, void* workspace, size_t workspace_bytes,
-                                            b200kge_stream_t stream);
-int b200kge_score_1vsN_loss_csr_backward_dropout_dir(int model, int combine, int mask_dir, const b200kge_rows_t* ent,
-                                                     const b200kge_rows_t* rel, const int64_t* q_idx,
-                                                     const int64_t* p_idx, int64_t n, const int64_t* csr_off,
-                                                     const int64_t* csr_col, float label_smoothing, int loss_kind,
-                                                     float offset, int64_t batch_size, const b200kge_dropout_t* drop,
-                                                     float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                                                     void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
-/* b200kge_score_1vsN_loss_csr_backward_dropout_dir with the model's l_norm: TransE 1 | 2, RotatE 1 (else
- * B200KGE_ERR_UNSUPPORTED before any launch); ignored by the dot family.  Same workspace. */
-int b200kge_score_1vsN_loss_csr_backward_dropout_norm(int model, int combine, int mask_dir, float l_norm,
-                                                      const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                                      const int64_t* q_idx, const int64_t* p_idx, int64_t n,
-                                                      const int64_t* csr_off, const int64_t* csr_col,
-                                                      float label_smoothing, int loss_kind, float offset,
-                                                      int64_t batch_size, const b200kge_dropout_t* drop, float* d_ent,
-                                                      int64_t lde, float* d_rel, int64_t ldr, void* workspace,
-                                                      size_t workspace_bytes, b200kge_stream_t stream);
-
-/* ---- The 1vsAll step of a reciprocal-relations model ----------------------------------------------------------------
- * LibKGE's ReciprocalRelationsModel (reciprocal_relations_model.py:85-92) keeps 2R relation rows and answers score_po
- * as the sp_ query (o, p + R) against the same table.  The step is
- *   (loss(score_sp(s, p), o) + loss(score_sp(o, p + R), s)) / n
- * with rel->rows == 2 * num_relations (else B200KGE_ERR_INVALID).  Without dropout (drop == NULL) it is the stacked
- * problem of b200kge_train_1vsall_forward with the rows [n, 2n) folded as sp_ queries (o_i, p_i + R), labelled s_i —
- * CP included, which stacks here because both halves read the table columns [D/2, D).  The backward (OVERWRITES d_ent
- * and all 2R rows of d_rel) runs the same G planes / split-K GEMMs or distance row-gradient passes and unfolds the
- * second half into d_ent[o], d_rel[p + R].  With `drop`, direction 0 draws streams 0-2 as the plain step and
- * direction 1 draws the _po streams 3-5 (embed_all, embed(p + R), embed(o)), with the mask rows of the plain step.
- * Model coverage of both calls: that of b200kge_train_1vsall_backward (dot family, TransE L1/L2, RotatE L1 for the
- * backward; the forward also takes the other norms).  Workspace (either call, with or without dropout):
- * b200kge_train_1vsall_reciprocal_workspace_bytes. */
-size_t b200kge_train_1vsall_reciprocal_workspace_bytes(int model, int64_t n, int64_t E, int32_t D);
-int b200kge_train_1vsall_reciprocal_forward(int model, float l_norm, int precision, const b200kge_rows_t* ent,
-                                            const b200kge_rows_t* rel, int64_t num_relations, const int64_t* triples,
-                                            int64_t n, int loss_kind, float offset, const b200kge_dropout_t* drop,
-                                            float* loss_out, void* workspace, size_t workspace_bytes,
-                                            b200kge_stream_t stream);
-int b200kge_train_1vsall_reciprocal_backward(int model, float l_norm, const b200kge_rows_t* ent,
-                                             const b200kge_rows_t* rel, int64_t num_relations, const int64_t* triples,
-                                             int64_t n, int loss_kind, float offset, const b200kge_dropout_t* drop,
-                                             float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
-                                             size_t workspace_bytes, b200kge_stream_t stream);
 
 /* ---- Embedding dropout of the negative-sampling training step ------------------------------------------------------
  * Per slot (0 = S or 2 = O; the P slot is not served) and sub-batch, train_negative_sampling.py:139-148 makes six draws,
@@ -635,19 +559,29 @@ int b200kge_ns_score_dropout(int model, float l_norm, const b200kge_rows_t* ent,
                              const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
                              const b200kge_dropout_t* drop, float* out, int64_t ldo, b200kge_stream_t stream);
 
-/* Backward of b200kge_ns_score_dropout under the same key: grad_scores [n, 1 + K] (row stride ldg) holds dL/dz already
- * scaled (the grad_out of b200kge_ns_loss), so every loss trains through it.  The masks are regenerated, the gradients of
- * the masked operands are masked and scaled again and ADDED into d_ent [E, lde] / d_rel [R, ldr].  Same coverage as the
- * forward; B200KGE_NS_BATCH (not RESCAL) also needs D <= 1024.  The positive column and `triple` run row-wise (one warp
- * per triple); the `batch` negatives run ns_kernel / ns_backward_kernel with a mask policy (q folded once per row from
- * the masked fixed rows, sampled rows masked by id, the fixed rows' gradient reduced per row).
- * workspace: b200kge_ns_dropout_workspace_bytes(model, n, K, D) bytes (K is not used). */
-size_t b200kge_ns_dropout_workspace_bytes(int model, int64_t n, int64_t K, int32_t D);
-int b200kge_ns_backward_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
-                                const b200kge_dropout_t* drop, const float* grad_scores, int64_t ldg, float* d_ent,
-                                int64_t lde, float* d_rel, int64_t ldr, void* workspace, size_t workspace_bytes,
-                                b200kge_stream_t stream);
+/* Backward of one slot of a negative-sampling batch (kge/job/train_negative_sampling.py:113-164): the [n, 1+K] block of
+ * the slot (column 0 = the positive triple, label 1; columns 1.. = the sampled ids neg [n,K], label 0).  ADDS into
+ * d_ent [E, lde] and d_rel [R, ldr] (zero them before the first slot).  slot 0 (S) or 2 (O); TransE with l_norm 1 or 2,
+ * RotatE with l_norm 1, and the dot family.  Where dL/dz comes from:
+ *   grad_scores == NULL: BCE with `offset`, the loss summed and divided by batch_size; the kernel computes the gradient.
+ *   grad_scores [n, 1+K] (row stride ldg): dL/dz already scaled (e.g. the grad_out of b200kge_ns_loss with
+ *     scale = 1 / batch_size); offset and batch_size are not used.  The fold, per-column walk, scatter and unfold are
+ *     the BCE form's; only the per-column gradient is read instead of computed — so every loss of b200kge_ns_loss
+ *     trains through the same kernel (loss.backward() at train_negative_sampling.py:164).
+ *   drop != NULL: the backward of b200kge_ns_score_dropout under the same key and `impl` (impl is ignored without
+ *     drop); grad_scores is required (else B200KGE_ERR_INVALID).  The masks are regenerated, the gradients of the
+ *     masked operands are masked and scaled again and added.  Same coverage as that forward; B200KGE_NS_BATCH (not
+ *     RESCAL) also needs D <= 1024.  The positive column and `triple` run row-wise (one warp per triple); the `batch`
+ *     negatives run ns_kernel / ns_backward_kernel with a mask policy (q folded once per row from the masked fixed rows,
+ *     sampled rows masked by id, the fixed rows' gradient reduced per row).
+ * workspace: b200kge_ns_backward_workspace_bytes(model, n, K, D, drop != NULL) bytes (K is not used; without dropout
+ * n * round_up(K_folded, 32) floats are used). */
+size_t b200kge_ns_backward_workspace_bytes(int model, int64_t n, int64_t K, int32_t D, int dropout);
+int b200kge_ns_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                        const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
+                        const b200kge_dropout_t* drop, const float* grad_scores, int64_t ldg, float offset,
+                        int64_t batch_size, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
+                        size_t workspace_bytes, b200kge_stream_t stream);
 
 #ifdef __cplusplus
 }

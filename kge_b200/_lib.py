@@ -82,9 +82,13 @@ SIGNATURES = {
                                                   C.c_void_p]),
     "b200kge_filter_index_build": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
                                              C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
-    "b200kge_train_1vsall_forward": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_void_p,
-                                               C.c_int64, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
+    "b200kge_train_1vsall_forward": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_int64, C.c_void_p,
+                                               C.c_int64, C.c_int, C.c_float, _DP, C.c_void_p, C.c_void_p,
                                                C.c_size_t, C.c_void_p]),
+    "b200kge_train_1vsall_backward": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_int64, C.c_void_p, C.c_int64,
+                                                C.c_int, C.c_float, _DP, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                                C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_train_1vsall_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32, C.c_int]),
     "b200kge_train_1vsall_forward_host": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_void_p,
                                                     C.c_int64, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
                                                     C.c_size_t, C.c_void_p]),
@@ -98,86 +102,39 @@ SIGNATURES = {
     "b200kge_gemm_nt_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64]),
     "b200kge_gemm_nt": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                     C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
-    "b200kge_train_1vsall_backward_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32]),
-    "b200kge_train_1vsall_backward": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int64, C.c_int, C.c_float,
-                                                  C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
-                                                  C.c_size_t, C.c_void_p]),
     "b200kge_score_1vsN_backward_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32]),
     "b200kge_score_1vsN_backward": (C.c_int, [C.c_int, C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                               C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                                               C.c_size_t, C.c_void_p]),
-    "b200kge_score_1vsN_loss_csr_backward": (C.c_int, [C.c_int, C.c_int, _RP, _RP, C.c_void_p, C.c_void_p, C.c_int64,
-                                                       C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_float, C.c_int64,
-                                                       C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t,
-                                                       C.c_void_p]),
-    "b200kge_score_1vsN_loss_csr_backward_norm": (C.c_int, [C.c_int, C.c_int, C.c_float, _RP, _RP, C.c_void_p,
-                                                            C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float,
-                                                            C.c_int, C.c_float, C.c_int64, C.c_void_p, C.c_int64,
-                                                            C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_score_1vsN_loss_csr_backward": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_float, _RP, _RP, C.c_void_p,
+                                                       C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float,
+                                                       C.c_int, C.c_float, C.c_int64, _DP, C.c_void_p, C.c_int64,
+                                                       C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_score_1vsN_loss_csr_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32, C.c_int64]),
     "b200kge_score_1vsN_loss_csr": (C.c_int, [C.c_int, C.c_int, C.c_float, C.c_int, _RP, _RP, _RP, C.c_int64,
                                                 C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_int, C.c_float,
                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_ns_backward_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32, C.c_int]),
     "b200kge_ns_backward": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
-                                        C.c_int64, C.c_float, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
-                                        C.c_void_p, C.c_size_t, C.c_void_p]),
+                                      C.c_int64, C.c_int, _DP, C.c_void_p, C.c_int64, C.c_float, C.c_int64, C.c_void_p,
+                                      C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_ns_loss_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "b200kge_ns_loss": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_float, C.c_float,
                                   C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t,
                                   C.c_void_p]),
-    "b200kge_ns_backward_grad": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
-                                           C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
-                                           C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_lookup_penalty": (C.c_int, [_RP, C.c_void_p, C.c_float, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
                                            C.c_size_t, C.c_void_p]),
     "b200kge_normalize_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_float, C.c_void_p]),
     "b200kge_dropout_mask": (C.c_int, [C.c_float, C.c_uint64, C.c_uint64, C.c_int, C.c_int64, C.c_int64, C.c_int32,
                                        C.c_void_p, C.c_void_p]),
-    "b200kge_train_1vsall_dropout_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32]),
-    "b200kge_train_1vsall_forward_dropout": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_void_p, C.c_int64,
-                                                       C.c_int, C.c_float, _DP, C.c_void_p, C.c_void_p, C.c_size_t,
-                                                       C.c_void_p]),
-    "b200kge_train_1vsall_backward_dropout": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int64, C.c_int,
-                                                        C.c_float, _DP, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
-                                                        C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_score_1vsN_loss_csr_dropout_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32,
                                                                          C.c_int64]),
-    "b200kge_score_1vsN_loss_csr_dropout": (C.c_int, [C.c_int, C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_void_p,
-                                                      C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
-                                                      C.c_float, C.c_int, C.c_float, _DP, C.c_void_p, C.c_void_p,
-                                                      C.c_void_p, C.c_size_t, C.c_void_p]),
-    "b200kge_score_1vsN_loss_csr_backward_dropout": (C.c_int, [C.c_int, C.c_int, _RP, _RP, C.c_void_p, C.c_void_p,
-                                                               C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.c_int,
-                                                               C.c_float, C.c_int64, _DP, C.c_void_p, C.c_int64,
-                                                               C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t,
-                                                               C.c_void_p]),
-    "b200kge_score_1vsN_loss_csr_dropout_dir": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _RP, _RP,
-                                                          C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
-                                                          C.c_int64, C.c_float, C.c_int, C.c_float, _DP, C.c_void_p,
-                                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
-    "b200kge_score_1vsN_loss_csr_backward_dropout_dir": (C.c_int, [C.c_int, C.c_int, C.c_int, _RP, _RP, C.c_void_p,
-                                                                   C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
-                                                                   C.c_float, C.c_int, C.c_float, C.c_int64, _DP,
-                                                                   C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
-                                                                   C.c_void_p, C.c_size_t, C.c_void_p]),
-    "b200kge_score_1vsN_loss_csr_backward_dropout_norm": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_float, _RP, _RP,
-                                                                    C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
-                                                                    C.c_void_p, C.c_float, C.c_int, C.c_float, C.c_int64,
-                                                                    _DP, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
-                                                                    C.c_void_p, C.c_size_t, C.c_void_p]),
-    "b200kge_train_1vsall_reciprocal_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32]),
-    "b200kge_train_1vsall_reciprocal_forward": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_int64, C.c_void_p,
-                                                          C.c_int64, C.c_int, C.c_float, _DP, C.c_void_p, C.c_void_p,
-                                                          C.c_size_t, C.c_void_p]),
-    "b200kge_train_1vsall_reciprocal_backward": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_int64, C.c_void_p,
-                                                           C.c_int64, C.c_int, C.c_float, _DP, C.c_void_p, C.c_int64,
-                                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_score_1vsN_loss_csr_dropout": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _RP, _RP,
+                                                      C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                                      C.c_int64, C.c_float, C.c_int, C.c_float, _DP, C.c_void_p,
+                                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_ns_score_dropout": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
                                            C.c_int64, C.c_int, _DP, C.c_void_p, C.c_int64, C.c_void_p]),
-    "b200kge_ns_dropout_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32]),
-    "b200kge_ns_backward_dropout": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
-                                              C.c_int64, C.c_int, _DP, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
-                                              C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 #: negative-sampling scoring implementations of the dropout entry points (B200KGE_NS_*); "all" draws like "batch"

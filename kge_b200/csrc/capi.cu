@@ -685,17 +685,13 @@ int b200kge_sample_uniform_filtered(uint64_t seed, uint64_t offset, int64_t voca
                                         (cudaStream_t)stream);
 }
 
-// num_rel > 0: the reciprocal-relations step (rows n..2n are the sp_ queries (o, p + num_rel), label s)
-static int train_1vsall_forward_impl(int model, float l_norm, int precision,
-                                     const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                     const int64_t* triples, int64_t n, int loss_kind, float offset,
-                                     float* loss_out, void* workspace, size_t workspace_bytes,
-                                     b200kge_stream_t stream, int64_t num_rel) {
-  if (!triples || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
-  if ((rc = check_loss_kind(loss_kind))) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (n <= 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
+// The 1vsAll step without dropout on validated arguments, n > 0.  num_rel > 0: the reciprocal-relations step (rows
+// n..2n are the sp_ queries (o, p + num_rel), label s)
+static int train_1vsall_forward_impl(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                                     const b200kge_rows_t* rel, const int64_t* triples, int64_t n, int loss_kind,
+                                     float offset, float* loss_out, void* workspace, size_t workspace_bytes,
+                                     cudaStream_t st, int64_t num_rel) {
+  int rc;
   Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
   Rows E = to_rows(ent), R = to_rows(rel);
   const int epi = (loss_kind == B200KGE_LOSS_BCE) ? EPI_BCE : EPI_KL;
@@ -784,15 +780,6 @@ static int train_1vsall_forward_impl(int model, float l_norm, int precision,
   return 0;
 }
 
-int b200kge_train_1vsall_forward(int model, float l_norm, int precision,
-                                 const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                 const int64_t* triples, int64_t n, int loss_kind, float offset,
-                                 float* loss_out, void* workspace, size_t workspace_bytes,
-                                 b200kge_stream_t stream) {
-  return train_1vsall_forward_impl(model, l_norm, precision, ent, rel, triples, n, loss_kind, offset, loss_out,
-                                   workspace, workspace_bytes, stream, 0);
-}
-
 int b200kge_train_1vsall_forward_host(int model, float l_norm, int precision,
                                       const b200kge_rows_t* ent, const b200kge_rows_t* rel,
                                       const int64_t* triples_host, int64_t n, int loss_kind,
@@ -808,8 +795,8 @@ int b200kge_train_1vsall_forward_host(int model, float l_norm, int precision,
   // triples.to(device)   train_1vsAll.py:59
   B2K_CUDA(cudaMemcpyAsync(tri, triples_host, (size_t)n * 3 * 8, cudaMemcpyHostToDevice, st));
   size_t used = (ws.off + 255) & ~size_t(255);
-  int rc = b200kge_train_1vsall_forward(model, l_norm, precision, ent, rel, tri, n, loss_kind, offset, loss_dev,
-                                        ws.base + used, workspace_bytes - used, stream);
+  int rc = b200kge_train_1vsall_forward(model, l_norm, precision, ent, rel, 0, tri, n, loss_kind, offset, nullptr,
+                                        loss_dev, ws.base + used, workspace_bytes - used, stream);
   if (rc) return rc;
   // .item()   train_1vsAll.py:66,77
   B2K_CUDA(cudaMemcpyAsync(loss_host, loss_dev, 4, cudaMemcpyDeviceToHost, st));
@@ -1002,7 +989,8 @@ int b200kge_gemm_nt(const float* A, int64_t lda, const float* B, int64_t ldb, in
   return gemm_planes(SA, SB, C, ldc, st);
 }
 
-size_t b200kge_train_1vsall_backward_workspace_bytes(int model, int64_t n, int64_t E, int32_t D) {
+// the workspace of train_1vsall_backward_impl
+static size_t train_1vsall_backward_bytes(int model, int64_t n, int64_t E, int32_t D) {
   const int64_t K = (model == B200KGE_CP) ? D / 2 : D;
   const int64_t nq = 2 * n, ldq = round_up(K, 32);
   if (model == B200KGE_TRANSE || model == B200KGE_ROTATE)   // Q, dQ, labels, z, G, G^T, z^T, row stats + scorer workspace
@@ -1011,16 +999,12 @@ size_t b200kge_train_1vsall_backward_workspace_bytes(int model, int64_t n, int64
   return (size_t)nq * ldq * 4 + (size_t)n * 5 * 8 + 4096 + backward_block_bytes(nq, E, K, ldq);
 }
 
-// num_rel > 0: the backward of the reciprocal-relations step (train_1vsall_forward_impl)
+// The backward of train_1vsall_forward_impl on validated arguments.  num_rel > 0: the reciprocal-relations step
 static int train_1vsall_backward_impl(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
                                       const int64_t* triples, int64_t n, int loss_kind, float offset, float* d_ent,
                                       int64_t lde, float* d_rel, int64_t ldr, void* workspace, size_t workspace_bytes,
-                                      b200kge_stream_t stream, int64_t num_rel) {
-  if (!triples || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
-  if ((rc = check_loss_kind(loss_kind))) return rc;
-  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
+                                      cudaStream_t st, int64_t num_rel) {
+  int rc;
   Rows E = to_rows(ent), R = to_rows(rel);
   B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
   if (n <= 0) { B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st)); return 0; }
@@ -1084,15 +1068,6 @@ static int train_1vsall_backward_impl(int model, float l_norm, const b200kge_row
     if ((rc = launch_unfold(model, E, R, triples, n, dir, dQ2 + (size_t)dir * n * ldq, ldq, d_ent, lde, d_rel, ldr, st))) return rc;
   return 0;
 }
-
-int b200kge_train_1vsall_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                    const int64_t* triples, int64_t n, int loss_kind, float offset, float* d_ent,
-                                    int64_t lde, float* d_rel, int64_t ldr, void* workspace, size_t workspace_bytes,
-                                    b200kge_stream_t stream) {
-  return train_1vsall_backward_impl(model, l_norm, ent, rel, triples, n, loss_kind, offset, d_ent, lde, d_rel, ldr,
-                                    workspace, workspace_bytes, stream, 0);
-}
-
 
 size_t b200kge_score_1vsN_backward_workspace_bytes(int model, int64_t n, int64_t E, int32_t D) {
   const int64_t K = (model == B200KGE_CP) ? D / 2 : D;
@@ -1162,58 +1137,6 @@ int b200kge_score_1vsN_backward(int model, int combine, float l_norm, const b200
   return launch_unfold(model, E, R, tri, n, combine, dQ, ldq, d_ent, lde, d_rel, ldr, st);
 }
 
-int b200kge_score_1vsN_loss_csr_backward_norm(int model, int combine, float l_norm, const b200kge_rows_t* ent,
-                                              const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx,
-                                              int64_t n, const int64_t* csr_off, const int64_t* csr_col,
-                                              float label_smoothing, int loss_kind, float offset, int64_t batch_size,
-                                              float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
-                                              size_t workspace_bytes, b200kge_stream_t stream) {
-  if (!q_idx || !p_idx || !csr_off || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
-  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
-  const bool distance = (model == B200KGE_TRANSE || model == B200KGE_ROTATE);
-  Folded f = folded_problem(model, combine, ent->dim, distance ? l_norm : 1.0f);     // the dot family folds with l_norm 1
-  if (distance && (rc = check_distance_pair(f.pair_op))) return rc;
-  if ((rc = check_loss_kind(loss_kind))) return rc;
-  if (batch_size <= 0 || !(label_smoothing >= 0.f && label_smoothing < 1.f)) { set_error("bad batch_size / label_smoothing"); return B200KGE_ERR_INVALID; }
-  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  Rows E = to_rows(ent), R = to_rows(rel);
-  B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
-  B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st));
-  if (n <= 0) return 0;
-  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
-  const int64_t ldq = round_up(f.K, 32);
-  float* Q = (float*)ws.take((size_t)n * ldq * 4);
-  float* dQ = (float*)ws.take((size_t)n * ldq * 4);
-  int64_t* tri = (int64_t*)ws.take((size_t)n * 3 * 8);
-  if (!Q || !dQ || !tri) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
-  pack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(q_idx, p_idx, n, combine, tri);
-  B2K_LAUNCH_CHECK("pack_triples_kernel");
-  Rows A = E; A.idx = q_idx; A.rows = n;
-  Rows Pr = R; Pr.idx = p_idx; Pr.rows = n;
-  if ((rc = launch_fold_queries(model, combine, A, Pr, n, 0, Q, ldq, st))) return rc;
-  const GradSpec g = csr_grad(q_idx, csr_off, csr_col, label_smoothing, E.rows, batch_size, loss_kind, offset);
-  if (distance) {
-    Block B{model, combine, &A, nullptr, &Pr, &E, n};
-    B.Qpre = Q;
-    if ((rc = distance_backward(B, l_norm, g, dQ, d_ent, lde, ws, st))) return rc;
-    return launch_unfold_distance(model, E, R, tri, n, combine, dQ, ldq, d_ent, lde, d_rel, ldr, st);
-  }
-  if ((rc = backward_block(model, E, R, n, combine, false, Q, ldq, f.col_off, f.K, g, d_ent, lde, dQ, ws, st))) return rc;
-  return launch_unfold(model, E, R, tri, n, combine, dQ, ldq, d_ent, lde, d_rel, ldr, st);
-}
-
-int b200kge_score_1vsN_loss_csr_backward(int model, int combine, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                         const int64_t* q_idx, const int64_t* p_idx, int64_t n, const int64_t* csr_off,
-                                         const int64_t* csr_col, float label_smoothing, int loss_kind, float offset,
-                                         int64_t batch_size, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                                         void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
-  return b200kge_score_1vsN_loss_csr_backward_norm(model, combine, 1.0f, ent, rel, q_idx, p_idx, n, csr_off, csr_col,
-                                                   label_smoothing, loss_kind, offset, batch_size, d_ent, lde, d_rel,
-                                                   ldr, workspace, workspace_bytes, stream);
-}
-
 int b200kge_lookup_penalty(const b200kge_rows_t* rows, const float* counts, float p, int complex_abs, float scale,
                              float* out, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
   if (!rows || !out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
@@ -1228,42 +1151,6 @@ int b200kge_normalize_rows(float* weight, int64_t ld, int64_t rows, int32_t dim,
   return launch_normalize_rows(weight, ld, rows, dim, p, (cudaStream_t)stream);
 }
 
-
-int b200kge_ns_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                          const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, float offset,
-                          int64_t batch_size, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
-                          size_t workspace_bytes, b200kge_stream_t stream) {
-  if (!triples || (!neg && n * K > 0) || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
-  if (batch_size <= 0) { set_error("batch_size must be positive"); return B200KGE_ERR_INVALID; }
-  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
-  Rows E = to_rows(ent), R = to_rows(rel);
-  Folded f = folded_problem(model, B200KGE_SP_, E.dim, l_norm);
-  const int64_t ldq = round_up(f.K, 32);
-  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
-  float* dQ = (float*)ws.take((size_t)n * ldq * 4);
-  if (!dQ && n > 0) { set_error("workspace too small (need n * round_up(K,32) floats)"); return B200KGE_ERR_WORKSPACE; }
-  return launch_ns_backward(model, l_norm, E, R, triples, slot, neg, n, K, offset, 1.0f / (float)batch_size, nullptr, 0,
-                            d_ent, lde, d_rel, ldr, dQ, ldq, (cudaStream_t)stream);
-}
-
-int b200kge_ns_backward_grad(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                             const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K,
-                             const float* grad_scores, int64_t ldg, float* d_ent, int64_t lde, float* d_rel,
-                             int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
-  if (!triples || (!neg && n * K > 0) || (!grad_scores && n > 0) || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
-  if (ldg < K + 1) { set_error("grad_scores is narrower than the 1 + K columns of the block"); return B200KGE_ERR_INVALID; }
-  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
-  Rows E = to_rows(ent), R = to_rows(rel);
-  Folded f = folded_problem(model, B200KGE_SP_, E.dim, l_norm);
-  const int64_t ldq = round_up(f.K, 32);
-  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
-  float* dQ = (float*)ws.take((size_t)n * ldq * 4);
-  if (!dQ && n > 0) { set_error("workspace too small (need n * round_up(K,32) floats)"); return B200KGE_ERR_WORKSPACE; }
-  return launch_ns_backward(model, l_norm, E, R, triples, slot, neg, n, K, 0.f, 1.f, grad_scores, ldg, d_ent, lde,
-                            d_rel, ldr, dQ, ldq, (cudaStream_t)stream);
-}
 
 size_t b200kge_ns_loss_workspace_bytes(int64_t n) { return (size_t)n * 2 * 4 + 256 + 1024; }
 
@@ -1530,26 +1417,17 @@ int b200kge_dropout_mask(float p, uint64_t seed, uint64_t call, int mask_stream,
   return launch_dropout_mask(drop_mask(p, seed, call, mask_stream, row_base), rows, dim, out, (cudaStream_t)stream);
 }
 
-size_t b200kge_train_1vsall_dropout_workspace_bytes(int model, int64_t n, int64_t E, int32_t D) {
-  size_t dir = b200kge_score_1vsN_backward_workspace_bytes(model, n, E, D) + (size_t)n * 2 * 4 + 1024;
-  const size_t fwd = b200kge_workspace_bytes(model, n, E, D, 0);
-  return masked_bytes(model, n, E, D) + (dir > fwd ? dir : fwd);
-}
-
-// The 1vsAll step under embedding dropout; the masks of direction dir are drawn on dir's streams.  num_rel > 0: the
-// reciprocal-relations step (reciprocal_relations_model.py:85-92): both directions are sp_ queries against the table;
-// the second one, (o, p + R) labelled s, is score_po and draws its masks on the _po streams in the reference's call
-// order (embed_all: B200KGE_DROP_PO_TABLE, embed(p + R): B200KGE_DROP_PO_REL, embed(o): B200KGE_DROP_PO_ENT).
+// The 1vsAll step under embedding dropout on validated arguments, n > 0; the masks of direction dir are drawn on dir's
+// streams.  num_rel > 0: the reciprocal-relations step (reciprocal_relations_model.py:85-92): both directions are sp_
+// queries against the table; the second one, (o, p + R) labelled s, is score_po and draws its masks on the _po streams
+// in the reference's call order (embed_all: B200KGE_DROP_PO_TABLE, embed(p + R): B200KGE_DROP_PO_REL, embed(o):
+// B200KGE_DROP_PO_ENT).
 static int train_1vsall_forward_dropout_impl(int model, float l_norm, int precision, const b200kge_rows_t* ent,
                                              const b200kge_rows_t* rel, const int64_t* triples, int64_t n,
                                              int loss_kind, float offset, const b200kge_dropout_t* drop,
                                              float* loss_out, void* workspace, size_t workspace_bytes,
                                              cudaStream_t st, int64_t num_rel) {
-  if (!triples || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
-  if ((rc = check_loss_kind(loss_kind))) return rc;
-  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
-  if (n <= 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
+  int rc;
   Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
   Rows E = to_rows(ent), R = to_rows(rel);
   int64_t* sidx = (int64_t*)ws.take((size_t)n * 8);
@@ -1561,7 +1439,7 @@ static int train_1vsall_forward_dropout_impl(int model, float l_norm, int precis
   MaskedOps o;
   if (!sidx || !pidx || !oidx || (num_rel > 0 && !pinv) || !lab || !dir_loss ||
       !take_masked(ws, n, E.rows, E.dim, R.dim, o)) {
-    set_error("workspace too small (see b200kge_train_1vsall_%s_workspace_bytes)", num_rel > 0 ? "reciprocal" : "dropout");
+    set_error("workspace too small (see b200kge_train_1vsall_workspace_bytes)");
     return B200KGE_ERR_WORKSPACE;
   }
   Rows S, O, P;
@@ -1584,17 +1462,13 @@ static int train_1vsall_forward_dropout_impl(int model, float l_norm, int precis
   return launch_rows_sum(dir_loss, 2, 1.0f / (float)n, loss_out, st);    // (loss_sp + loss_po) / n
 }
 
-// the backward of train_1vsall_forward_dropout_impl
+// the backward of train_1vsall_forward_dropout_impl, on validated arguments
 static int train_1vsall_backward_dropout_impl(int model, float l_norm, const b200kge_rows_t* ent,
                                               const b200kge_rows_t* rel, const int64_t* triples, int64_t n,
                                               int loss_kind, float offset, const b200kge_dropout_t* drop, float* d_ent,
                                               int64_t lde, float* d_rel, int64_t ldr, void* workspace,
                                               size_t workspace_bytes, cudaStream_t st, int64_t num_rel) {
-  if (!triples || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
-  if ((rc = check_loss_kind(loss_kind))) return rc;
-  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
-  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
+  int rc;
   const Folded f = folded_problem(model, B200KGE_SP_, ent->dim, l_norm);
   if (f.pair_op != PAIR_DOT && (rc = check_distance_pair(f.pair_op))) return rc;
   Rows E = to_rows(ent), R = to_rows(rel);
@@ -1610,7 +1484,7 @@ static int train_1vsall_backward_dropout_impl(int model, float l_norm, const b20
   BackBufs b;
   if (!sidx || !pidx || !oidx || (num_rel > 0 && !pinv) || !lab ||
       !take_back(ws, n, E.rows, E.dim, R.dim, round_up(f.K, 32), b)) {
-    set_error("workspace too small (see b200kge_train_1vsall_%s_workspace_bytes)", num_rel > 0 ? "reciprocal" : "dropout");
+    set_error("workspace too small (see b200kge_train_1vsall_workspace_bytes)");
     return B200KGE_ERR_WORKSPACE;
   }
   Rows S, O, P;
@@ -1632,56 +1506,54 @@ static int train_1vsall_backward_dropout_impl(int model, float l_norm, const b20
   return 0;
 }
 
-int b200kge_train_1vsall_forward_dropout(int model, float l_norm, int precision, const b200kge_rows_t* ent,
-                                         const b200kge_rows_t* rel, const int64_t* triples, int64_t n, int loss_kind,
-                                         float offset, const b200kge_dropout_t* drop, float* loss_out, void* workspace,
-                                         size_t workspace_bytes, b200kge_stream_t stream) {
-  return train_1vsall_forward_dropout_impl(model, l_norm, precision, ent, rel, triples, n, loss_kind, offset, drop,
-                                           loss_out, workspace, workspace_bytes, (cudaStream_t)stream, 0);
-}
-
-int b200kge_train_1vsall_backward_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                          const int64_t* triples, int64_t n, int loss_kind, float offset,
-                                          const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
-                                          int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
-  return train_1vsall_backward_dropout_impl(model, l_norm, ent, rel, triples, n, loss_kind, offset, drop, d_ent, lde,
-                                            d_rel, ldr, workspace, workspace_bytes, (cudaStream_t)stream, 0);
-}
-
-size_t b200kge_train_1vsall_reciprocal_workspace_bytes(int model, int64_t n, int64_t E, int32_t D) {
-  const size_t fwd = b200kge_workspace_bytes(model, n, E, D, 0);
-  const size_t bwd = b200kge_train_1vsall_backward_workspace_bytes(model, n, E, D);
-  const size_t drop = b200kge_train_1vsall_dropout_workspace_bytes(model, n, E, D) + (size_t)n * 8 + 256;
-  const size_t m = fwd > bwd ? fwd : bwd;
-  return m > drop ? m : drop;
-}
-
-int b200kge_train_1vsall_reciprocal_forward(int model, float l_norm, int precision, const b200kge_rows_t* ent,
-                                            const b200kge_rows_t* rel, int64_t num_relations, const int64_t* triples,
-                                            int64_t n, int loss_kind, float offset, const b200kge_dropout_t* drop,
-                                            float* loss_out, void* workspace, size_t workspace_bytes,
-                                            b200kge_stream_t stream) {
+// rel holds the 2 * num_rel rows of a reciprocal-relations base model; num_rel = 0 is the plain model
+int b200kge_train_1vsall_forward(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                                 const b200kge_rows_t* rel, int64_t num_relations, const int64_t* triples, int64_t n,
+                                 int loss_kind, float offset, const b200kge_dropout_t* drop, float* loss_out,
+                                 void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
   if (!ent || !rel || !triples || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  int rc = check_reciprocal(rel, num_relations); if (rc) return rc;
-  if (!drop)
-    return train_1vsall_forward_impl(model, l_norm, precision, ent, rel, triples, n, loss_kind, offset, loss_out,
-                                     workspace, workspace_bytes, stream, num_relations);
-  return train_1vsall_forward_dropout_impl(model, l_norm, precision, ent, rel, triples, n, loss_kind, offset, drop,
-                                           loss_out, workspace, workspace_bytes, (cudaStream_t)stream, num_relations);
+  int rc;
+  if (num_relations != 0 && (rc = check_reciprocal(rel, num_relations))) return rc;
+  if ((rc = check_tables(model, l_norm, ent, rel))) return rc;
+  if ((rc = check_loss_kind(loss_kind))) return rc;
+  if (drop && (rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n <= 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
+  if (drop)
+    return train_1vsall_forward_dropout_impl(model, l_norm, precision, ent, rel, triples, n, loss_kind, offset, drop,
+                                             loss_out, workspace, workspace_bytes, st, num_relations);
+  return train_1vsall_forward_impl(model, l_norm, precision, ent, rel, triples, n, loss_kind, offset, loss_out,
+                                   workspace, workspace_bytes, st, num_relations);
 }
 
-int b200kge_train_1vsall_reciprocal_backward(int model, float l_norm, const b200kge_rows_t* ent,
-                                             const b200kge_rows_t* rel, int64_t num_relations, const int64_t* triples,
-                                             int64_t n, int loss_kind, float offset, const b200kge_dropout_t* drop,
-                                             float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
-                                             size_t workspace_bytes, b200kge_stream_t stream) {
+int b200kge_train_1vsall_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                  int64_t num_relations, const int64_t* triples, int64_t n, int loss_kind, float offset,
+                                  const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
+                                  void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
   if (!ent || !rel || !triples || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  int rc = check_reciprocal(rel, num_relations); if (rc) return rc;
-  if (!drop)
-    return train_1vsall_backward_impl(model, l_norm, ent, rel, triples, n, loss_kind, offset, d_ent, lde, d_rel, ldr,
-                                      workspace, workspace_bytes, stream, num_relations);
-  return train_1vsall_backward_dropout_impl(model, l_norm, ent, rel, triples, n, loss_kind, offset, drop, d_ent, lde,
-                                            d_rel, ldr, workspace, workspace_bytes, (cudaStream_t)stream, num_relations);
+  int rc;
+  if (num_relations != 0 && (rc = check_reciprocal(rel, num_relations))) return rc;
+  if ((rc = check_tables(model, l_norm, ent, rel))) return rc;
+  if ((rc = check_loss_kind(loss_kind))) return rc;
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
+  if (drop && (rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (drop)
+    return train_1vsall_backward_dropout_impl(model, l_norm, ent, rel, triples, n, loss_kind, offset, drop, d_ent, lde,
+                                              d_rel, ldr, workspace, workspace_bytes, st, num_relations);
+  return train_1vsall_backward_impl(model, l_norm, ent, rel, triples, n, loss_kind, offset, d_ent, lde, d_rel, ldr,
+                                    workspace, workspace_bytes, st, num_relations);
+}
+
+size_t b200kge_train_1vsall_workspace_bytes(int model, int64_t n, int64_t E, int32_t D, int dropout) {
+  const size_t fwd = b200kge_workspace_bytes(model, n, E, D, 0);
+  if (dropout) {
+    // the masked copies and per-direction buffers, the larger of one direction's forward and backward, the p + R index
+    const size_t dir = b200kge_score_1vsN_backward_workspace_bytes(model, n, E, D) + (size_t)n * 2 * 4 + 1024;
+    return masked_bytes(model, n, E, D) + (dir > fwd ? dir : fwd) + (size_t)n * 8 + 256;
+  }
+  const size_t bwd = train_1vsall_backward_bytes(model, n, E, D);
+  return fwd > bwd ? fwd : bwd;
 }
 
 size_t b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(int model, int64_t n, int64_t E, int32_t D, int64_t nnz) {
@@ -1690,13 +1562,12 @@ size_t b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(int model, int64_t n,
   return masked_bytes(model, n, E, D) + (fwd > bwd ? fwd : bwd);
 }
 
-int b200kge_score_1vsN_loss_csr_dropout_dir(int model, int combine, int mask_dir, float l_norm, int precision,
-                                            const b200kge_rows_t* ent, const b200kge_rows_t* rel, const int64_t* q_idx,
-                                            const int64_t* p_idx, int64_t n, const int64_t* csr_off,
-                                            const int64_t* csr_col, int64_t nnz, float label_smoothing, int loss_kind,
-                                            float offset, const b200kge_dropout_t* drop, float* loss_out,
-                                            float* row_loss_out, void* workspace, size_t workspace_bytes,
-                                            b200kge_stream_t stream) {
+int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, int mask_dir, float l_norm, int precision,
+                                        const b200kge_rows_t* ent, const b200kge_rows_t* rel, const int64_t* q_idx,
+                                        const int64_t* p_idx, int64_t n, const int64_t* csr_off, const int64_t* csr_col,
+                                        int64_t nnz, float label_smoothing, int loss_kind, float offset,
+                                        const b200kge_dropout_t* drop, float* loss_out, float* row_loss_out,
+                                        void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
   if ((!q_idx && n > 0) || (!p_idx && n > 0) || !loss_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
   if (mask_dir != B200KGE_SP_ && mask_dir != B200KGE__PO) { set_error("bad mask direction %d", mask_dir); return B200KGE_ERR_INVALID; }
@@ -1722,28 +1593,15 @@ int b200kge_score_1vsN_loss_csr_dropout_dir(int model, int combine, int mask_dir
                                      stream);
 }
 
-int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, float l_norm, int precision, const b200kge_rows_t* ent,
-                                        const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx, int64_t n,
-                                        const int64_t* csr_off, const int64_t* csr_col, int64_t nnz,
-                                        float label_smoothing, int loss_kind, float offset,
-                                        const b200kge_dropout_t* drop, float* loss_out, float* row_loss_out,
-                                        void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
-  return b200kge_score_1vsN_loss_csr_dropout_dir(model, combine, combine, l_norm, precision, ent, rel, q_idx, p_idx, n,
-                                                 csr_off, csr_col, nnz, label_smoothing, loss_kind, offset, drop,
-                                                 loss_out, row_loss_out, workspace, workspace_bytes, stream);
-}
-
-int b200kge_score_1vsN_loss_csr_backward_dropout_norm(int model, int combine, int mask_dir, float l_norm,
-                                                      const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                                      const int64_t* q_idx, const int64_t* p_idx, int64_t n,
-                                                      const int64_t* csr_off, const int64_t* csr_col,
-                                                      float label_smoothing, int loss_kind, float offset,
-                                                      int64_t batch_size, const b200kge_dropout_t* drop, float* d_ent,
-                                                      int64_t lde, float* d_rel, int64_t ldr, void* workspace,
-                                                      size_t workspace_bytes, b200kge_stream_t stream) {
+int b200kge_score_1vsN_loss_csr_backward(int model, int combine, int mask_dir, float l_norm, const b200kge_rows_t* ent,
+                                         const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx,
+                                         int64_t n, const int64_t* csr_off, const int64_t* csr_col,
+                                         float label_smoothing, int loss_kind, float offset, int64_t batch_size,
+                                         const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
+                                         int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
   if (!q_idx || !p_idx || !csr_off || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
   if (combine != B200KGE_SP_ && combine != B200KGE__PO) { set_error("cannot handle combine=%d", combine); return B200KGE_ERR_INVALID; }
-  if (mask_dir != B200KGE_SP_ && mask_dir != B200KGE__PO) { set_error("bad mask direction %d", mask_dir); return B200KGE_ERR_INVALID; }
+  if (drop && mask_dir != B200KGE_SP_ && mask_dir != B200KGE__PO) { set_error("bad mask direction %d", mask_dir); return B200KGE_ERR_INVALID; }
   int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
   const bool distance = (model == B200KGE_TRANSE || model == B200KGE_ROTATE);
   if (!distance) l_norm = 1.0f;                                           // the dot family folds with l_norm 1
@@ -1752,47 +1610,42 @@ int b200kge_score_1vsN_loss_csr_backward_dropout_norm(int model, int combine, in
   if ((rc = check_loss_kind(loss_kind))) return rc;
   if (batch_size <= 0 || !(label_smoothing >= 0.f && label_smoothing < 1.f)) { set_error("bad batch_size / label_smoothing"); return B200KGE_ERR_INVALID; }
   if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
-  if ((rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
+  if (drop && (rc = validate_dropout(drop, n > 0 ? n : 0, ent->rows, ent->dim, rel->dim))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   Rows E = to_rows(ent), R = to_rows(rel);
   B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
   B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st));
   if (n <= 0) return 0;
   Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
-  BackBufs b;
-  if (!take_back(ws, n, E.rows, E.dim, R.dim, round_up(f.K, 32), b)) {
-    set_error("workspace too small (see b200kge_score_1vsN_loss_csr_dropout_workspace_bytes)");
-    return B200KGE_ERR_WORKSPACE;
-  }
-  if ((rc = launch_identity_triples(n, b.tri, st))) return rc;
+  const int64_t ldq = round_up(f.K, 32);
   const GradSpec g = csr_grad(q_idx, csr_off, csr_col, label_smoothing, E.rows, batch_size, loss_kind, offset);
-  return dropout_backward_dir(model, l_norm, combine, mask_dir, E, R, q_idx, p_idx, n, *drop, g, b, rest_of(ws), d_ent,
-                              lde, d_rel, ldr, st);
-}
-
-int b200kge_score_1vsN_loss_csr_backward_dropout_dir(int model, int combine, int mask_dir, const b200kge_rows_t* ent,
-                                                     const b200kge_rows_t* rel, const int64_t* q_idx,
-                                                     const int64_t* p_idx, int64_t n, const int64_t* csr_off,
-                                                     const int64_t* csr_col, float label_smoothing, int loss_kind,
-                                                     float offset, int64_t batch_size, const b200kge_dropout_t* drop,
-                                                     float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                                                     void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
-  return b200kge_score_1vsN_loss_csr_backward_dropout_norm(model, combine, mask_dir, 1.0f, ent, rel, q_idx, p_idx, n,
-                                                           csr_off, csr_col, label_smoothing, loss_kind, offset,
-                                                           batch_size, drop, d_ent, lde, d_rel, ldr, workspace,
-                                                           workspace_bytes, stream);
-}
-
-int b200kge_score_1vsN_loss_csr_backward_dropout(int model, int combine, const b200kge_rows_t* ent,
-                                                 const b200kge_rows_t* rel, const int64_t* q_idx, const int64_t* p_idx,
-                                                 int64_t n, const int64_t* csr_off, const int64_t* csr_col,
-                                                 float label_smoothing, int loss_kind, float offset, int64_t batch_size,
-                                                 const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
-                                                 int64_t ldr, void* workspace, size_t workspace_bytes,
-                                                 b200kge_stream_t stream) {
-  return b200kge_score_1vsN_loss_csr_backward_dropout_dir(model, combine, combine, ent, rel, q_idx, p_idx, n, csr_off,
-                                                          csr_col, label_smoothing, loss_kind, offset, batch_size, drop,
-                                                          d_ent, lde, d_rel, ldr, workspace, workspace_bytes, stream);
+  if (drop) {
+    BackBufs b;
+    if (!take_back(ws, n, E.rows, E.dim, R.dim, ldq, b)) {
+      set_error("workspace too small (see b200kge_score_1vsN_loss_csr_dropout_workspace_bytes)");
+      return B200KGE_ERR_WORKSPACE;
+    }
+    if ((rc = launch_identity_triples(n, b.tri, st))) return rc;
+    return dropout_backward_dir(model, l_norm, combine, mask_dir, E, R, q_idx, p_idx, n, *drop, g, b, rest_of(ws), d_ent,
+                                lde, d_rel, ldr, st);
+  }
+  float* Q = (float*)ws.take((size_t)n * ldq * 4);
+  float* dQ = (float*)ws.take((size_t)n * ldq * 4);
+  int64_t* tri = (int64_t*)ws.take((size_t)n * 3 * 8);
+  if (!Q || !dQ || !tri) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
+  pack_triples_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(q_idx, p_idx, n, combine, tri);
+  B2K_LAUNCH_CHECK("pack_triples_kernel");
+  Rows A = E; A.idx = q_idx; A.rows = n;
+  Rows Pr = R; Pr.idx = p_idx; Pr.rows = n;
+  if ((rc = launch_fold_queries(model, combine, A, Pr, n, 0, Q, ldq, st))) return rc;
+  if (distance) {
+    Block B{model, combine, &A, nullptr, &Pr, &E, n};
+    B.Qpre = Q;
+    if ((rc = distance_backward(B, l_norm, g, dQ, d_ent, lde, ws, st))) return rc;
+    return launch_unfold_distance(model, E, R, tri, n, combine, dQ, ldq, d_ent, lde, d_rel, ldr, st);
+  }
+  if ((rc = backward_block(model, E, R, n, combine, false, Q, ldq, f.col_off, f.K, g, d_ent, lde, dQ, ws, st))) return rc;
+  return launch_unfold(model, E, R, tri, n, combine, dQ, ldq, d_ent, lde, d_rel, ldr, st);
 }
 
 }  // extern "C"
@@ -1858,24 +1711,41 @@ int b200kge_ns_score_dropout(int model, float l_norm, const b200kge_rows_t* ent,
                            nullptr, 0, out, ldo, nullptr, 0, nullptr, 0, nullptr, 0, (cudaStream_t)stream);
 }
 
-size_t b200kge_ns_dropout_workspace_bytes(int model, int64_t n, int64_t K, int32_t D) {
+size_t b200kge_ns_backward_workspace_bytes(int model, int64_t n, int64_t K, int32_t D, int dropout) {
   (void)K;
-  return (n > 0 && D > 0) ? ns_dropout_workspace_bytes(model, n, D) : 0;
+  if (dropout) return (n > 0 && D > 0) ? ns_dropout_workspace_bytes(model, n, D) : 0;
+  return (size_t)n * (D + 32) * 4 + 1024;    // dQ [n, round_up(K_folded, 32)] floats
 }
 
-int b200kge_ns_backward_dropout(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
-                                const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
-                                const b200kge_dropout_t* drop, const float* grad_scores, int64_t ldg, float* d_ent,
-                                int64_t lde, float* d_rel, int64_t ldr, void* workspace, size_t workspace_bytes,
-                                b200kge_stream_t stream) {
-  int rc = validate_ns_dropout(model, l_norm, ent, rel, triples, slot, neg, n, K, impl, drop); if (rc) return rc;
-  if (n == 0) return 0;
-  if (!grad_scores || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
-  if (ldg < K + 1) { set_error("grad_scores is narrower than the 1 + K columns of the block"); return B200KGE_ERR_INVALID; }
+int b200kge_ns_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                        const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
+                        const b200kge_dropout_t* drop, const float* grad_scores, int64_t ldg, float offset,
+                        int64_t batch_size, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
+                        size_t workspace_bytes, b200kge_stream_t stream) {
+  int rc;
+  if (drop) {
+    if ((rc = validate_ns_dropout(model, l_norm, ent, rel, triples, slot, neg, n, K, impl, drop))) return rc;
+    if (n == 0) return 0;
+  }
+  // dropout has no in-kernel BCE form: it needs grad_scores
+  if (!triples || (!neg && n * K > 0) || (drop && !grad_scores) || !d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if ((rc = check_tables(model, l_norm, ent, rel))) return rc;
+  if (!grad_scores && batch_size <= 0) { set_error("batch_size must be positive"); return B200KGE_ERR_INVALID; }
+  if (grad_scores && ldg < K + 1) { set_error("grad_scores is narrower than the 1 + K columns of the block"); return B200KGE_ERR_INVALID; }
   if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
-  return launch_ns_dropout(model, l_norm, to_rows(ent), to_rows(rel), triples, slot, neg, n, K, impl, ns_drop_keys(*drop),
-                           grad_scores, ldg, nullptr, 0, d_ent, lde, d_rel, ldr, workspace, workspace_bytes,
-                           (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  Rows E = to_rows(ent), R = to_rows(rel);
+  if (drop)
+    return launch_ns_dropout(model, l_norm, E, R, triples, slot, neg, n, K, impl, ns_drop_keys(*drop), grad_scores, ldg,
+                             nullptr, 0, d_ent, lde, d_rel, ldr, workspace, workspace_bytes, st);
+  const int64_t ldq = round_up(folded_problem(model, B200KGE_SP_, E.dim, l_norm).K, 32);
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  float* dQ = (float*)ws.take((size_t)n * ldq * 4);
+  if (!dQ && n > 0) { set_error("workspace too small (need n * round_up(K,32) floats)"); return B200KGE_ERR_WORKSPACE; }
+  // BCE: dL/dz computed in the kernel from the offset, scaled 1 / batch_size; else read from grad_scores
+  return launch_ns_backward(model, l_norm, E, R, triples, slot, neg, n, K, grad_scores ? 0.f : offset,
+                            grad_scores ? 1.f : 1.0f / (float)batch_size, grad_scores, grad_scores ? ldg : 0, d_ent, lde,
+                            d_rel, ldr, dQ, ldq, st);
 }
 
 }  // extern "C"

@@ -366,7 +366,7 @@ int launch_ns_dropout(int model, float l_norm, const Rows& ent, const Rows& rel,
     const int D = ent.dim, Dr = rel.dim;
     const int64_t ldq = (D + 31) / 32 * 32;
     if (workspace_bytes < ns_dropout_workspace_bytes(model, n, D) || !workspace) {
-      set_error("workspace too small (see b200kge_ns_dropout_workspace_bytes)");
+      set_error("workspace too small (see b200kge_ns_backward_workspace_bytes)");
       return B200KGE_ERR_WORKSPACE;
     }
     uint8_t* w = (uint8_t*)workspace;

@@ -45,6 +45,16 @@ def _i64(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
     return t
 
 
+def _f32_rows(t: torch.Tensor) -> torch.Tensor:
+    """t as float32 with unit column stride (a row stride the kernels can take), copied only if it is not already."""
+    return t if (t.dtype == torch.float32 and t.stride(1) == 1) else t.float().contiguous()
+
+
+def _i64_block(t: torch.Tensor) -> torch.Tensor:
+    """t (triples [n, 3], negatives [n, K]) as a contiguous int64 block, copied only if it is not already."""
+    return t if (t.dtype == torch.int64 and t.is_contiguous()) else t.long().contiguous()
+
+
 class _Keep:
     """Keeps tensors alive for the duration of a call (the C side borrows raw pointers)."""
 
@@ -228,8 +238,7 @@ def rank_sp_po(model: str, s_tab, rel, o_tab, cand_tab, true_scores, s=None, p=N
         ties = torch.zeros(2 * n, dtype=torch.int64, device=dev)
     f = None
     if filter_labels is not None:
-        f = filter_labels if (filter_labels.dtype == torch.float32 and filter_labels.stride(1) == 1) \
-            else filter_labels.float().contiguous()
+        f = _f32_rows(filter_labels)
     ws = _workspace(MODELS[model], n, m, rs.dim, cand is not None, dev)
     _lib.check(lib.b200kge_rank_sp_po(
         MODELS[model], l_norm, PREC[precision], C.byref(rs), C.byref(rp), C.byref(ro), C.byref(rc), n, t.data_ptr(),
@@ -332,7 +341,7 @@ def _labels(k: _Keep, labels: torch.Tensor) -> Labels:
         k.refs.append(li)
         lab.idx, lab.dense, lab.ldl = li.data_ptr(), None, 0
     else:
-        ld = labels if (labels.dtype == torch.float32 and labels.stride(1) == 1) else labels.float().contiguous()
+        ld = _f32_rows(labels)
         k.refs.append(ld)
         lab.idx, lab.dense, lab.ldl = None, ld.data_ptr(), ld.stride(0)
     return lab
@@ -374,8 +383,7 @@ def score_1vsN_rank(model: str, combine: str, q_tab, rel, cand_tab, true_scores,
         ties = torch.zeros(n, dtype=torch.int64, device=dev)
     f = None
     if filter_labels is not None:
-        f = filter_labels if (filter_labels.dtype == torch.float32 and filter_labels.stride(1) == 1) \
-            else filter_labels.float().contiguous()
+        f = _f32_rows(filter_labels)
     ws = _workspace(MODELS[model], n, m, rq.dim, cand is not None, dev)
     _lib.check(lib.b200kge_score_1vsN_rank(
         MODELS[model], SP_ if combine == "sp_" else _PO, l_norm, PREC[precision], C.byref(rq), C.byref(rp),
@@ -389,7 +397,7 @@ def loss_dense(scores, labels, loss: str = "bce", offset: float = 0.0, return_ro
     """KgeLoss (sum) on a dense score matrix (loss.py:153-159 / :198-213)."""
     _require_cuda(scores, labels)
     lib, k = _lib.load(), _Keep()
-    x = scores if (scores.dtype == torch.float32 and scores.stride(1) == 1) else scores.float().contiguous()
+    x = _f32_rows(scores)
     n, m = x.shape
     lab = _labels(k, labels)
     dev = x.device
@@ -408,7 +416,7 @@ def rank_dense(scores, true_scores, filter_labels=None, rtol: float = 1e-4, atol
     """_get_ranks_and_num_ties (+ optional filter subtraction) on dense scores; integer, bit-exact."""
     _require_cuda(scores, true_scores, filter_labels)
     lib = _lib.load()
-    x = scores if (scores.dtype == torch.float32 and scores.stride(1) == 1) else scores.float().contiguous()
+    x = _f32_rows(scores)
     n, m = x.shape
     dev = x.device
     t = true_scores.reshape(-1).float().contiguous()
@@ -418,8 +426,7 @@ def rank_dense(scores, true_scores, filter_labels=None, rtol: float = 1e-4, atol
         ties = torch.zeros(n, dtype=torch.int64, device=dev)
     f = None
     if filter_labels is not None:
-        f = filter_labels if (filter_labels.dtype == torch.float32 and filter_labels.stride(1) == 1) \
-            else filter_labels.float().contiguous()
+        f = _f32_rows(filter_labels)
     _lib.check(lib.b200kge_rank_dense(x.data_ptr(), x.stride(0), n, m, t.data_ptr(),
                                       f.data_ptr() if f is not None else None,
                                       f.stride(0) if f is not None else 0, rtol, atol, rank.data_ptr(),
@@ -440,8 +447,8 @@ def ns_score(model: str, ent, rel, triples, negatives, slot: int, with_positive:
         if not with_positive:
             raise ValueError("ns_score with dropout returns the [n, 1+K] block (with_positive=True)")
         re_, rr = k.rows(ent), k.rows(rel)
-        tri = triples if (triples.dtype == torch.int64 and triples.is_contiguous()) else triples.long().contiguous()
-        neg = negatives if (negatives.dtype == torch.int64 and negatives.is_contiguous()) else negatives.long().contiguous()
+        tri = _i64_block(triples)
+        neg = _i64_block(negatives)
         n, K = neg.shape
         out = torch.empty((n, K + 1), dtype=torch.float32, device=ent.device)
         _lib.check(lib.b200kge_ns_score_dropout(MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(),
@@ -498,7 +505,7 @@ def sample_uniform_filtered(n: int, K: int, vocab: int, seed: int, offset: int, 
     if index.vocab != vocab:
         raise ValueError(f"the filter index was built for a vocabulary of {index.vocab}, not {vocab}")
     _require_cuda(triples, index.keys)
-    tri = triples if (triples.dtype == torch.int64 and triples.is_contiguous()) else triples.long().contiguous()
+    tri = _i64_block(triples)
     if tri.dim() != 2 or tri.shape[1] != 3 or tri.shape[0] != n:
         raise ValueError(f"expected triples [{n}, 3], got {tuple(tri.shape)}")
     out = torch.empty((n, K), dtype=torch.int64, device=tri.device)
@@ -508,32 +515,35 @@ def sample_uniform_filtered(n: int, K: int, vocab: int, seed: int, offset: int, 
     return out
 
 
-def train_1vsall_forward(model: str, ent, rel, triples, loss: str = "bce", offset: float = 0.0,
-                         l_norm: float = 1.0, precision: str = "auto", out=None, workspace=None,
-                         dropout: Optional["DropoutKey"] = None):
-    """One fused 1vsAll forward step for device-resident triples [n,3]; returns the 0-d loss
-    (loss(score_sp,o) + loss(score_po,s)) / n  (train_1vsAll.py:48-82).  With `dropout` the six embedding-dropout draws
-    of the step are applied (b200kge_train_1vsall_forward_dropout; `workspace` is not used)."""
+def _train_1vsall_forward(model, ent, rel, triples, num_relations, loss, offset, l_norm, precision, dropout, out=None,
+                          workspace=None):
     _require_cuda(ent, rel, triples)
     lib, k = _lib.load(), _Keep()
     re_, rr = k.rows(ent), k.rows(rel)
-    tri = triples if (triples.dtype == torch.int64 and triples.is_contiguous()) else triples.long().contiguous()
+    tri = _i64_block(triples)
     n = tri.shape[0]
     dev = ent.device
     if out is None:
         out = torch.empty((), dtype=torch.float32, device=dev)
     if dropout is not None:
-        ws = torch.empty(lib.b200kge_train_1vsall_dropout_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1]),
+        ws = torch.empty(lib.b200kge_train_1vsall_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1], 1),
                          dtype=torch.uint8, device=dev)
-        _lib.check(lib.b200kge_train_1vsall_forward_dropout(
-            MODELS[model], l_norm, PREC[precision], C.byref(re_), C.byref(rr), tri.data_ptr(), n, LOSS[loss], offset,
-            C.byref(dropout.struct()), out.data_ptr(), ws.data_ptr(), ws.numel(), _stream(dev)))
-        return out
-    ws = workspace if workspace is not None else _workspace(MODELS[model], n, ent.shape[0], ent.shape[1], False, dev)
+    else:
+        ws = workspace if workspace is not None else _workspace(MODELS[model], n, ent.shape[0], ent.shape[1], False, dev)
     _lib.check(lib.b200kge_train_1vsall_forward(
-        MODELS[model], l_norm, PREC[precision], C.byref(re_), C.byref(rr), tri.data_ptr(), n, LOSS[loss],
-        offset, out.data_ptr(), ws.data_ptr(), ws.numel(), _stream(dev)))
+        MODELS[model], l_norm, PREC[precision], C.byref(re_), C.byref(rr), int(num_relations), tri.data_ptr(), n,
+        LOSS[loss], offset, None if dropout is None else C.byref(dropout.struct()), out.data_ptr(), ws.data_ptr(),
+        ws.numel(), _stream(dev)))
     return out
+
+
+def train_1vsall_forward(model: str, ent, rel, triples, loss: str = "bce", offset: float = 0.0,
+                         l_norm: float = 1.0, precision: str = "auto", out=None, workspace=None,
+                         dropout: Optional["DropoutKey"] = None):
+    """One fused 1vsAll forward step for device-resident triples [n,3]; returns the 0-d loss
+    (loss(score_sp,o) + loss(score_po,s)) / n  (train_1vsAll.py:48-82).  With `dropout` the six embedding-dropout draws
+    of the step are applied (b200kge_train_1vsall_forward with a dropout key; `workspace` is not used)."""
+    return _train_1vsall_forward(model, ent, rel, triples, 0, loss, offset, l_norm, precision, dropout, out, workspace)
 
 
 class Step1vsAll:
@@ -557,18 +567,19 @@ class Step1vsAll:
         self.loss_np = self.loss_host.numpy()
         self.key = (self.ent.data_ptr(), self.rel.data_ptr(), tuple(ent.shape), tuple(rel.shape))
         self.args = (MODELS[model], C.c_float(l_norm), PREC[precision], C.byref(self.re), C.byref(self.rr))
-        self.tail = (LOSS[loss], C.c_float(offset), C.c_void_p(self.out.data_ptr()), C.c_void_p(self.ws.data_ptr()),
-                     self.ws.numel())
+        self.loss_args = (LOSS[loss], C.c_float(offset))
+        self.out_ptr = C.c_void_p(self.out.data_ptr())
+        self.ws_args = (C.c_void_p(self.ws.data_ptr()), self.ws.numel())
         self.dev = ent.device
 
     def matches(self, ent, rel, n):
         return n <= self.max_n and self.key == (ent.data_ptr(), rel.data_ptr(), tuple(ent.shape), tuple(rel.shape))
 
     def __call__(self, triples: torch.Tensor) -> torch.Tensor:
-        if triples.dtype != torch.int64 or not triples.is_contiguous():
-            triples = triples.long().contiguous()
-        rc = self.lib.b200kge_train_1vsall_forward(*self.args, C.c_void_p(triples.data_ptr()), triples.shape[0],
-                                                   *self.tail, _stream(self.dev))
+        triples = _i64_block(triples)
+        # plain model (num_relations = 0), no dropout
+        rc = self.lib.b200kge_train_1vsall_forward(*self.args, 0, C.c_void_p(triples.data_ptr()), triples.shape[0],
+                                                   *self.loss_args, None, self.out_ptr, *self.ws_args, _stream(self.dev))
         if rc:
             _lib.check(rc)
         return self.out
@@ -578,8 +589,8 @@ class Step1vsAll:
         4-byte read-back and the stream synchronisation inside ONE library call (triples.to(device) ... .item(),
         train_1vsAll.py:59-77)."""
         rc = self.lib.b200kge_train_1vsall_forward_host(
-            *self.args, C.c_void_p(triples_host.data_ptr()), triples_host.shape[0], self.tail[0], self.tail[1],
-            C.c_void_p(self.loss_host.data_ptr()), self.tail[3], self.ws.numel(), _stream(self.dev))
+            *self.args, C.c_void_p(triples_host.data_ptr()), triples_host.shape[0], *self.loss_args,
+            C.c_void_p(self.loss_host.data_ptr()), *self.ws_args, _stream(self.dev))
         if rc:
             _lib.check(rc)
         return float(self.loss_np[0])
@@ -628,32 +639,30 @@ def gemm_nt(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     return out
 
 
-def train_1vsall_backward(model: str, ent, rel, triples, loss: str = "bce", offset: float = 0.0, l_norm: float = 1.0,
-                          dropout: Optional["DropoutKey"] = None):
-    """(d_ent, d_rel): dense table gradients of train_1vsall_forward's loss (dot family; TransE L1/L2; RotatE L1), with
-    the forward's dropout masks when `dropout` is the forward's key."""
+def _train_1vsall_backward(model, ent, rel, triples, num_relations, loss, offset, l_norm, dropout):
     _require_cuda(ent, rel, triples)
     lib, k = _lib.load(), _Keep()
     re_, rr = k.rows(ent), k.rows(rel)
-    tri = triples if (triples.dtype == torch.int64 and triples.is_contiguous()) else triples.long().contiguous()
+    tri = _i64_block(triples)
     n = tri.shape[0]
     dev = ent.device
     d_ent = torch.empty_like(_f32(ent))
     d_rel = torch.empty_like(_f32(rel))
-    if dropout is not None:
-        ws = torch.empty(lib.b200kge_train_1vsall_dropout_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1]),
-                         dtype=torch.uint8, device=dev)
-        _lib.check(lib.b200kge_train_1vsall_backward_dropout(
-            MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), n, LOSS[loss], offset,
-            C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0),
-            ws.data_ptr(), ws.numel(), _stream(dev)))
-        return d_ent, d_rel
-    nbytes = lib.b200kge_train_1vsall_backward_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1])
+    nbytes = lib.b200kge_train_1vsall_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1],
+                                                      0 if dropout is None else 1)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     _lib.check(lib.b200kge_train_1vsall_backward(
-        MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), n, LOSS[loss], offset, d_ent.data_ptr(),
-        d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0), ws.data_ptr(), ws.numel(), _stream(dev)))
+        MODELS[model], l_norm, C.byref(re_), C.byref(rr), int(num_relations), tri.data_ptr(), n, LOSS[loss], offset,
+        None if dropout is None else C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(),
+        d_rel.stride(0), ws.data_ptr(), ws.numel(), _stream(dev)))
     return d_ent, d_rel
+
+
+def train_1vsall_backward(model: str, ent, rel, triples, loss: str = "bce", offset: float = 0.0, l_norm: float = 1.0,
+                          dropout: Optional["DropoutKey"] = None):
+    """(d_ent, d_rel): dense table gradients of train_1vsall_forward's loss (dot family; TransE L1/L2; RotatE L1), with
+    the forward's dropout masks when `dropout` is the forward's key."""
+    return _train_1vsall_backward(model, ent, rel, triples, 0, loss, offset, l_norm, dropout)
 
 
 def train_1vsall_reciprocal_forward(model: str, ent, rel, triples, num_relations: int, loss: str = "bce",
@@ -661,43 +670,16 @@ def train_1vsall_reciprocal_forward(model: str, ent, rel, triples, num_relations
                                     dropout: Optional["DropoutKey"] = None):
     """The 1vsAll step of a reciprocal-relations model (rel holds 2 * num_relations rows): 0-d
     (loss(score_sp(s, p), o) + loss(score_sp(o, p + R), s)) / n  (reciprocal_relations_model.py:85-92), with the
-    embedding-dropout draws of `dropout` (direction 1 on the _po streams) — b200kge_train_1vsall_reciprocal_forward."""
-    _require_cuda(ent, rel, triples)
-    lib, k = _lib.load(), _Keep()
-    re_, rr = k.rows(ent), k.rows(rel)
-    tri = triples if (triples.dtype == torch.int64 and triples.is_contiguous()) else triples.long().contiguous()
-    n = tri.shape[0]
-    dev = ent.device
-    out = torch.empty((), dtype=torch.float32, device=dev)
-    ws = torch.empty(lib.b200kge_train_1vsall_reciprocal_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1]),
-                     dtype=torch.uint8, device=dev)
-    drop = None if dropout is None else C.byref(dropout.struct())
-    _lib.check(lib.b200kge_train_1vsall_reciprocal_forward(
-        MODELS[model], l_norm, PREC[precision], C.byref(re_), C.byref(rr), int(num_relations), tri.data_ptr(), n,
-        LOSS[loss], offset, drop, out.data_ptr(), ws.data_ptr(), ws.numel(), _stream(dev)))
-    return out
+    embedding-dropout draws of `dropout` (direction 1 on the _po streams) — b200kge_train_1vsall_forward with
+    num_relations > 0."""
+    return _train_1vsall_forward(model, ent, rel, triples, num_relations, loss, offset, l_norm, precision, dropout)
 
 
 def train_1vsall_reciprocal_backward(model: str, ent, rel, triples, num_relations: int, loss: str = "bce",
                                      offset: float = 0.0, l_norm: float = 1.0, dropout: Optional["DropoutKey"] = None):
     """(d_ent, d_rel): dense table gradients (all 2R relation rows) of train_1vsall_reciprocal_forward's loss, under the
     forward's masks when `dropout` is the forward's key (dot family; TransE L1/L2; RotatE L1)."""
-    _require_cuda(ent, rel, triples)
-    lib, k = _lib.load(), _Keep()
-    re_, rr = k.rows(ent), k.rows(rel)
-    tri = triples if (triples.dtype == torch.int64 and triples.is_contiguous()) else triples.long().contiguous()
-    n = tri.shape[0]
-    dev = ent.device
-    d_ent = torch.empty_like(_f32(ent))
-    d_rel = torch.empty_like(_f32(rel))
-    ws = torch.empty(lib.b200kge_train_1vsall_reciprocal_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1]),
-                     dtype=torch.uint8, device=dev)
-    drop = None if dropout is None else C.byref(dropout.struct())
-    _lib.check(lib.b200kge_train_1vsall_reciprocal_backward(
-        MODELS[model], l_norm, C.byref(re_), C.byref(rr), int(num_relations), tri.data_ptr(), n, LOSS[loss], offset,
-        drop, d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0), ws.data_ptr(), ws.numel(),
-        _stream(dev)))
-    return d_ent, d_rel
+    return _train_1vsall_backward(model, ent, rel, triples, num_relations, loss, offset, l_norm, dropout)
 
 
 def score_1vsN_backward(model: str, combine: str, ent, rel, q, p, grad_scores, l_norm: float = 1.0):
@@ -707,7 +689,7 @@ def score_1vsN_backward(model: str, combine: str, ent, rel, q, p, grad_scores, l
     lib, k = _lib.load(), _Keep()
     re_, rr = k.rows(ent), k.rows(rel)
     qi, pi = _i64(q), _i64(p)
-    g = grad_scores if (grad_scores.dtype == torch.float32 and grad_scores.stride(1) == 1) else grad_scores.float().contiguous()
+    g = _f32_rows(grad_scores)
     n = qi.numel()
     dev = ent.device
     d_ent = torch.empty_like(_f32(ent))
@@ -737,22 +719,17 @@ def score_1vsN_loss_csr_backward(model: str, combine: str, ent, rel, q, p, csr_o
     d_ent = torch.empty_like(_f32(ent))
     d_rel = torch.empty_like(_f32(rel))
     if dropout is not None:
-        ws = torch.empty(lib.b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(
-            MODELS[model], n, ent.shape[0], ent.shape[1], int(cols.numel())), dtype=torch.uint8, device=dev)
-        _lib.check(lib.b200kge_score_1vsN_loss_csr_backward_dropout_norm(
-            MODELS[model], SP_ if combine == "sp_" else _PO, SP_ if (dropout_streams or combine) == "sp_" else _PO,
-            l_norm, C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(),
-            cols.data_ptr() if cols.numel() else None, label_smoothing, LOSS[loss], offset, batch_size or n,
-            C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0),
-            ws.data_ptr(), ws.numel(), _stream(dev)))
-        return d_ent, d_rel
-    ws = torch.empty(lib.b200kge_score_1vsN_backward_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1]),
-                     dtype=torch.uint8, device=dev)
-    _lib.check(lib.b200kge_score_1vsN_loss_csr_backward_norm(
-        MODELS[model], SP_ if combine == "sp_" else _PO, l_norm, C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(),
-        n, offs.data_ptr(), cols.data_ptr() if cols.numel() else None, label_smoothing, LOSS[loss], offset,
-        batch_size or n, d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0), ws.data_ptr(), ws.numel(),
-        _stream(dev)))
+        nbytes = lib.b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1],
+                                                                          int(cols.numel()))
+    else:
+        nbytes = lib.b200kge_score_1vsN_backward_workspace_bytes(MODELS[model], n, ent.shape[0], ent.shape[1])
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    _lib.check(lib.b200kge_score_1vsN_loss_csr_backward(
+        MODELS[model], SP_ if combine == "sp_" else _PO, SP_ if (dropout_streams or combine) == "sp_" else _PO, l_norm,
+        C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(),
+        cols.data_ptr() if cols.numel() else None, label_smoothing, LOSS[loss], offset, batch_size or n,
+        None if dropout is None else C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(),
+        d_rel.stride(0), ws.data_ptr(), ws.numel(), _stream(dev)))
     return d_ent, d_rel
 
 
@@ -810,53 +787,36 @@ def ns_backward(model: str, ent, rel, triples, negatives: dict, offset: float = 
     and `offset` / `batch_size` are not used: any loss of ns_loss trains through the same kernel.
 
     With `dropout` (the forward's engine.DropoutKey and `implementation`) the gradients go through the forward's masks
-    (b200kge_ns_backward_dropout); grad_scores is then required."""
+    (b200kge_ns_backward with a dropout key); grad_scores is then required."""
     _require_cuda(ent, rel, triples)
     lib, k = _lib.load(), _Keep()
     re_, rr = k.rows(ent), k.rows(rel)
-    tri = triples if (triples.dtype == torch.int64 and triples.is_contiguous()) else triples.long().contiguous()
+    tri = _i64_block(triples)
     n = tri.shape[0]
     dev = ent.device
     d_ent = torch.zeros_like(_f32(ent))
     d_rel = torch.zeros_like(_f32(rel))
     if dropout is not None and grad_scores is None:
         raise ValueError("ns_backward with dropout needs grad_scores (e.g. the G of ns_loss(..., want_grad=True))")
-    if dropout is not None:
-        nbytes = lib.b200kge_ns_dropout_workspace_bytes(MODELS[model], n, 0, ent.shape[1])
-    else:
-        nbytes = n * (ent.shape[1] + 32) * 4 + 1024
+    nbytes = lib.b200kge_ns_backward_workspace_bytes(MODELS[model], n, 0, ent.shape[1], 0 if dropout is None else 1)
     ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    drop = None if dropout is None else C.byref(dropout.struct())
+    impl = 0 if dropout is None else NS_IMPL[implementation]
     for slot, neg in negatives.items():
-        ng = neg if (neg.dtype == torch.int64 and neg.is_contiguous()) else neg.long().contiguous()
-        if dropout is not None:
+        ng = _i64_block(neg)
+        g = None
+        if grad_scores is not None:
             g = grad_scores[slot]
             _require_cuda(g)
             if g.shape != (n, ng.shape[1] + 1):
                 raise ValueError(f"grad_scores[{slot}] has shape {tuple(g.shape)}, expected {(n, ng.shape[1] + 1)}")
-            g = g if (g.dtype == torch.float32 and g.stride(1) == 1) else g.float().contiguous()
+            g = _f32_rows(g)
             k.refs.append(g)
-            _lib.check(lib.b200kge_ns_backward_dropout(
-                MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), int(slot), ng.data_ptr(), n,
-                ng.shape[1], NS_IMPL[implementation], C.byref(dropout.struct()), g.data_ptr(), g.stride(0),
-                d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0), ws.data_ptr(), ws.numel(),
-                _stream(dev)))
-            continue
-        if grad_scores is None:
-            _lib.check(lib.b200kge_ns_backward(
-                MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), int(slot), ng.data_ptr(), n,
-                ng.shape[1], offset, batch_size or n, d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(),
-                d_rel.stride(0), ws.data_ptr(), ws.numel(), _stream(dev)))
-            continue
-        g = grad_scores[slot]
-        _require_cuda(g)
-        if g.shape != (n, ng.shape[1] + 1):
-            raise ValueError(f"grad_scores[{slot}] has shape {tuple(g.shape)}, expected {(n, ng.shape[1] + 1)}")
-        g = g if (g.dtype == torch.float32 and g.stride(1) == 1) else g.float().contiguous()
-        k.refs.append(g)
-        _lib.check(lib.b200kge_ns_backward_grad(
+        _lib.check(lib.b200kge_ns_backward(
             MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), int(slot), ng.data_ptr(), n, ng.shape[1],
-            g.data_ptr(), g.stride(0), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0),
-            ws.data_ptr(), ws.numel(), _stream(dev)))
+            impl, drop, g.data_ptr() if g is not None else None, g.stride(0) if g is not None else 0, offset,
+            batch_size or n, d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(), d_rel.stride(0), ws.data_ptr(),
+            ws.numel(), _stream(dev)))
     return d_ent, d_rel
 
 
@@ -900,7 +860,7 @@ def score_1vsN_loss_csr(model: str, combine: str, q_tab, rel, cand_tab, csr_offs
     embedding-dropout draws of the query type are applied (b200kge_score_1vsN_loss_csr_dropout): the queries are rows
     q of the entity table q_tab, which must also be the candidate table.  `dropout_streams` ("sp_" | "_po") draws the
     masks of that query type instead of `combine`'s (a reciprocal-relations model's _po queries: combine "sp_",
-    streams "_po"; b200kge_score_1vsN_loss_csr_dropout_dir)."""
+    streams "_po": the `mask_dir` of b200kge_score_1vsN_loss_csr_dropout)."""
     _require_cuda(q_tab, rel, cand_tab, csr_offsets, csr_cols)
     lib, k = _lib.load(), _Keep()
     rq, rp, rc = k.rows(q_tab, q), k.rows(rel, p), k.rows(cand_tab)
@@ -918,7 +878,7 @@ def score_1vsN_loss_csr(model: str, combine: str, q_tab, rel, cand_tab, csr_offs
         k.refs += [qi, pi]
         ws = torch.empty(lib.b200kge_score_1vsN_loss_csr_dropout_workspace_bytes(MODELS[model], n, m, rq.dim, nnz),
                          dtype=torch.uint8, device=dev)
-        _lib.check(lib.b200kge_score_1vsN_loss_csr_dropout_dir(
+        _lib.check(lib.b200kge_score_1vsN_loss_csr_dropout(
             MODELS[model], SP_ if combine == "sp_" else _PO, SP_ if (dropout_streams or combine) == "sp_" else _PO,
             l_norm, PREC[precision], C.byref(re_), C.byref(rr), qi.data_ptr(), pi.data_ptr(), n, offs.data_ptr(),
             cols.data_ptr() if nnz else None, nnz, label_smoothing, LOSS[loss], offset, C.byref(dropout.struct()),

@@ -228,7 +228,7 @@ def _install_embedder_kernels(emb):
 class _KvsAllLossFn(torch.autograd.Function):
     """KvsAll loss of one query type with CSR labels / batch_size: forward = fused score + loss with the CSR consumed in
     the epilogue; backward = the gradient kernels (b200kge_score_1vsN_loss_csr_backward).  With a dropout key both run
-    the dropout entry points under the same masks."""
+    the dropout forms (b200kge_score_1vsN_loss_csr_dropout, the backward with its dropout key) under the same masks."""
 
     @staticmethod
     def forward(ctx, ent_w, rel_w, model, combine, a, p, offs, cols, loss, offset, smoothing, batch_size, dropout=None,
@@ -260,9 +260,10 @@ class _NsSlotLossFn(torch.autograd.Function):
     """One slot of a negative-sampling batch: forward = fused gather+score [n, 1+K] and the loss kernel; backward = the
     fused NS gradient kernel (b200kge_ns_backward: per-row fold, per-column recompute, scatter).  BCE runs the dense-loss
     kernel and the kernel's own BCE gradient; every other loss runs the row-loss kernel (b200kge_ns_loss), which also
-    writes G = dL/dscores, and the backward reads G (b200kge_ns_backward_grad).  With a dropout key (engine.DropoutKey)
+    writes G = dL/dscores, and the backward reads G (b200kge_ns_backward with grad_scores).  With a dropout key (engine.DropoutKey)
     the forward scores the masked block (b200kge_ns_score_dropout, draws of `implementation`), every loss BCE included
-    runs the row-loss kernel, and the backward regenerates the same masks from the key (b200kge_ns_backward_dropout)."""
+    runs the row-loss kernel, and the backward regenerates the same masks from the key (b200kge_ns_backward with the
+    key)."""
 
     @staticmethod
     def forward(ctx, ent_w, rel_w, model, triples, negatives, slot, offset, batch_size, loss="bce", temperature=1.0,

@@ -9,8 +9,10 @@ baseline run reproduces bit for bit must be bit-identical in the changed tree, a
 baseline's own run-to-run spread (largest max |difference| between two of its runs), and every launch count must be
 equal.  Gradients scattered with atomics vary from run to run, so give enough baseline runs to bound that spread.  Paths: the 1vsAll training step forward
 and backward of every model for BCE and KL, plain, under dropout, with reciprocal relations and both; the backward of a
-dense score block; the KvsAll CSR loss and its backward with and without dropout; the evaluation ranking; the
-default-precision scorers.
+dense score block; the KvsAll CSR loss and its backward with and without dropout (on the _po streams too), for the dot
+family and for TransE L1 / L2 and RotatE L1; the evaluation ranking; the default-precision scorers; negative sampling:
+the scores of the S and O slots, plain and with dropout (`triple`, `batch`), and their backward in BCE, given-gradient
+and dropout form for ComplEx, TransE L1 / L2 and RotatE L1.
 """
 import argparse
 import json
@@ -106,6 +108,39 @@ def run(tree, out):
                     rec(nm + "/bwd", lambda: eng.score_1vsN_loss_csr_backward(model, "sp_", ent, rel, s, p, offs, cols,
                                                                               loss=loss, label_smoothing=ls,
                                                                               dropout=drop, dropout_streams=streams))
+    # the KvsAll CSR loss and its backward for the distance family
+    for model, l_norm in (("transe", 1.0), ("transe", 2.0), ("rotate", 1.0)):
+        ent, rel = tables(model, 2 * R)
+        for loss in ("kl", "bce"):
+            for ls in (0.0, 0.1):
+                for drop, streams in ((None, None), (key, None), (key, "_po")):
+                    nm = f"csr/{model}/l{l_norm:g}/{loss}/ls{ls}/{'drop' if drop else 'plain'}{streams or ''}"
+                    rec(nm + "/fwd", lambda: eng.score_1vsN_loss_csr(model, "sp_", ent, rel, ent, offs, cols, q=s, p=p,
+                                                                     loss=loss, label_smoothing=ls, l_norm=l_norm,
+                                                                     dropout=drop, dropout_streams=streams,
+                                                                     return_rows=True))
+                    rec(nm + "/bwd", lambda: eng.score_1vsN_loss_csr_backward(model, "sp_", ent, rel, s, p, offs, cols,
+                                                                              loss=loss, label_smoothing=ls,
+                                                                              dropout=drop, dropout_streams=streams,
+                                                                              l_norm=l_norm))
+    # negative sampling: the scores of a slot and its backward (BCE in the kernel, a given gradient, dropout)
+    K = 16
+    negs = torch.randint(0, E, (N, K), generator=g).to(dev)
+    grads = {slot: (torch.randn(N, K + 1, generator=g) * 0.01).to(dev) for slot in (0, 2)}
+    for model, l_norm in (("complex", 1.0), ("transe", 1.0), ("transe", 2.0), ("rotate", 1.0)):
+        ent, rel = tables(model, R)
+        for slot in (0, 2):
+            nm = f"ns/{model}/l{l_norm:g}/slot{slot}"
+            rec(nm + "/score", lambda: eng.ns_score(model, ent, rel, tri, negs, slot, with_positive=True, l_norm=l_norm))
+            rec(nm + "/bwd_bce", lambda: eng.ns_backward(model, ent, rel, tri, {slot: negs}, offset=0.5, l_norm=l_norm))
+            rec(nm + "/bwd_grad", lambda: eng.ns_backward(model, ent, rel, tri, {slot: negs}, l_norm=l_norm,
+                                                          grad_scores=grads))
+            for impl in ("triple", "batch"):
+                rec(nm + f"/score_drop_{impl}", lambda: eng.ns_score(model, ent, rel, tri, negs, slot, with_positive=True,
+                                                                     l_norm=l_norm, dropout=key, implementation=impl))
+                rec(nm + f"/bwd_drop_{impl}", lambda: eng.ns_backward(model, ent, rel, tri, {slot: negs}, l_norm=l_norm,
+                                                                      grad_scores=grads, dropout=key,
+                                                                      implementation=impl))
     np.savez(out, **res)
     print(f"{len(res)} arrays -> {out}")
 

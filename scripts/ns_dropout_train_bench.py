@@ -2,7 +2,7 @@
 optimizer step), three routes of B200TrainingJobNegativeSampling alternated in one process:
 
   (a) dropout   user.b200_ns_dropout: true — masked scores (b200kge_ns_score_dropout) -> row-loss kernel -> masked
-                backward (b200kge_ns_backward_dropout)
+                backward (b200kge_ns_backward with the key)
   (b) fallback  the same job without the option: the reference's _process_subbatch (reference embedders, torch dropout,
                 eager scoring, autograd)
   (c) nodrop    the native NS step with dropout 0 (what the batch costs without dropout)

@@ -27,7 +27,7 @@ def test_header_symbols_all_exported(lib):
     assert declared == set(_lib.SIGNATURES), declared ^ set(_lib.SIGNATURES)
     for name in declared:
         assert hasattr(lib, name), name
-    assert lib.b200kge_version() == 100
+    assert lib.b200kge_version() == 101
 
 
 def test_sass_is_hopper_native():

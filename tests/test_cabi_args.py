@@ -30,7 +30,7 @@ class Args:
     def __init__(self, bad=None):
         from kge_b200 import _lib
 
-        self.model, self.l_norm, self.loss, self.num_rel = COMPLEX, 1.0, BCE, R
+        self.model, self.l_norm, self.loss, self.num_rel, self.mask_dir = COMPLEX, 1.0, BCE, R, None
         dim, ld, rel_rows, p_ent = D, D, 2 * R, 0.1
         idx = None
         if bad == "model":
@@ -45,6 +45,10 @@ class Args:
             p_ent = 1.0
         elif bad == "rel_rows":
             rel_rows = R
+        elif bad == "num_rel":
+            self.num_rel = -R
+        elif bad == "mask_dir":
+            self.mask_dir = 2
         self._keep = []
         self.ent_buf = self._f32(E, ld)
         self.rel_buf = self._f32(2 * R, ld)
@@ -66,6 +70,7 @@ class Args:
         self.csr_off = self._i64(N + 1).ctypes.data
         self.csr_col = self._i64(N).ctypes.data
         self.f = self._f32(N, E).ctypes.data          # scores / grad_scores / loss / rank outputs
+        self.grad = None if bad == "no_grad" else self.f      # a dropout backward without grad_scores
         self.d_ent = self._f32(E, ld).ctypes.data
         self.d_rel = self._f32(2 * R, ld).ctypes.data
         self.ws = self._f32(1 << 16)
@@ -86,87 +91,73 @@ def _grad(a):
     return (a.d_ent, a.lde, a.d_rel, a.ldr, a.wsp, a.wsn, None)
 
 
-# entry point -> (call, the bad arguments it must refuse)
+# entry point (":mode" for the training entries that take several) -> (call, the bad arguments it must refuse).  Modes:
+# plain, dropout, reciprocal relations (num_relations > 0) and both for the 1vsAll step; plain and dropout with mask_dir
+# = combine (sp_) or not for the CSR backward; the in-kernel BCE gradient, a given gradient and dropout for NS.
 COMMON = ("null", "idx", "model", "odd_dim")
+
+
+def _fwd_1vsall(reciprocal, drop):
+    return lambda L, a: L.b200kge_train_1vsall_forward(a.model, a.l_norm, 0, a.ent, a.rel, a.num_rel if reciprocal else 0,
+                                                       a.triples, N, a.loss, 0.0, a.drop if drop else None, a.f, a.wsp,
+                                                       a.wsn, None)
+
+
+def _bwd_1vsall(reciprocal, drop):
+    return lambda L, a: L.b200kge_train_1vsall_backward(a.model, a.l_norm, a.ent, a.rel, a.num_rel if reciprocal else 0,
+                                                        a.triples, N, a.loss, 0.0, a.drop if drop else None, *_grad(a))
+
+
+def _csr_bwd(mask_dir, drop):
+    return lambda L, a: L.b200kge_score_1vsN_loss_csr_backward(a.model, 0, a.mask_dir if a.mask_dir is not None else
+                                                               mask_dir, a.l_norm, a.ent, a.rel, a.idx, a.idx, N,
+                                                               a.csr_off, a.csr_col, 0.0, a.loss, 0.0, N,
+                                                               a.drop if drop else None, *_grad(a))
+
+
+def _ns_bwd(drop, grad):
+    return lambda L, a: L.b200kge_ns_backward(a.model, a.l_norm, a.ent, a.rel, a.triples, 0, a.neg, N, K, 0,
+                                              a.drop if drop else None, a.grad if grad else None, E, 0.0, N, *_grad(a))
+
+
 ENTRIES = {
-    "train_1vsall_forward": (
-        lambda L, a: L.b200kge_train_1vsall_forward(a.model, a.l_norm, 0, a.ent, a.rel, a.triples, N, a.loss, 0.0,
-                                                    a.f, a.wsp, a.wsn, None),
-        COMMON + ("l_norm", "loss")),
-    "train_1vsall_backward": (
-        lambda L, a: L.b200kge_train_1vsall_backward(a.model, a.l_norm, a.ent, a.rel, a.triples, N, a.loss, 0.0,
-                                                     *_grad(a)),
-        COMMON + ("l_norm", "loss", "lde")),
-    "train_1vsall_forward_dropout": (
-        lambda L, a: L.b200kge_train_1vsall_forward_dropout(a.model, a.l_norm, 0, a.ent, a.rel, a.triples, N, a.loss,
-                                                            0.0, a.drop, a.f, a.wsp, a.wsn, None),
-        COMMON + ("l_norm", "loss", "dropout")),
-    "train_1vsall_backward_dropout": (
-        lambda L, a: L.b200kge_train_1vsall_backward_dropout(a.model, a.l_norm, a.ent, a.rel, a.triples, N, a.loss,
-                                                             0.0, a.drop, *_grad(a)),
-        COMMON + ("l_norm", "loss", "lde", "dropout")),
-    "train_1vsall_reciprocal_forward": (
-        lambda L, a: L.b200kge_train_1vsall_reciprocal_forward(a.model, a.l_norm, 0, a.ent, a.rel, a.num_rel,
-                                                               a.triples, N, a.loss, 0.0, None, a.f, a.wsp, a.wsn,
-                                                               None),
-        COMMON + ("l_norm", "loss", "rel_rows")),
-    "train_1vsall_reciprocal_forward_dropout": (
-        lambda L, a: L.b200kge_train_1vsall_reciprocal_forward(a.model, a.l_norm, 0, a.ent, a.rel, a.num_rel,
-                                                               a.triples, N, a.loss, 0.0, a.drop, a.f, a.wsp, a.wsn,
-                                                               None),
-        COMMON + ("l_norm", "loss", "rel_rows", "dropout")),
-    "train_1vsall_reciprocal_backward": (
-        lambda L, a: L.b200kge_train_1vsall_reciprocal_backward(a.model, a.l_norm, a.ent, a.rel, a.num_rel,
-                                                                a.triples, N, a.loss, 0.0, None, *_grad(a)),
-        COMMON + ("l_norm", "loss", "lde", "rel_rows")),
-    "train_1vsall_reciprocal_backward_dropout": (
-        lambda L, a: L.b200kge_train_1vsall_reciprocal_backward(a.model, a.l_norm, a.ent, a.rel, a.num_rel,
-                                                                a.triples, N, a.loss, 0.0, a.drop, *_grad(a)),
-        COMMON + ("l_norm", "loss", "lde", "rel_rows", "dropout")),
+    "train_1vsall_forward:plain": (_fwd_1vsall(False, False), COMMON + ("l_norm", "loss")),
+    "train_1vsall_backward:plain": (_bwd_1vsall(False, False), COMMON + ("l_norm", "loss", "lde")),
+    "train_1vsall_forward:dropout": (_fwd_1vsall(False, True), COMMON + ("l_norm", "loss", "dropout")),
+    "train_1vsall_backward:dropout": (_bwd_1vsall(False, True), COMMON + ("l_norm", "loss", "lde", "dropout")),
+    "train_1vsall_forward:reciprocal": (_fwd_1vsall(True, False),
+                                        COMMON + ("l_norm", "loss", "rel_rows", "num_rel")),
+    "train_1vsall_forward:reciprocal+dropout": (_fwd_1vsall(True, True),
+                                                COMMON + ("l_norm", "loss", "rel_rows", "num_rel", "dropout")),
+    "train_1vsall_backward:reciprocal": (_bwd_1vsall(True, False),
+                                         COMMON + ("l_norm", "loss", "lde", "rel_rows", "num_rel")),
+    "train_1vsall_backward:reciprocal+dropout": (_bwd_1vsall(True, True),
+                                                 COMMON + ("l_norm", "loss", "lde", "rel_rows", "num_rel", "dropout")),
     "score_1vsN_backward": (
         lambda L, a: L.b200kge_score_1vsN_backward(a.model, 0, a.l_norm, a.ent, a.rel, a.idx, a.idx, N, a.f, E,
                                                    *_grad(a)),
         COMMON + ("l_norm", "lde")),
-    "score_1vsN_loss_csr_backward": (
-        lambda L, a: L.b200kge_score_1vsN_loss_csr_backward(a.model, 0, a.ent, a.rel, a.idx, a.idx, N, a.csr_off,
-                                                            a.csr_col, 0.0, a.loss, 0.0, N, *_grad(a)),
-        COMMON + ("loss", "lde")),
-    "score_1vsN_loss_csr_dropout": (
-        lambda L, a: L.b200kge_score_1vsN_loss_csr_dropout(a.model, 0, a.l_norm, 0, a.ent, a.rel, a.idx, a.idx, N,
+    "score_1vsN_loss_csr_backward:plain": (_csr_bwd(1, False), COMMON + ("loss", "lde")),
+    "score_1vsN_loss_csr_dropout:mask_dir=sp_": (
+        lambda L, a: L.b200kge_score_1vsN_loss_csr_dropout(a.model, 0, 0, a.l_norm, 0, a.ent, a.rel, a.idx, a.idx, N,
                                                            a.csr_off, a.csr_col, N, 0.0, a.loss, 0.0, a.drop, a.f,
                                                            None, a.wsp, a.wsn, None),
         COMMON + ("dropout",)),
-    "score_1vsN_loss_csr_dropout_dir": (
-        lambda L, a: L.b200kge_score_1vsN_loss_csr_dropout_dir(a.model, 0, 1, a.l_norm, 0, a.ent, a.rel, a.idx, a.idx,
-                                                               N, a.csr_off, a.csr_col, N, 0.0, a.loss, 0.0, a.drop,
-                                                               a.f, None, a.wsp, a.wsn, None),
+    "score_1vsN_loss_csr_dropout:mask_dir=_po": (
+        lambda L, a: L.b200kge_score_1vsN_loss_csr_dropout(a.model, 0, 1, a.l_norm, 0, a.ent, a.rel, a.idx, a.idx, N,
+                                                           a.csr_off, a.csr_col, N, 0.0, a.loss, 0.0, a.drop, a.f,
+                                                           None, a.wsp, a.wsn, None),
         COMMON + ("dropout",)),
-    "score_1vsN_loss_csr_backward_dropout": (
-        lambda L, a: L.b200kge_score_1vsN_loss_csr_backward_dropout(a.model, 0, a.ent, a.rel, a.idx, a.idx, N,
-                                                                    a.csr_off, a.csr_col, 0.0, a.loss, 0.0, N, a.drop,
-                                                                    *_grad(a)),
-        COMMON + ("loss", "lde", "dropout")),
-    "score_1vsN_loss_csr_backward_dropout_dir": (
-        lambda L, a: L.b200kge_score_1vsN_loss_csr_backward_dropout_dir(a.model, 0, 1, a.ent, a.rel, a.idx, a.idx, N,
-                                                                        a.csr_off, a.csr_col, 0.0, a.loss, 0.0, N,
-                                                                        a.drop, *_grad(a)),
-        COMMON + ("loss", "lde", "dropout")),
-    "ns_backward": (
-        lambda L, a: L.b200kge_ns_backward(a.model, a.l_norm, a.ent, a.rel, a.triples, 0, a.neg, N, K, 0.0, N,
-                                           *_grad(a)),
-        COMMON + ("l_norm", "lde")),
-    "ns_backward_grad": (
-        lambda L, a: L.b200kge_ns_backward_grad(a.model, a.l_norm, a.ent, a.rel, a.triples, 0, a.neg, N, K, a.f, E,
-                                                *_grad(a)),
-        COMMON + ("l_norm", "lde")),
+    "score_1vsN_loss_csr_backward:dropout,mask_dir=sp_": (_csr_bwd(0, True), COMMON + ("loss", "lde", "dropout", "mask_dir")),
+    "score_1vsN_loss_csr_backward:dropout,mask_dir=_po": (_csr_bwd(1, True),
+                                                 COMMON + ("loss", "lde", "dropout", "mask_dir")),
+    "ns_backward:bce": (_ns_bwd(False, False), COMMON + ("l_norm", "lde")),
+    "ns_backward:grad_scores": (_ns_bwd(False, True), COMMON + ("l_norm", "lde")),
     "ns_score_dropout": (
         lambda L, a: L.b200kge_ns_score_dropout(a.model, a.l_norm, a.ent, a.rel, a.triples, 0, a.neg, N, K, 0, a.drop,
                                                 a.f, E, None),
         COMMON + ("l_norm", "dropout")),
-    "ns_backward_dropout": (
-        lambda L, a: L.b200kge_ns_backward_dropout(a.model, a.l_norm, a.ent, a.rel, a.triples, 0, a.neg, N, K, 0,
-                                                   a.drop, a.f, E, *_grad(a)),
-        COMMON + ("l_norm", "lde", "dropout")),
+    "ns_backward:dropout": (_ns_bwd(True, True), COMMON + ("l_norm", "lde", "dropout", "no_grad")),
     "rank_sp_po_eval": (
         lambda L, a: L.b200kge_rank_sp_po_eval(a.model, a.l_norm, 0, a.ent, a.rel, a.num_rel, a.idx, a.idx, a.idx, N,
                                                a.f, a.idx, a.csr_off, a.csr_col, None, None, 0.0, 0.0, a.d_ent,

@@ -1,5 +1,5 @@
 """Embedding dropout of the negative-sampling step on the H100: the mask kernel on the NS streams against the CPU mirror
-bit for bit, b200kge_ns_score_dropout / b200kge_ns_backward_dropout against the fp64 masked expression of
+bit for bit, b200kge_ns_score_dropout / b200kge_ns_backward (dropout key) against the fp64 masked expression of
 tests/ns_dropout_oracle.py (and its autograd), determinism, and the job plugin with `user.b200_ns_dropout` against the
 reference job drawing the mirror's masks."""
 import pytest

@@ -1,5 +1,5 @@
 """The negative-sampling losses on the H100: the row-loss kernel (b200kge_ns_loss) against the reference's recorded
-values and gradients (tests/golden/ns_losses.npz), the G-driven NS backward (b200kge_ns_backward_grad) against the CPU
+values and gradients (tests/golden/ns_losses.npz), the G-driven NS backward (b200kge_ns_backward with grad_scores) against the CPU
 algebra in fp64, and B200TrainingJobNegativeSampling training with every loss against the reference job."""
 import os
 
