@@ -295,6 +295,31 @@ int b200kge_sample_uniform_filtered(uint64_t seed, uint64_t offset, int64_t voca
                                     const int64_t* triples, int slot, const int64_t* keys, const int64_t* offsets,
                                     const int64_t* values, int64_t num_keys, int64_t* out, b200kge_stream_t stream);
 
+/* Frequency negative sampling (negative_sampling.sampling_type: frequency; KgeFrequencySampler, kge/util/sampler.py:755-793):
+ * out[i*K + k] i.i.d. with P(x) = q_x / Q, where q are the integer weights of b200kge_frequency_cdf_build (proportional to
+ * the slot's training counts plus the smoothing) and cdf [vocab+1] (device, uint64) is their exclusive prefix,
+ * cdf[0] = 0, cdf[vocab] = Q.  Counter domain: element e = i*K + k takes exactly the 64-bit word r of
+ * b200kge_sample_uniform (word pair e & 1 of Philox block (e/2, offset) under key seed), t = floor(r * Q / 2^64), and
+ * the output is the largest x with cdf[x] <= t: each id's preimage is an interval of r, so P(x) = q_x / Q to within
+ * 2^-64, and an id of zero weight is never drawn.  With all q_x equal the output is b200kge_sample_uniform's. */
+int b200kge_sample_frequency(uint64_t seed, uint64_t offset, int64_t vocab, const uint64_t* cdf, int64_t n, int64_t K,
+                             int64_t* out, b200kge_stream_t stream);
+
+/* Filtered frequency negative sampling (filtering.<slot> with the standard implementation, sampler.py:108-128,163-196,
+ * 755-793): out[i*K + k] i.i.d. with P(y) = q_y / (Q - M_i) over the non-positives y of row i's key, M_i the weight of
+ * the key's positives: the law of the reference's redraw loop.  Triples, slot and filter index as in
+ * b200kge_sample_uniform_filtered; cdf as in b200kge_sample_frequency; below [nnz] (device, uint64) is
+ * b200kge_frequency_filter_build's output for this cdf and index.  Counter domains: each element first takes
+ * b200kge_sample_frequency's draw x, so every position whose x is not a positive equals that entry's output bit for bit.
+ * A positive x is replaced by one draw u = floor(r * (Q - M_i) / 2^64), r the same word pair of block (e/2 | 2^63,
+ * offset), mapped to the id holding the u-th unit of non-positive weight.  No loop's length depends on chance.  Rows
+ * whose key is absent are unfiltered; rows whose positives carry all the weight (Q - M_i = 0) receive -1.  With all
+ * q_x equal the output is b200kge_sample_uniform_filtered's. */
+int b200kge_sample_frequency_filtered(uint64_t seed, uint64_t offset, int64_t vocab, int64_t n, int64_t K,
+                                      const int64_t* triples, int slot, const int64_t* keys, const int64_t* offsets,
+                                      const int64_t* values, int64_t num_keys, const uint64_t* cdf,
+                                      const uint64_t* below, int64_t* out, b200kge_stream_t stream);
+
 /* ---- Embedding dropout of the 1vsAll / KvsAll training steps ---------------------------------------------------------
  * LookupEmbedder._postprocess (lookup_embedder.py:96-105) draws a fresh element-wise Bernoulli mask per embed(idx) /
  * embed_all() call and scales kept values by 1/(1-p).  One sub-batch of 1vsAll training (train_1vsAll.py:64,75 with
@@ -422,6 +447,24 @@ int b200kge_kvsall_gather(const int64_t* keys, const int64_t* offsets, const int
 int b200kge_filter_index_build(const int64_t* keys, const int64_t* offsets, const int64_t* values, int64_t num_keys,
                                int64_t vocab, int64_t* keys_out, int64_t* offsets_out, int64_t* values_out,
                                int64_t* num_keys_out, int64_t* max_count);
+
+/* The weights of frequency sampling (host arrays; KgeFrequencySampler.__init__, sampler.py:762-780 defines them as
+ * w_x = counts[x] + smoothing over the slot's training counts).  The library samples from integer weights
+ * q_x = round((counts[x] + smoothing) * 2^s), rounded half to even, where s >= 0 is the largest integer with
+ * Q = sum q_x <= 2^62: exactly proportional to w for an integral smoothing, and with a relative error per id of at
+ * most 2^-62 * Q / q_x otherwise.  cdf_out [vocab+1] receives the exclusive prefix of q (cdf_out[0] = 0, cdf_out[vocab] = Q).
+ * B200KGE_ERR_INVALID for vocab <= 0, a negative count, a negative or non-finite smoothing, Q = 0 (smoothing 0 and no
+ * id counted) or smoothed counts summing to more than 2^62. */
+int b200kge_frequency_cdf_build(const int64_t* counts, int64_t vocab, double smoothing, uint64_t* cdf_out);
+
+/* The per-entry table of b200kge_sample_frequency_filtered (host arrays): for every value v_j of every key of a filter
+ * index (b200kge_filter_index_build's offsets / values), below_out[j - offsets[0]] = cdf[v_j] - sum_{l<j} q_{v_l}, the
+ * weight of the key's non-positives below v_j.  *num_full receives the number of keys whose positives carry all the
+ * weight (no negative can be drawn for them), *first_full the index of the first such key or -1.  B200KGE_ERR_INVALID
+ * for a cdf that does not start at 0, decreases or ends at 0, decreasing offsets (checked before any value is read), or
+ * values of a key that are not ascending, distinct and in [0, vocab). */
+int b200kge_frequency_filter_build(const uint64_t* cdf, int64_t vocab, const int64_t* offsets, const int64_t* values,
+                                   int64_t num_keys, uint64_t* below_out, int64_t* num_full, int64_t* first_full);
 
 /* ---- SURVEY 8(f) rows: gradients, penalties, CSR labels -------------
  *

@@ -82,6 +82,14 @@ SIGNATURES = {
                                                   C.c_void_p]),
     "b200kge_filter_index_build": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
                                              C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "b200kge_sample_frequency": (C.c_int, [C.c_uint64, C.c_uint64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64,
+                                           C.c_void_p, C.c_void_p]),
+    "b200kge_sample_frequency_filtered": (C.c_int, [C.c_uint64, C.c_uint64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
+                                                    C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                                    C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200kge_frequency_cdf_build": (C.c_int, [C.c_void_p, C.c_int64, C.c_double, C.c_void_p]),
+    "b200kge_frequency_filter_build": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                                 C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "b200kge_train_1vsall_forward": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_int64, C.c_void_p,
                                                C.c_int64, C.c_int, C.c_float, _DP, C.c_void_p, C.c_void_p,
                                                C.c_size_t, C.c_void_p]),

@@ -685,6 +685,29 @@ int b200kge_sample_uniform_filtered(uint64_t seed, uint64_t offset, int64_t voca
                                         (cudaStream_t)stream);
 }
 
+int b200kge_sample_frequency(uint64_t seed, uint64_t offset, int64_t vocab, const uint64_t* cdf, int64_t n, int64_t K,
+                             int64_t* out, b200kge_stream_t stream) {
+  if (vocab <= 0) { set_error("vocabulary size must be positive"); return B200KGE_ERR_INVALID; }
+  if (n < 0 || K < 0) { set_error("negative size"); return B200KGE_ERR_INVALID; }
+  if (n * K > 0 && (!out || !cdf)) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  return launch_sample_frequency(seed, offset, vocab, cdf, n * K, out, (cudaStream_t)stream);
+}
+
+int b200kge_sample_frequency_filtered(uint64_t seed, uint64_t offset, int64_t vocab, int64_t n, int64_t K,
+                                      const int64_t* triples, int slot, const int64_t* keys, const int64_t* offsets,
+                                      const int64_t* values, int64_t num_keys, const uint64_t* cdf,
+                                      const uint64_t* below, int64_t* out, b200kge_stream_t stream) {
+  if (vocab <= 0) { set_error("vocabulary size must be positive"); return B200KGE_ERR_INVALID; }
+  if (slot < 0 || slot > 2) { set_error("slot must be 0 (S), 1 (P) or 2 (O)"); return B200KGE_ERR_INVALID; }
+  if (n < 0 || K < 0 || num_keys < 0) { set_error("negative size"); return B200KGE_ERR_INVALID; }
+  if (n * K > 0 && (!out || !triples || !cdf || (num_keys > 0 && (!keys || !offsets || !values || !below)))) {
+    set_error("null operand");
+    return B200KGE_ERR_INVALID;
+  }
+  return launch_sample_frequency_filtered(seed, offset, vocab, n, K, triples, slot, keys, offsets, values, num_keys, cdf,
+                                          below, out, (cudaStream_t)stream);
+}
+
 // The 1vsAll step without dropout on validated arguments, n > 0.  num_rel > 0: the reciprocal-relations step (rows
 // n..2n are the sp_ queries (o, p + num_rel), label s)
 static int train_1vsall_forward_impl(int model, float l_norm, int precision, const b200kge_rows_t* ent,

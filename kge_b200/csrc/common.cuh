@@ -442,6 +442,13 @@ int launch_sample_uniform(uint64_t seed, uint64_t offset, int64_t vocab, int64_t
 int launch_sample_uniform_filtered(uint64_t seed, uint64_t offset, int64_t vocab, int64_t n, int64_t K,
                                    const int64_t* triples, int slot, const int64_t* keys, const int64_t* offsets,
                                    const int64_t* values, int64_t num_keys, int64_t* out, cudaStream_t st);
+// frequency-weighted draws over cdf[0..vocab] (b200kge_sample_frequency / _filtered)
+int launch_sample_frequency(uint64_t seed, uint64_t offset, int64_t vocab, const uint64_t* cdf, int64_t total,
+                            int64_t* out, cudaStream_t st);
+int launch_sample_frequency_filtered(uint64_t seed, uint64_t offset, int64_t vocab, int64_t n, int64_t K,
+                                     const int64_t* triples, int slot, const int64_t* keys, const int64_t* offsets,
+                                     const int64_t* values, int64_t num_keys, const uint64_t* cdf,
+                                     const uint64_t* below, int64_t* out, cudaStream_t st);
 int launch_loss_dense(int loss_kind, const float* scores, int64_t lds, int64_t n, int64_t m,
                       const EpiParams& P, cudaStream_t st);
 int loss_dense_nchunks(int64_t m);

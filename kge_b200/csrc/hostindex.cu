@@ -7,6 +7,7 @@
 // device epilogues consume instead of `coord_to_sparse_tensor(...).to_dense()` (util.py:32-60).
 // No device code here; the functions run without a GPU.
 #include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <numeric>
 #include <vector>
@@ -28,6 +29,26 @@ inline int64_t find_key(const int64_t* keys, int64_t num_keys, int64_t k0, int64
   }
   if (lo < num_keys && keys[2 * lo] == k0 && keys[2 * lo + 1] == k1) return lo;
   return -1;
+}
+
+// Frequency weights quantised at scale 2^s: q_x = c_x * 2^s + round(alpha * 2^s), rounded half to even.  True if
+// Q = sum q_x <= 2^62; then cdf (when given, [vocab + 1]) receives the exclusive prefix of q, cdf[vocab] = Q.
+bool quantised_total(const int64_t* counts, int64_t vocab, double alpha, int s, uint64_t* cdf) {
+  constexpr uint64_t LIM = 1ull << 62;
+  const double qa = std::nearbyint(std::ldexp(alpha, s));
+  if (!(qa <= (double)LIM)) return false;
+  const uint64_t ua = (uint64_t)qa;
+  uint64_t total = 0;
+  if (cdf) cdf[0] = 0;
+  for (int64_t x = 0; x < vocab; ++x) {
+    const uint64_t c = (uint64_t)counts[x];
+    if (c > 0 && (s > 62 || c > (LIM >> s))) return false;
+    const uint64_t q = (c << (s > 62 ? 0 : s)) + ua;   // <= 2^63: no wrap
+    if (q > LIM - total) return false;
+    total += q;
+    if (cdf) cdf[x + 1] = total;
+  }
+  return true;
 }
 
 }  // namespace
@@ -171,6 +192,66 @@ int b200kge_filter_index_build(const int64_t* keys, const int64_t* offsets, cons
   offsets_out[nk] = (int64_t)ent.size();
   *num_keys_out = nk;
   *max_count = mx;
+  return 0;
+}
+
+int b200kge_frequency_cdf_build(const int64_t* counts, int64_t vocab, double smoothing, uint64_t* cdf_out) {
+  if (vocab <= 0) { set_error("vocabulary size must be positive"); return B200KGE_ERR_INVALID; }
+  if (!counts || !cdf_out) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (!std::isfinite(smoothing) || smoothing < 0) {
+    set_error("smoothing must be finite and >= 0 (got %g)", smoothing);
+    return B200KGE_ERR_INVALID;
+  }
+  for (int64_t x = 0; x < vocab; ++x)
+    if (counts[x] < 0) { set_error("count %lld of id %lld is negative", (long long)counts[x], (long long)x); return B200KGE_ERR_INVALID; }
+  // q_x(s) = c_x * 2^s + round(alpha * 2^s) = round((c_x + alpha) * 2^s) for s >= 0 (c_x * 2^s is an integer); ldexp
+  // is exact and nearbyint rounds half to even, so every q_x is exact.  Q(s) = sum q_x does not decrease in s.
+  if (!quantised_total(counts, vocab, smoothing, 0, nullptr)) {
+    set_error("the smoothed counts sum to more than 2^62");
+    return B200KGE_ERR_INVALID;
+  }
+  int lo = 0, hi = 2200;                  // fits at lo; beyond any alpha * 2^s a double can hold at hi
+  while (hi - lo > 1) {
+    const int mid = lo + (hi - lo) / 2;
+    if (quantised_total(counts, vocab, smoothing, mid, nullptr)) lo = mid;
+    else hi = mid;
+  }
+  quantised_total(counts, vocab, smoothing, lo, cdf_out);
+  if (cdf_out[vocab] == 0) { set_error("every weight is zero (smoothing 0 and no id occurs)"); return B200KGE_ERR_INVALID; }
+  return 0;
+}
+
+int b200kge_frequency_filter_build(const uint64_t* cdf, int64_t vocab, const int64_t* offsets, const int64_t* values,
+                                   int64_t num_keys, uint64_t* below_out, int64_t* num_full, int64_t* first_full) {
+  if (vocab <= 0) { set_error("vocabulary size must be positive"); return B200KGE_ERR_INVALID; }
+  if (num_keys < 0 || !cdf || !offsets || !num_full || !first_full) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (cdf[0] != 0 || cdf[vocab] == 0) { set_error("cdf must start at 0 and end above 0"); return B200KGE_ERR_INVALID; }
+  for (int64_t x = 0; x < vocab; ++x)
+    if (cdf[x + 1] < cdf[x]) { set_error("cdf must not decrease"); return B200KGE_ERR_INVALID; }
+  for (int64_t k = 0; k < num_keys; ++k)
+    if (offsets[k + 1] < offsets[k]) { set_error("offsets must not decrease"); return B200KGE_ERR_INVALID; }
+  const int64_t base = offsets[0];
+  if (offsets[num_keys] > base && (!values || !below_out)) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  const uint64_t Q = cdf[vocab];
+  int64_t full = 0, first = -1;
+  for (int64_t k = 0; k < num_keys; ++k) {
+    uint64_t pos = 0;                     // mass of the key's positives below values[j]
+    for (int64_t j = offsets[k]; j < offsets[k + 1]; ++j) {
+      const int64_t v = values[j - base];
+      if (v < 0 || v >= vocab || (j > offsets[k] && v <= values[j - 1 - base])) {
+        set_error("values of key %lld must be ascending, distinct and in [0, %lld)", (long long)k, (long long)vocab);
+        return B200KGE_ERR_INVALID;
+      }
+      below_out[j - base] = cdf[v] - pos;
+      pos += cdf[v + 1] - cdf[v];
+    }
+    if (pos == Q) {
+      if (first < 0) first = k;
+      ++full;
+    }
+  }
+  *num_full = full;
+  *first_full = first;
   return 0;
 }
 

@@ -410,6 +410,38 @@ __device__ __forceinline__ uint64_t philox_u64(uint64_t seed, uint64_t offset, u
   return odd ? ((uint64_t)c[3] << 32) | c[2] : ((uint64_t)c[1] << 32) | c[0];
 }
 
+// thread 0's lookup of row i's key (tri[3i + c0], tri[3i + c1]) among the sorted keys of a filter index: the start and
+// count of its values, (0, 0) for an absent key
+__device__ __forceinline__ void key_values(const int64_t* __restrict__ tri, int64_t i, int c0, int c1,
+                                           const int64_t* __restrict__ keys, const int64_t* __restrict__ offsets,
+                                           int64_t num_keys, int64_t& begin, int64_t& m) {
+  const int64_t a = tri[3 * i + c0], b = tri[3 * i + c1];
+  int64_t lo = 0, hi = num_keys;
+  while (lo < hi) {
+    const int64_t mid = lo + ((hi - lo) >> 1);
+    const int64_t ka = keys[2 * mid], kb = keys[2 * mid + 1];
+    if (ka < a || (ka == a && kb < b)) lo = mid + 1;
+    else hi = mid;
+  }
+  begin = 0;
+  m = 0;
+  if (lo < num_keys && keys[2 * lo] == a && keys[2 * lo + 1] == b) {
+    begin = offsets[lo];
+    m = offsets[lo + 1] - begin;
+  }
+}
+
+// lower bound of x among the m sorted positives v
+__device__ __forceinline__ int64_t positive_lower_bound(const int64_t* __restrict__ v, int64_t m, int64_t x) {
+  int64_t lo = 0, hi = m;
+  while (lo < hi) {
+    const int64_t mid = lo + ((hi - lo) >> 1);
+    if (__ldg(v + mid) < x) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
 // one CTA per row: thread 0 looks the row's key up once, every thread then takes elements k, k + blockDim.x, ...
 __global__ void __launch_bounds__(256)
 sample_uniform_filtered_kernel(uint64_t seed, uint64_t offset, uint64_t vocab, int64_t K, const int64_t* __restrict__ tri,
@@ -418,19 +450,8 @@ sample_uniform_filtered_kernel(uint64_t seed, uint64_t offset, uint64_t vocab, i
   __shared__ int64_t s_begin, s_m;
   const int64_t i = blockIdx.x;
   if (threadIdx.x == 0) {
-    const int64_t a = tri[3 * i + c0], b = tri[3 * i + c1];
-    int64_t lo = 0, hi = num_keys;
-    while (lo < hi) {
-      const int64_t mid = lo + ((hi - lo) >> 1);
-      const int64_t ka = keys[2 * mid], kb = keys[2 * mid + 1];
-      if (ka < a || (ka == a && kb < b)) lo = mid + 1;
-      else hi = mid;
-    }
-    int64_t begin = 0, m = 0;
-    if (lo < num_keys && keys[2 * lo] == a && keys[2 * lo + 1] == b) {
-      begin = offsets[lo];
-      m = offsets[lo + 1] - begin;
-    }
+    int64_t begin, m;
+    key_values(tri, i, c0, c1, keys, offsets, num_keys, begin, m);
     s_begin = begin;
     s_m = m;
   }
@@ -445,12 +466,7 @@ sample_uniform_filtered_kernel(uint64_t seed, uint64_t offset, uint64_t vocab, i
   for (int64_t k = threadIdx.x; k < K; k += blockDim.x) {
     const uint64_t e = (uint64_t)(i * K + k);
     const int64_t x = (int64_t)__umul64hi(philox_u64(seed, offset, e >> 1, e & 1), vocab);
-    int64_t lo = 0, hi = m;                  // lower bound of x among the positives
-    while (lo < hi) {
-      const int64_t mid = lo + ((hi - lo) >> 1);
-      if (__ldg(v + mid) < x) lo = mid + 1;
-      else hi = mid;
-    }
+    int64_t lo = positive_lower_bound(v, m, x), hi;
     if (lo == m || __ldg(v + lo) != x) { orow[k] = x; continue; }
     const int64_t u = (int64_t)__umul64hi(philox_u64(seed, offset, (e >> 1) | FILTER_DOMAIN, e & 1), vocab - (uint64_t)m);
     lo = 0; hi = m;                          // c = #{j : v[j] - j <= u}
@@ -463,7 +479,122 @@ sample_uniform_filtered_kernel(uint64_t seed, uint64_t offset, uint64_t vocab, i
   }
 }
 
+// Frequency sampling (KgeFrequencySampler, sampler.py:755-793): P(x) = q_x / Q over the integer weights q of
+// b200kge_frequency_cdf_build, given as the exclusive prefix cdf[0..V] (cdf[0] = 0, cdf[V] = Q).  A 64-bit draw r maps
+// to t = floor(r * Q / 2^64) and then to the largest x with cdf[x] <= t: the preimage of x is an interval of q_x / Q of
+// the r range (to within 2^-64), and an id of zero weight is never drawn.
+//
+// The largest x in [0, len - 1) with cdf[x] <= t[j], for N targets at once: a branchless lower bound whose trip count,
+// ceil(log2(len)), depends on len only, so the lanes of a warp never diverge.  Needs cdf[0] <= t[j] < cdf[len - 1].
+template <int N>
+__device__ __forceinline__ void cdf_search(const uint64_t* __restrict__ cdf, int64_t len, const uint64_t (&t)[N],
+                                           int64_t (&x)[N]) {
+#pragma unroll
+  for (int j = 0; j < N; ++j) x[j] = 0;
+  for (int64_t w = len; w > 1;) {
+    const int64_t half = w >> 1;
+#pragma unroll
+    for (int j = 0; j < N; ++j) x[j] += __ldg(cdf + x[j] + half) <= t[j] ? half : 0;
+    w -= half;
+  }
+}
+
+// two elements per Philox block, exactly the words sample_uniform_kernel takes; the two searches run interleaved
+__global__ void __launch_bounds__(256)
+sample_frequency_kernel(uint64_t seed, uint64_t offset, const uint64_t* __restrict__ cdf, int64_t len, int64_t total,
+                        int64_t* __restrict__ out) {
+  const int64_t pair = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (2 * pair >= total) return;
+  uint32_t c[4] = {(uint32_t)pair, (uint32_t)((uint64_t)pair >> 32), (uint32_t)offset, (uint32_t)(offset >> 32)};
+  philox4x32_10(c, seed);
+  const uint64_t Q = __ldg(cdf + len - 1);
+  const uint64_t t[2] = {__umul64hi(((uint64_t)c[1] << 32) | c[0], Q), __umul64hi(((uint64_t)c[3] << 32) | c[2], Q)};
+  int64_t x[2];
+  cdf_search(cdf, len, t, x);
+  out[2 * pair] = x[0];
+  if (2 * pair + 1 < total) out[2 * pair + 1] = x[1];
+}
+
+// Filtered frequency sampling: i.i.d. from q restricted to the non-positives of row i's key, P(y) = q_y / (Q - M_i) with
+// M_i the mass of the key's m positives v_0 < ... < v_{m-1} (the law of the reference's redraw loop).  Element e first
+// takes sample_frequency_kernel's draw x; if x is not a positive it is the output.  Otherwise u = floor(r' * (Q - M_i) /
+// 2^64), r' word pair (e & 1) of block (e/2 | 2^63, offset), picks the u-th unit of non-positive mass.  below[j] =
+// G_j = cdf[v_j] - sum_{l<j} q_{v_l} is the non-positive mass below v_j (non-decreasing in j); with g = #{j : G_j <= u}
+// and PW_g = sum_{l<g} q_{v_l} = cdf[v_{g-1} + 1] - G_{g-1}, the target u + PW_g lies in [cdf[v_{g-1} + 1], cdf[v_g]),
+// so the CDF search lands strictly between two positives on an id of nonzero weight.  No loop's length depends on
+// chance.  Absent keys are unfiltered; a row whose positives carry all the mass (Q - M_i = 0) gets -1.
+__global__ void __launch_bounds__(256)
+sample_frequency_filtered_kernel(uint64_t seed, uint64_t offset, const uint64_t* __restrict__ cdf, int64_t len,
+                                 int64_t K, const int64_t* __restrict__ tri, int c0, int c1,
+                                 const int64_t* __restrict__ keys, const int64_t* __restrict__ offsets,
+                                 const int64_t* __restrict__ values, const uint64_t* __restrict__ below,
+                                 int64_t num_keys, int64_t* __restrict__ out) {
+  __shared__ int64_t s_begin, s_m;
+  __shared__ uint64_t s_q, s_rest;
+  const int64_t i = blockIdx.x;
+  if (threadIdx.x == 0) {
+    int64_t begin, m;
+    key_values(tri, i, c0, c1, keys, offsets, num_keys, begin, m);
+    const uint64_t Q = cdf[len - 1];
+    s_begin = begin;
+    s_m = m;
+    s_q = Q;
+    s_rest = m > 0 ? Q - (cdf[values[begin + m - 1] + 1] - below[begin + m - 1]) : Q;
+  }
+  __syncthreads();
+  const int64_t* __restrict__ v = values + s_begin;
+  const uint64_t* __restrict__ G = below + s_begin;
+  const int64_t m = s_m;
+  const uint64_t Q = s_q, rest = s_rest;
+  int64_t* __restrict__ orow = out + i * K;
+  if (rest == 0) {
+    for (int64_t k = threadIdx.x; k < K; k += blockDim.x) orow[k] = -1;
+    return;
+  }
+  for (int64_t k = threadIdx.x; k < K; k += blockDim.x) {
+    const uint64_t e = (uint64_t)(i * K + k);
+    uint64_t t[1] = {__umul64hi(philox_u64(seed, offset, e >> 1, e & 1), Q)};
+    int64_t x[1];
+    cdf_search(cdf, len, t, x);
+    int64_t lo = positive_lower_bound(v, m, x[0]), hi;
+    if (lo == m || __ldg(v + lo) != x[0]) { orow[k] = x[0]; continue; }
+    const uint64_t u = __umul64hi(philox_u64(seed, offset, (e >> 1) | FILTER_DOMAIN, e & 1), rest);
+    lo = 0; hi = m;                          // g = #{j : G_j <= u}
+    while (lo < hi) {
+      const int64_t mid = lo + ((hi - lo) >> 1);
+      if (__ldg(G + mid) <= u) lo = mid + 1;
+      else hi = mid;
+    }
+    t[0] = u + (lo == 0 ? 0 : __ldg(cdf + __ldg(v + lo - 1) + 1) - __ldg(G + lo - 1));
+    cdf_search(cdf, len, t, x);
+    orow[k] = x[0];
+  }
+}
+
 }  // namespace
+
+int launch_sample_frequency(uint64_t seed, uint64_t offset, int64_t vocab, const uint64_t* cdf, int64_t total,
+                            int64_t* out, cudaStream_t st) {
+  if (total <= 0) return 0;
+  const int64_t pairs = (total + 1) / 2;
+  sample_frequency_kernel<<<(unsigned)((pairs + 255) / 256), 256, 0, st>>>(seed, offset, cdf, vocab + 1, total, out);
+  B2K_LAUNCH_CHECK("sample_frequency_kernel");
+  return 0;
+}
+
+int launch_sample_frequency_filtered(uint64_t seed, uint64_t offset, int64_t vocab, int64_t n, int64_t K,
+                                     const int64_t* triples, int slot, const int64_t* keys, const int64_t* offsets,
+                                     const int64_t* values, int64_t num_keys, const uint64_t* cdf,
+                                     const uint64_t* below, int64_t* out, cudaStream_t st) {
+  if (n <= 0 || K <= 0) return 0;
+  if (n > 2147483647LL) { set_error("too many rows (%lld)", (long long)n); return B200KGE_ERR_UNSUPPORTED; }
+  const int c0 = slot == 0 ? 1 : 0, c1 = slot == 2 ? 1 : 2;   // the key pair of the slot, as launch_sample_uniform_filtered
+  const int threads = K >= 256 ? 256 : (int)((K + 31) / 32) * 32;
+  sample_frequency_filtered_kernel<<<(unsigned)n, threads, 0, st>>>(seed, offset, cdf, vocab + 1, K, triples, c0, c1,
+                                                                     keys, offsets, values, below, num_keys, out);
+  B2K_LAUNCH_CHECK("sample_frequency_filtered_kernel");
+  return 0;
+}
 
 int launch_sample_uniform_filtered(uint64_t seed, uint64_t offset, int64_t vocab, int64_t n, int64_t K,
                                    const int64_t* triples, int slot, const int64_t* keys, const int64_t* offsets,

@@ -515,6 +515,69 @@ def sample_uniform_filtered(n: int, K: int, vocab: int, seed: int, offset: int, 
     return out
 
 
+class FrequencyTable:
+    """The weights of frequency sampling for one slot (KgeFrequencySampler, sampler.py:755-793): counts [V] per id (the
+    slot's column of the training split, bincount'ed) plus `smoothing`, quantised once on the host to integer weights
+    (indexing.frequency_cdf) and uploaded as their exclusive prefix `cdf` [V+1] (int64, cdf[V] = Q <= 2^62)."""
+
+    def __init__(self, counts: torch.Tensor, smoothing: float, device):
+        from .indexing import frequency_cdf
+
+        cdf = frequency_cdf(counts, smoothing)
+        self.vocab = cdf.numel() - 1
+        self.smoothing = float(smoothing)
+        self.total = int(cdf[-1])
+        self.cdf = cdf.to(device)
+
+    def attach(self, index: "FilterIndex") -> "FilterIndex":
+        """Gives `index` the per-entry table of sample_frequency_filtered under these weights: `index.below` [nnz]
+        (device), `index.full_keys` (number of keys whose positives carry all the weight, so that no negative exists
+        for them) and `index.first_full_key` (its (a, b), or None).  Returns `index`."""
+        from .indexing import frequency_below
+
+        if index.vocab != self.vocab:
+            raise ValueError(f"the filter index was built for a vocabulary of {index.vocab}, not {self.vocab}")
+        below, full, first = frequency_below(self.cdf.cpu(), index.offsets.cpu(), index.values.cpu())
+        index.below = below.to(index.values.device)
+        index.below_table = self
+        index.full_keys = full
+        index.first_full_key = tuple(index.keys[first].tolist()) if first >= 0 else None
+        return index
+
+
+def sample_frequency(n: int, K: int, table: FrequencyTable, seed: int, offset: int) -> torch.Tensor:
+    """[n, K] int64 ids drawn on the device with P(x) = q_x / Q, the quantised weights of `table`; each element takes the
+    64-bit draw of sample_uniform(n, K, vocab, seed, offset) (equal weights reproduce it)."""
+    _require_cuda(table.cdf)
+    out = torch.empty((n, K), dtype=torch.int64, device=table.cdf.device)
+    _lib.check(_lib.load().b200kge_sample_frequency(
+        seed & (2 ** 64 - 1), offset & (2 ** 64 - 1), table.vocab, table.cdf.data_ptr(), n, K, out.data_ptr(),
+        _stream(out.device)))
+    return out
+
+
+def sample_frequency_filtered(n: int, K: int, table: FrequencyTable, seed: int, offset: int, triples: torch.Tensor,
+                              slot: int, index: FilterIndex) -> torch.Tensor:
+    """[n, K] int64 ids drawn on the device with P(y) = q_y / (Q - M_i) over the ids y that are not positives of row i's
+    key (M_i: the weight of its positives); keys as in sample_uniform_filtered, `index` attached to `table`
+    (FrequencyTable.attach).  Positions whose first draw is not a positive equal sample_frequency(n, K, table, seed,
+    offset); rows whose positives carry all the weight get -1."""
+    if index.vocab != table.vocab:
+        raise ValueError(f"the filter index was built for a vocabulary of {index.vocab}, not {table.vocab}")
+    if getattr(index, "below_table", None) is not table:
+        raise ValueError("the filter index is not attached to this frequency table (FrequencyTable.attach)")
+    _require_cuda(triples, index.keys, table.cdf)
+    tri = _i64_block(triples)
+    if tri.dim() != 2 or tri.shape[1] != 3 or tri.shape[0] != n:
+        raise ValueError(f"expected triples [{n}, 3], got {tuple(tri.shape)}")
+    out = torch.empty((n, K), dtype=torch.int64, device=tri.device)
+    _lib.check(_lib.load().b200kge_sample_frequency_filtered(
+        seed & (2 ** 64 - 1), offset & (2 ** 64 - 1), table.vocab, n, K, tri.data_ptr(), int(slot),
+        index.keys.data_ptr(), index.offsets.data_ptr(), index.values.data_ptr(), len(index), table.cdf.data_ptr(),
+        index.below.data_ptr(), out.data_ptr(), _stream(out.device)))
+    return out
+
+
 def _train_1vsall_forward(model, ent, rel, triples, num_relations, loss, offset, l_norm, precision, dropout, out=None,
                           workspace=None):
     _require_cuda(ent, rel, triples)

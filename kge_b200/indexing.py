@@ -148,6 +148,32 @@ def filter_csr(index, vocab: int) -> Tuple[torch.Tensor, torch.Tensor, torch.Ten
     return keys_out[:nk].clone(), offs_out[: nk + 1].clone(), vals_out[: int(offs_out[nk])].clone(), mx.value
 
 
+def frequency_cdf(counts: torch.Tensor, smoothing: float) -> torch.Tensor:
+    """cdf [V+1] int64 (every entry <= 2^62): the exclusive prefix of the integer weights of frequency sampling,
+    q_x = round((counts[x] + smoothing) * 2^s) with the largest s that keeps their sum within 2^62
+    (b200kge_frequency_cdf_build).  ValueError for a negative count, a negative or non-finite smoothing, or all-zero
+    weights."""
+    c = _i64(counts).view(-1)
+    cdf = torch.empty((c.numel() + 1,), dtype=torch.int64)
+    _lib.check(_lib.load().b200kge_frequency_cdf_build(c.data_ptr(), c.numel(), float(smoothing), cdf.data_ptr()))
+    return cdf
+
+
+def frequency_below(cdf: torch.Tensor, offsets: torch.Tensor, values: torch.Tensor) -> Tuple[torch.Tensor, int, int]:
+    """(below [nnz] int64, number of keys, first key index or -1): for every value v_j of a key of a filter index
+    (filter_csr's offsets / values), the weight of the key's non-positives below v_j under `cdf`, and the keys whose
+    positives carry all the weight (b200kge_frequency_filter_build)."""
+    cdf, offs, vals = _i64(cdf).view(-1), _i64(offsets).view(-1), _i64(values).view(-1)
+    below = torch.empty_like(vals)
+    import ctypes as C
+
+    full, first = C.c_int64(0), C.c_int64(0)
+    _lib.check(_lib.load().b200kge_frequency_filter_build(
+        cdf.data_ptr(), cdf.numel() - 1, offs.data_ptr(), vals.data_ptr(), offs.numel() - 1, below.data_ptr(),
+        C.byref(full), C.byref(first)))
+    return below, full.value, first.value
+
+
 def sp_po_label_csr(triples: torch.Tensor, num_entities: int, sp_index: KvsAllIndex, po_index: KvsAllIndex,
                     ) -> Tuple[torch.Tensor, torch.Tensor]:
     """CSR over the [n, 2E] label / filter matrix of a batch of (s,p,o) triples: known objects of (s,p,?) in

@@ -37,11 +37,13 @@ import torch
 from kge.job.eval_entity_ranking import EntityRankingJob
 from kge.job.train_1vsAll import TrainingJob1vsAll
 from kge.job.train_KvsAll import TrainingJobKvsAll
+from kge.job.train import TrainingJob
 from kge.job.train_negative_sampling import TrainingJobNegativeSampling
 from kge.job import Job
 from kge.model.reciprocal_relations_model import ReciprocalRelationsModel
 from kge.util.loss import (BCEWithLogitsKgeLoss, KLDivWithSoftmaxKgeLoss, MarginRankingKgeLoss, SEKgeLoss,
                            SoftMarginKgeLoss)
+from kge.util.sampler import KgeSampler
 
 from .. import engine
 
@@ -335,6 +337,30 @@ class B200TrainingJobKvsAll(_DropoutKeys, _BatchSplit, TrainingJobKvsAll):
             result.backward_time += time.time()
 
 
+class B200FrequencySampler(KgeSampler):
+    """`negative_sampling.sampling_type: frequency` on the device route of B200TrainingJobNegativeSampling: the options
+    and filtering indexes of KgeSampler.__init__, plus the weights KgeFrequencySampler.__init__ defines
+    (sampler.py:762-780), kept as `counts[slot]` = bincount(train[:, slot]) and `smoothing` (w = counts + smoothing).
+    KgeFrequencySampler itself cannot be built on current torch (torch._multinomial_alias_setup is gone); the job draws
+    on the device (engine.sample_frequency and sample_frequency_filtered), so the host `_sample` refuses."""
+
+    def __init__(self, config, configuration_key, dataset):
+        super().__init__(config, configuration_key, dataset)
+        self.smoothing = float(self.get_option("frequency.smoothing"))
+        train = dataset.split(config.get("train.split"))
+        self.counts = []
+        for slot in (S, P, O):
+            vocab = int(self.vocabulary_size[slot])
+            c = torch.bincount(train[:, slot].long(), minlength=vocab)
+            if c.numel() != vocab:
+                raise ValueError(f"{config.get('train.split')} holds {SLOT_STR[slot]} ids outside [0, {vocab})")
+            self.counts.append(c)
+
+    def _sample(self, positive_triples, slot, num_samples):
+        raise NotImplementedError("frequency negative sampling is drawn on the device only: use "
+                                  "B200TrainingJobNegativeSampling with user.b200_device_sampling: true")
+
+
 class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNegativeSampling):
     """`TrainingJobNegativeSampling` (train_negative_sampling.py:103-164): per slot ONE kernel gathers the sampled
     rows and scores them, with the positive triple in column 0 — neither `[n*K, D]` gathers (`triple`
@@ -345,16 +371,28 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
     DataLoader workers only slice the triples, and no [n, K] id tensors travel host -> device
     (KgeUniformSampler._sample, sampler.py:588-596, is a CPU torch.randint).  `negative_sampling.filtering.<slot>` is
     served there too: the sampling kernel replaces positives of the filtering split with uniform non-positives
-    (engine.sample_uniform_filtered), from an index uploaded once when the job is created."""
+    (engine.sample_uniform_filtered), from an index uploaded once when the job is created.
+
+    `negative_sampling.sampling_type: frequency` (not shared) is served on this route only: the job builds
+    B200FrequencySampler instead of the reference's KgeFrequencySampler, uploads one weight table per sampled slot and
+    draws with engine.sample_frequency, or engine.sample_frequency_filtered for a filtered slot."""
 
     def __init__(self, config, dataset, parent_job=None, model=None, forward_only=False):
-        super().__init__(config, dataset, parent_job, model=model, forward_only=forward_only)
-        try:
-            want = bool(config.get("user.b200_device_sampling"))
-        except KeyError:
-            want = False
+        want = bool(_user_option(config, "b200_device_sampling", False))
+        if (want and config.get("negative_sampling.sampling_type") == "frequency"
+                and not config.get("negative_sampling.shared")):
+            # TrainingJobNegativeSampling.__init__ (train_negative_sampling.py:16-27) with the plugin's sampler in place
+            # of KgeSampler.create, which would build KgeFrequencySampler
+            TrainingJob.__init__(self, config, dataset, parent_job, model=model, forward_only=forward_only)
+            self._sampler = B200FrequencySampler(config, "negative_sampling", dataset)
+            self.type_str = "negative_sampling"
+        else:
+            super().__init__(config, dataset, parent_job, model=model, forward_only=forward_only)
         sm = self._sampler
-        self._device_sampling = bool(want and type(sm).__name__ == "KgeUniformSampler" and not sm.shared)
+        frequency = isinstance(sm, B200FrequencySampler)
+        self._device_sampling = bool(
+            want and (frequency or type(sm).__name__ == "KgeUniformSampler") and not sm.shared)
+        self._frequency = self._b200_frequency_tables() if frequency else {}
         self._filter_index = self._b200_filter_indexes() if self._device_sampling else {}
         self._sample_calls = 0
         if self.__class__ == B200TrainingJobNegativeSampling:
@@ -374,10 +412,12 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
         the sampler's filtering split (the index the sampler created, sampler.py:44-48), uploaded once.  A key whose
         positives cover the vocabulary is refused here: the reference's redraw loop would never end on it."""
         sm = self._sampler
+        filtered = [slot for slot in (S, P, O) if sm.filter_positives[slot] and sm.num_samples[slot] > 0]
+        if self._frequency and filtered and sm.filter_implementation == "fast":
+            # what KgeSampler._filter_and_resample_fast raises for every sampler but the uniform one (sampler.py:197-210)
+            raise NotImplementedError("Use filtering.implementation=standard for this sampler.")
         out = {}
-        for slot in (S, P, O):
-            if not sm.filter_positives[slot] or sm.num_samples[slot] <= 0:
-                continue
+        for slot in filtered:
             name = f"{sm.filtering_split}_{['po', 'so', 'sp'][slot]}_to_{SLOT_STR[slot]}"
             vocab = int(sm.vocabulary_size[slot])
             index = engine.FilterIndex(self.dataset.index(name), vocab, self.device)
@@ -385,8 +425,19 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
                 raise NotImplementedError(
                     f"negative_sampling.filtering.{SLOT_STR[slot]}: a key of {name} has all {vocab} ids as positives, "
                     "so no negative exists for it")
+            table = self._frequency.get(slot)
+            if table is not None and table.attach(index).full_keys:
+                raise NotImplementedError(
+                    f"negative_sampling.filtering.{SLOT_STR[slot]}: the positives of key {index.first_full_key} of "
+                    f"{name} carry all the frequency weight (smoothing {table.smoothing}), so no negative exists for it")
             out[slot] = index
         return out
+
+    def _b200_frequency_tables(self):
+        """{slot: engine.FrequencyTable} for every sampled slot: the sampler's counts and smoothing, uploaded once."""
+        sm = self._sampler
+        return {slot: engine.FrequencyTable(sm.counts[slot], sm.smoothing, self.device)
+                for slot in (S, P, O) if sm.num_samples[slot] > 0}
 
     def _device_negatives(self, n, slot, batch_index, triples):
         sm = self._sampler
@@ -394,7 +445,11 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
         offset = ((self.epoch * (1 << 24) + batch_index) << 2) | slot
         self._sample_calls += 1
         K, vocab = int(sm.num_samples[slot]), int(sm.vocabulary_size[slot])
-        index = self._filter_index.get(slot)
+        index, table = self._filter_index.get(slot), self._frequency.get(slot)
+        if table is not None:
+            if index is None:
+                return engine.sample_frequency(n, K, table, torch.initial_seed(), offset)
+            return engine.sample_frequency_filtered(n, K, table, torch.initial_seed(), offset, triples, slot, index)
         if index is None:
             return engine.sample_uniform(n, K, vocab, torch.initial_seed(), offset, self.device)
         # the dataset's own triples: with reciprocal relations the S slot is filtered on (p, o), as the reference's
