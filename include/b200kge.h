@@ -327,11 +327,14 @@ int b200kge_sample_frequency_filtered(uint64_t seed, uint64_t offset, int64_t vo
  *   score_sp(s, p): 0 = embed(s), 1 = embed(p), 2 = embed_all()       (entity, relation, entity table)
  *   score_po(p, o): 3 = embed_all(), 4 = embed(p), 5 = embed(o)       (entity table, relation, entity)
  * so the two directions use different masks on the candidate table and on p.  KvsAll (train_KvsAll.py:274-285) draws
- * streams 0-2 for its sp_ queries and 3-5 for its _po queries.
+ * streams 0-2 for its sp_ queries and 3-5 for its _po queries; its s_o queries (score_so(s, o), kge_model.py:727-747)
+ * draw three more, after streams 6-23 of negative sampling:
+ *   score_so(s, o): 24 = embed(s), 25 = embed(o), 26 = embed_all() of the relations  (entity, entity, relation table)
  *
  * Mask layout (never stored: the backward regenerates the forward's mask from the same key):
  *   element (row, k) of a draw over rows of width dim has elem = row * dim + k, where row is the GLOBAL row: the entity
- *   id for the table draws (2, 3), row_base + i for row i of the sub-batch's queries (0, 1, 4, 5);
+ *   id for the table draws (2, 3), the relation id for 26, row_base + i for row i of the sub-batch's queries (0, 1, 4,
+ *   5, 24, 25);
  *   Philox4x32-10 with key = seed (64 bits) and counter = ((stream << 46) | (elem >> 2), call), both 64-bit halves
  *   little-endian as four 32-bit words; the element takes output word elem & 3;
  *   kept iff word < floor((1 - p) * 2^32), kept value x * (1 / (1 - p)) in fp32.
@@ -342,6 +345,9 @@ int b200kge_sample_frequency_filtered(uint64_t seed, uint64_t offset, int64_t vo
 #define B200KGE_DROP_PO_TABLE 3
 #define B200KGE_DROP_PO_REL 4
 #define B200KGE_DROP_PO_ENT 5
+#define B200KGE_DROP_SO_S 24
+#define B200KGE_DROP_SO_O 25
+#define B200KGE_DROP_SO_TABLE 26
 
 typedef struct {
   float p_ent;      /* entity_embedder.dropout   */
@@ -575,6 +581,40 @@ int b200kge_score_1vsN_loss_csr_dropout(int model, int combine, int mask_dir, fl
                                         int64_t nnz, float label_smoothing, int loss_kind, float offset,
                                         const b200kge_dropout_t* drop, float* loss_out, float* row_loss_out,
                                         void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+
+/* KvsAll's s_o query type (relation prediction: train_KvsAll.py:251-254,278-281 with score_so, kge_model.py:727-747)
+ * for the dot family.  Row i is the pair (ent[s_idx[i]], ent[o_idx[i]]) scored against every relation r of rel; its
+ * labels are the relation ids csr_col[csr_off[i] .. csr_off[i+1]) (sorted; a repeated id counts as often as it
+ * appears).  There is no label smoothing: the reference never smooths the relation targets (train_KvsAll.py:263).
+ * The pair is folded into one query row Q_i (width K = the relation width: D, D/2 for CP, D^2 for RESCAL) with
+ * score(s_i, r, o_i) = Q_i . rel[r]:
+ *   DistMult s*o;  ComplEx [s_re*o_re + s_im*o_im | s_re*o_im - s_im*o_re];  SimplE 1/2 [s[:h]*o[h:] | s[h:]*o[:h]];
+ *   CP s[:h]*o[h:];  RESCAL Q[r*D + c] = s_r o_c (the row-major relation matrix).
+ * The relation table is then the candidate table of b200kge_score_1vsN_loss_csr's steps: on the pre-split tensor-core
+ * path (precision auto: 32 <= K <= 1024 and n >= 16) one fused pass scores, reduces and emits the listed scores;
+ * elsewhere the listed scores come from the row-wise triple kernel on (s_i, r, o_i).
+ *   *loss_out = sum_i loss(score row i, y_i) (BCE with offset | KL), row_loss_out (optional) the per-row terms.
+ * TransE and RotatE return B200KGE_ERR_UNSUPPORTED before any launch; l_norm is not used.
+ * drop != NULL: embedding dropout with the key's masks on streams 24 (s rows, p_ent), 25 (o rows, p_ent) and 26 (the
+ * relation table, p_rel), applied to masked copies of the operands.
+ * Workspace: b200kge_score_so_loss_csr_workspace_bytes(model, n, R, D, nnz, drop != NULL), R = rel->rows. */
+size_t b200kge_score_so_loss_csr_workspace_bytes(int model, int64_t n, int64_t R, int32_t D, int64_t nnz, int dropout);
+int b200kge_score_so_loss_csr(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                              const b200kge_rows_t* rel, const int64_t* s_idx, const int64_t* o_idx, int64_t n,
+                              const int64_t* csr_off, const int64_t* csr_col, int64_t nnz, int loss_kind, float offset,
+                              const b200kge_dropout_t* drop, float* loss_out, float* row_loss_out, void* workspace,
+                              size_t workspace_bytes, b200kge_stream_t stream);
+
+/* Backward of b200kge_score_so_loss_csr / batch_size under the same drop: d_ent [E, lde] and d_rel [R, ldr], both
+ * OVERWRITTEN.  Fold, recompute, G planes of [n, R] patched at the listed entries, dT = G^T Q stored into d_rel,
+ * dQ = G rel (split-K tensor-core GEMMs, as b200kge_score_1vsN_loss_csr_backward), then the fold's VJP added
+ * atomically into d_ent[s_i] and d_ent[o_i] (with dropout: masked with the forward's draws first).
+ * Workspace: b200kge_score_so_loss_csr_workspace_bytes (nnz is not used by the backward). */
+int b200kge_score_so_loss_csr_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                       const int64_t* s_idx, const int64_t* o_idx, int64_t n, const int64_t* csr_off,
+                                       const int64_t* csr_col, int loss_kind, float offset, int64_t batch_size,
+                                       const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
+                                       int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
 
 /* ---- Embedding dropout of the negative-sampling training step ------------------------------------------------------
  * Per slot (0 = S or 2 = O; the P slot is not served) and sub-batch, train_negative_sampling.py:139-148 makes six draws,

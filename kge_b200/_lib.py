@@ -143,6 +143,15 @@ SIGNATURES = {
                                                       C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_ns_score_dropout": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
                                            C.c_int64, C.c_int, _DP, C.c_void_p, C.c_int64, C.c_void_p]),
+    "b200kge_score_so_loss_csr_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32, C.c_int64,
+                                                               C.c_int]),
+    "b200kge_score_so_loss_csr": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_void_p, C.c_void_p, C.c_int64,
+                                            C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_float, _DP, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_score_so_loss_csr_backward": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_void_p, C.c_int64,
+                                                     C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int64, _DP,
+                                                     C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                                     C.c_size_t, C.c_void_p]),
 }
 
 #: negative-sampling scoring implementations of the dropout entry points (B200KGE_NS_*); "all" draws like "batch"

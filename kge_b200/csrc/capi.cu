@@ -977,6 +977,94 @@ int check_distance_pair(int pair_op) {
   return 0;
 }
 
+// Buffers of the CSR-label loss steps below: the label-free pass's label vector, the listed entries' selections and
+// scores (tot = nnz, plus n for KL's column-0 scores), the per-row terms and the finaliser's scalar and scratch.
+struct CsrBufs {
+  int64_t *lab, *qsel, *psel, *esel;
+  float *zpos, *fused, *rows, *total;
+  void* scratch;
+};
+bool take_csr_bufs(Arena& ws, int64_t n, int64_t nnz, int loss_kind, float* row_loss_out, CsrBufs& b) {
+  const int64_t tot = nnz + (loss_kind == B200KGE_LOSS_KL ? n : 0);
+  b.lab = (int64_t*)ws.take((size_t)n * 8);
+  b.qsel = (int64_t*)ws.take((size_t)tot * 8 + 8);
+  b.psel = (int64_t*)ws.take((size_t)tot * 8 + 8);
+  b.esel = (int64_t*)ws.take((size_t)tot * 8 + 8);
+  b.zpos = (float*)ws.take((size_t)tot * 4 + 8);
+  b.fused = (float*)ws.take((size_t)n * 4);
+  b.rows = row_loss_out ? row_loss_out : (float*)ws.take((size_t)n * 4);
+  b.total = (float*)ws.take(256);
+  b.scratch = ws.take(1024);
+  return b.lab && b.qsel && b.psel && b.esel && b.zpos && b.fused && b.rows && b.total && b.scratch;
+}
+
+// Steps 1 and 2 of a CSR-label KvsAll loss (b200kge_score_1vsN_loss_csr, b200kge_score_so_loss_csr) for the n query
+// rows of block B against its candidate table: b.fused[i] = the label-free row term, b.zpos = the scores of the listed
+// columns (and of column 0 for KL).  `roles` places the row-wise triple kernel's operands (row i of q and p, the
+// listed row of cand) as (s, p, o): B200KGE_SP_ (q, p, cand), B200KGE__PO (cand, p, q), ROLES_SO (q, cand, p).
+constexpr int ROLES_SO = 2;
+int csr_loss_terms(const Block& B, int model, int roles, float l_norm, int precision, const Rows& q, const Rows& p,
+                   const Rows& cand, const int64_t* csr_off, const int64_t* csr_col, int64_t nnz, int loss_kind,
+                   float offset, float* zsum, const CsrBufs& b, const Arena& ws, cudaStream_t st) {
+  const int64_t n = B.n, tot = nnz + (loss_kind == B200KGE_LOSS_KL ? n : 0);
+  int rc;
+  // 1. label-free fused pass: BCE with no label (index -1) -> sum_j softplus;  KL with the one-hot label at
+  //    column 0 -> lse_i - z_i0.  On the pre-split tensor-core path the SAME pass also emits the scores of the listed
+  //    columns (and z_i0) from its epilogue (per-thread cursor into the row's sorted CSR segment, tc_common.cuh):
+  //    DRAM traffic = table + queries + nnz * 12 bytes.
+  B2K_CUDA(cudaMemsetAsync(b.lab, loss_kind == B200KGE_LOSS_BCE ? 0xFF : 0, (size_t)n * 8, st));
+  bool emitted = false;
+  {
+    // zsum (label smoothing of the distance family): the CUDA-core pass also sums each row's scores
+    const int epi = (loss_kind == B200KGE_LOSS_BCE) ? (zsum ? EPI_BCE_ZSUM : EPI_BCE) : (zsum ? EPI_KL_ZSUM : EPI_KL);
+    for (int attempt = 0; attempt < 2; ++attempt) {
+      EpiParams P = empty_epi();
+      P.label_idx = b.lab;
+      P.offset = (loss_kind == B200KGE_LOSS_BCE) ? offset : 0.f;
+      P.zsum_part = zsum;
+      if (attempt == 0) {
+        P.csr_off = csr_off; P.csr_col = csr_col; P.csr_out = b.zpos; P.csr_nnz = nnz;
+        P.csr_extra = (loss_kind == B200KGE_LOSS_KL) ? 1 : 0;
+      }
+      int nch = 0;
+      float* part = nullptr;
+      Arena w2 = ws;
+      rc = run_block(B, l_norm, precision, epi, P, w2, st, &nch, &part);
+      if (rc == B200KGE_ERR_UNSUPPORTED && attempt == 0) continue;      // not the pre-split path: compose below
+      if (rc) return rc;
+      emitted = (attempt == 0);
+      if ((rc = launch_loss_finalize(loss_kind, part, nch, n, b.total, b.fused, 1.0f, 0, b.scratch, 0, st))) return rc;
+      break;
+    }
+  }
+  // 2. otherwise: scores of the listed columns (and of column 0 for KL) through the row-wise triple kernel
+  if (!emitted) {
+    if ((rc = launch_csr_expand(csr_off, csr_col, n, nnz, loss_kind == B200KGE_LOSS_KL ? 1 : 0, q.idx, p.idx, b.qsel,
+                                b.psel, b.esel, st))) return rc;
+    if (tot > 0) {
+      Rows Qs = q; Qs.idx = b.qsel; Qs.rows = tot;
+      Rows Ps = p; Ps.idx = b.psel; Ps.rows = tot;
+      Rows Cs = cand; Cs.idx = b.esel; Cs.rows = tot;
+      if (roles == B200KGE_SP_)      rc = launch_spo(model, l_norm, Qs, Ps, Cs, tot, b.zpos, 1, st);
+      else if (roles == B200KGE__PO) rc = launch_spo(model, l_norm, Cs, Ps, Qs, tot, b.zpos, 1, st);
+      else                           rc = launch_spo(model, l_norm, Qs, Cs, Ps, tot, b.zpos, 1, st);
+      if (rc) return rc;
+    }
+  }
+  return 0;
+}
+
+// Step 4: the per-row combination with labels y = a * count + b over m candidates, and the scalar
+int csr_loss_rows(int loss_kind, const int64_t* csr_off, const int64_t* csr_col, int64_t n, int64_t nnz, int64_t m,
+                  float label_smoothing, float offset, const float* zsum, int zch, const CsrBufs& b, float* loss_out,
+                  cudaStream_t st) {
+  const float a = 1.0f - label_smoothing, c = label_smoothing > 0.f ? 1.0f / (float)m : 0.f;
+  int rc;
+  if ((rc = launch_csr_rows(loss_kind, csr_off, csr_col, b.zpos, n, nnz, b.fused, zsum, zch, a, c, (float)m,
+                            loss_kind == B200KGE_LOSS_BCE ? offset : 0.f, b.rows, st))) return rc;
+  return launch_rows_sum(b.rows, n, 1.0f, loss_out, st);
+}
+
 size_t backward_block_bytes(int64_t nq, int64_t m, int64_t K, int64_t ldq) {
   const int64_t Ep = round_up(m, 64), Np = round_up(nq, 64);
   size_t b = (size_t)nq * round_up(m, 4) * 4 + 256;
@@ -1225,65 +1313,18 @@ int b200kge_score_1vsN_loss_csr(int model, int combine, float l_norm, int precis
   cudaStream_t st = (cudaStream_t)stream;
   if (n == 0 || cand->rows == 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
   Rows Q = to_rows(q), Pr = to_rows(p), C = to_rows(cand);
-  const int64_t m = C.rows, tot = nnz + (loss_kind == B200KGE_LOSS_KL ? n : 0);
+  const int64_t m = C.rows;
   Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
-  int64_t* lab = (int64_t*)ws.take((size_t)n * 8);
-  int64_t* qsel = (int64_t*)ws.take((size_t)tot * 8 + 8);
-  int64_t* psel = (int64_t*)ws.take((size_t)tot * 8 + 8);
-  int64_t* esel = (int64_t*)ws.take((size_t)tot * 8 + 8);
-  float* zpos = (float*)ws.take((size_t)tot * 4 + 8);
-  float* fused = (float*)ws.take((size_t)n * 4);
-  float* rows = row_loss_out ? row_loss_out : (float*)ws.take((size_t)n * 4);
-  float* total = (float*)ws.take(256);
-  void* scratch = ws.take(1024);
+  CsrBufs cb;
+  const bool bufs = take_csr_bufs(ws, n, nnz, loss_kind, row_loss_out, cb);
   // label smoothing needs sum_j z_ij: the distance family's CUDA-core pass below sums it per row and column chunk
   const bool zsum_fused = label_smoothing > 0.f && !dot;
   const int zch = zsum_fused ? pairwise_simt_nchunks(n, m) : 1;
   float* zsum = zsum_fused ? (float*)ws.take((size_t)n * zch * 4) : nullptr;
-  if (!lab || !qsel || !psel || !esel || !zpos || !fused || !rows || !total || !scratch || (zsum_fused && !zsum)) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
-  // 1. label-free fused pass: BCE with no label (index -1) -> sum_j softplus;  KL with the one-hot label at
-  //    column 0 -> lse_i - z_i0.  On the pre-split tensor-core path the SAME pass also emits the scores of the listed
-  //    columns (and z_i0) from its epilogue (per-thread cursor into the row's sorted CSR segment, tc_common.cuh):
-  //    DRAM traffic = table + queries + nnz * 12 bytes.
-  B2K_CUDA(cudaMemsetAsync(lab, loss_kind == B200KGE_LOSS_BCE ? 0xFF : 0, (size_t)n * 8, st));
-  bool emitted = false;
-  {
-    const int epi = (loss_kind == B200KGE_LOSS_BCE) ? (zsum_fused ? EPI_BCE_ZSUM : EPI_BCE)
-                                                    : (zsum_fused ? EPI_KL_ZSUM : EPI_KL);
-    for (int attempt = 0; attempt < 2; ++attempt) {
-      EpiParams P = empty_epi();
-      P.label_idx = lab;
-      P.offset = (loss_kind == B200KGE_LOSS_BCE) ? offset : 0.f;
-      P.zsum_part = zsum;
-      if (attempt == 0) {
-        P.csr_off = csr_off; P.csr_col = csr_col; P.csr_out = zpos; P.csr_nnz = nnz;
-        P.csr_extra = (loss_kind == B200KGE_LOSS_KL) ? 1 : 0;
-      }
-      Block B{model, combine, &Q, nullptr, &Pr, &C, n};
-      int nch = 0;
-      float* part = nullptr;
-      Arena w2 = ws;
-      rc = run_block(B, l_norm, precision, epi, P, w2, st, &nch, &part);
-      if (rc == B200KGE_ERR_UNSUPPORTED && attempt == 0) continue;      // not the pre-split path: compose below
-      if (rc) return rc;
-      emitted = (attempt == 0);
-      if ((rc = launch_loss_finalize(loss_kind, part, nch, n, total, fused, 1.0f, 0, scratch, 0, st))) return rc;
-      break;
-    }
-  }
-  // 2. otherwise: scores of the listed columns (and of column 0 for KL) through the row-wise triple kernel
-  if (!emitted) {
-    if ((rc = launch_csr_expand(csr_off, csr_col, n, nnz, loss_kind == B200KGE_LOSS_KL ? 1 : 0, Q.idx, Pr.idx, qsel, psel,
-                                esel, st))) return rc;
-    if (tot > 0) {
-      Rows Qs = Q; Qs.idx = qsel; Qs.rows = tot;
-      Rows Ps = Pr; Ps.idx = psel; Ps.rows = tot;
-      Rows Es = C; Es.idx = esel; Es.rows = tot;
-      if (combine == B200KGE_SP_) rc = launch_spo(model, l_norm, Qs, Ps, Es, tot, zpos, 1, st);
-      else                        rc = launch_spo(model, l_norm, Es, Ps, Qs, tot, zpos, 1, st);
-      if (rc) return rc;
-    }
-  }
+  if (!bufs || (zsum_fused && !zsum)) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
+  Block B{model, combine, &Q, nullptr, &Pr, &C, n};
+  if ((rc = csr_loss_terms(B, model, combine, l_norm, precision, Q, Pr, C, csr_off, csr_col, nnz, loss_kind, offset, zsum,
+                           cb, ws, st))) return rc;
   // 3. label smoothing: sum_j z_ij = Q_i . colsum(T)   (dot family)
   if (label_smoothing > 0.f && dot) {
     Folded f = folded_problem(model, combine, Q.dim, l_norm);
@@ -1295,11 +1336,7 @@ int b200kge_score_1vsN_loss_csr(int model, int combine, float l_norm, int precis
     if ((rc = launch_fold_queries(model, combine, Q, Pr, n, 0, Qf, ldq, st))) return rc;
     if ((rc = launch_row_score_sums(Qf, ldq, n, C.base + f.col_off, C.ld, m, f.K, cs, zsum, st))) return rc;
   }
-  // 4. per-row combination and the scalar
-  const float a = 1.0f - label_smoothing, b = label_smoothing > 0.f ? 1.0f / (float)m : 0.f;
-  if ((rc = launch_csr_rows(loss_kind, csr_off, csr_col, zpos, n, nnz, fused, zsum, zch, a, b, (float)m,
-                            loss_kind == B200KGE_LOSS_BCE ? offset : 0.f, rows, st))) return rc;
-  return launch_rows_sum(rows, n, 1.0f, loss_out, st);
+  return csr_loss_rows(loss_kind, csr_off, csr_col, n, nnz, m, label_smoothing, offset, zsum, zch, cb, loss_out, st);
 }
 
 }  // extern "C"
@@ -1669,6 +1706,194 @@ int b200kge_score_1vsN_loss_csr_backward(int model, int combine, int mask_dir, f
   }
   if ((rc = backward_block(model, E, R, n, combine, false, Q, ldq, f.col_off, f.K, g, d_ent, lde, dQ, ws, st))) return rc;
   return launch_unfold(model, E, R, tri, n, combine, dQ, ldq, d_ent, lde, d_rel, ldr, st);
+}
+
+}  // extern "C"
+
+// ==================================================================================================
+// KvsAll's s_o query type (relation prediction, train_KvsAll.py:251-254,278-281 with kge_model.py:727-747): every (s, o)
+// pair scored against the whole relation table.  The s_o fold (fold.cu) turns the pair into one query row
+// Q_i = fold_so(s_i, o_i) with score(s_i, r, o_i) = Q_i . rel[r], so the relation table is the candidate table of a
+// plain dot-product block (the DistMult pair problem of width K = relation_dim): the CSR-label loss steps and the
+// backward block of the entity query types run on it unchanged, and the unfold is the fold's VJP.
+namespace {
+
+int check_so_args(int model, const b200kge_rows_t* ent, const b200kge_rows_t* rel, const int64_t* s_idx,
+                  const int64_t* o_idx, int64_t n, const int64_t* csr_off, int loss_kind) {
+  if (!ent || !rel || ((!s_idx || !o_idx) && n > 0) || !csr_off) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (n < 0) { set_error("negative n"); return B200KGE_ERR_INVALID; }
+  int rc = check_tables(model, 1.0f, ent, rel); if (rc) return rc;
+  if (model == B200KGE_TRANSE || model == B200KGE_ROTATE) {
+    set_error("the s_o query type covers the dot family (ComplEx, DistMult, SimplE, CP, RESCAL)");
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  return check_loss_kind(loss_kind);
+}
+
+// the three s_o draws (include/b200kge.h): embed(s), embed(o) at mask rows row_base + i, embed_all() of the relations
+struct SoMasks { DropMask s, o, t; };
+SoMasks so_masks(const b200kge_dropout_t& d) {
+  return SoMasks{drop_mask(d.p_ent, d.seed, d.call, B200KGE_DROP_SO_S, d.row_base),
+                 drop_mask(d.p_ent, d.seed, d.call, B200KGE_DROP_SO_O, d.row_base),
+                 drop_mask(d.p_rel, d.seed, d.call, B200KGE_DROP_SO_TABLE, 0)};
+}
+
+int validate_so_dropout(const b200kge_dropout_t* drop, int64_t n, const b200kge_rows_t* ent, const b200kge_rows_t* rel) {
+  int rc = validate_dropout(drop, n, ent->rows, ent->dim, rel->dim);
+  return rc ? rc : validate_dropout(drop, n, rel->rows, rel->dim, rel->dim);    // the relation table draw
+}
+
+// masked copies Sm, Om [n, D] and Tm [R, K] (row strides = widths)
+struct SoMasked { float *Sm, *Om, *Tm; };
+bool take_so_masked(Arena& ws, int64_t n, const Rows& E, const Rows& R, SoMasked& m) {
+  m.Sm = (float*)ws.take((size_t)n * E.dim * 4);
+  m.Om = (float*)ws.take((size_t)n * E.dim * 4);
+  m.Tm = (float*)ws.take((size_t)R.rows * R.dim * 4);
+  return m.Sm && m.Om && m.Tm;
+}
+int gather_so_masked(const SoMasks& k, const Rows& E, const Rows& R, const int64_t* s_idx, const int64_t* o_idx,
+                     int64_t n, const SoMasked& m, Rows& S, Rows& O, Rows& T, cudaStream_t st) {
+  Rows ss = E; ss.idx = s_idx; ss.rows = n;
+  Rows os = E; os.idx = o_idx; os.rows = n;
+  int rc;
+  if ((rc = launch_dropout_gather(k.s, ss, m.Sm, E.dim, st))) return rc;
+  if ((rc = launch_dropout_gather(k.o, os, m.Om, E.dim, st))) return rc;
+  if ((rc = launch_dropout_gather(k.t, R, m.Tm, R.dim, st))) return rc;
+  S = Rows{m.Sm, nullptr, n, E.dim, E.dim};
+  O = Rows{m.Om, nullptr, n, E.dim, E.dim};
+  T = Rows{m.Tm, nullptr, R.rows, R.dim, R.dim};
+  return 0;
+}
+
+size_t so_masked_bytes(int64_t n, int64_t R, int32_t D, int64_t K) {
+  return 2 * (2 * (size_t)n * D * 4 + (size_t)R * K * 4 + 3 * 256);    // Sm, Om, Tm and their gradients
+}
+
+// The s_o loss on validated operands, n > 0: S, O the pair rows (index views of the entity table or masked copies),
+// T the relation table (or its masked copy)
+int so_loss_impl(int model, int precision, const Rows& S, const Rows& O, const Rows& T, int64_t n, const int64_t* csr_off,
+                 const int64_t* csr_col, int64_t nnz, int loss_kind, float offset, float* loss_out, float* row_loss_out,
+                 Arena ws, cudaStream_t st) {
+  const int64_t ldq = round_up(T.dim, 32);
+  float* Q = (float*)ws.take((size_t)n * ldq * 4);
+  CsrBufs cb;
+  if (!Q || !take_csr_bufs(ws, n, nnz, loss_kind, row_loss_out, cb)) {
+    set_error("workspace too small (see b200kge_score_so_loss_csr_workspace_bytes)");
+    return B200KGE_ERR_WORKSPACE;
+  }
+  int rc;
+  if ((rc = launch_fold_so(model, S, O, n, Q, ldq, st))) return rc;
+  // the pre-folded rows against the relation table: a plain dot-product block of width K (placeholder operands)
+  Rows ph{nullptr, nullptr, n, T.dim, T.dim};
+  Block B{B200KGE_DISTMULT, B200KGE_SP_, &ph, nullptr, &ph, &T, n};
+  B.Qpre = Q;
+  if ((rc = csr_loss_terms(B, model, ROLES_SO, 1.0f, precision, S, O, T, csr_off, csr_col, nnz, loss_kind, offset,
+                           nullptr, cb, ws, st))) return rc;
+  return csr_loss_rows(loss_kind, csr_off, csr_col, n, nnz, T.rows, 0.f, offset, nullptr, 1, cb, loss_out, st);
+}
+
+// Its backward: d_T [R, ldt] OVERWRITTEN with dT = G^T Q, the pair rows' gradients ADDED into dS[s_dst[i]], dO[o_dst[i]]
+int so_backward_impl(int model, const Rows& S, const Rows& O, const Rows& T, int64_t n, const int64_t* csr_off,
+                     const int64_t* csr_col, int loss_kind, float offset, int64_t batch_size, float* dS, int64_t lds,
+                     const int64_t* s_dst, float* dO, int64_t ldo, const int64_t* o_dst, float* dT, int64_t ldt,
+                     Arena ws, cudaStream_t st) {
+  const int K = T.dim;
+  const int64_t ldq = round_up(K, 32);
+  float* Q = (float*)ws.take((size_t)n * ldq * 4);
+  float* dQ = (float*)ws.take((size_t)n * ldq * 4);
+  if (!Q || !dQ) { set_error("workspace too small (see b200kge_score_so_loss_csr_workspace_bytes)"); return B200KGE_ERR_WORKSPACE; }
+  int rc;
+  if ((rc = launch_fold_so(model, S, O, n, Q, ldq, st))) return rc;
+  // no label smoothing: the reference never smooths the relation targets (train_KvsAll.py:263)
+  const GradSpec g = csr_grad(nullptr, csr_off, csr_col, 0.f, T.rows, batch_size, loss_kind, offset);
+  if ((rc = backward_block(B200KGE_DISTMULT, T, T, n, B200KGE_SP_, false, Q, ldq, 0, K, g, dT, ldt, dQ, ws, st))) return rc;
+  return launch_unfold_so(model, S, O, n, dQ, ldq, dS, lds, s_dst, dO, ldo, o_dst, st);
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t b200kge_score_so_loss_csr_workspace_bytes(int model, int64_t n, int64_t R, int32_t D, int64_t nnz, int dropout) {
+  const int64_t K = relation_dim(model, D), ldq = round_up(K, 32), tot = nnz + n;
+  const size_t fwd = (size_t)n * ldq * 4 + b200kge_workspace_bytes(B200KGE_DISTMULT, n, R, (int32_t)K, 0) +
+                     (size_t)n * 8 + 3 * ((size_t)tot * 8 + 256) + (size_t)tot * 4 + 3 * ((size_t)n * 4 + 256) + 2048;
+  const size_t bwd = 2 * ((size_t)n * ldq * 4 + 256) + backward_block_bytes(n, R, K, ldq) + 1024;
+  return (fwd > bwd ? fwd : bwd) + (dropout ? so_masked_bytes(n, R, D, K) : 0);
+}
+
+int b200kge_score_so_loss_csr(int model, float l_norm, int precision, const b200kge_rows_t* ent,
+                              const b200kge_rows_t* rel, const int64_t* s_idx, const int64_t* o_idx, int64_t n,
+                              const int64_t* csr_off, const int64_t* csr_col, int64_t nnz, int loss_kind, float offset,
+                              const b200kge_dropout_t* drop, float* loss_out, float* row_loss_out, void* workspace,
+                              size_t workspace_bytes, b200kge_stream_t stream) {
+  (void)l_norm;                                  // the dot family scores without a norm
+  int rc = check_so_args(model, ent, rel, s_idx, o_idx, n, csr_off, loss_kind); if (rc) return rc;
+  if ((!csr_col && nnz > 0) || !loss_out || nnz < 0) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (drop && (rc = validate_so_dropout(drop, n, ent, rel))) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n == 0 || rel->rows == 0) { B2K_CUDA(cudaMemsetAsync(loss_out, 0, 4, st)); return 0; }
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  const Rows E = to_rows(ent), R = to_rows(rel);
+  if (!drop) {
+    Rows S = E; S.idx = s_idx; S.rows = n;
+    Rows O = E; O.idx = o_idx; O.rows = n;
+    return so_loss_impl(model, precision, S, O, R, n, csr_off, csr_col, nnz, loss_kind, offset, loss_out, row_loss_out,
+                        ws, st);
+  }
+  SoMasked m;
+  if (!take_so_masked(ws, n, E, R, m)) {
+    set_error("workspace too small (see b200kge_score_so_loss_csr_workspace_bytes)");
+    return B200KGE_ERR_WORKSPACE;
+  }
+  Rows S, O, T;
+  if ((rc = gather_so_masked(so_masks(*drop), E, R, s_idx, o_idx, n, m, S, O, T, st))) return rc;
+  return so_loss_impl(model, precision, S, O, T, n, csr_off, csr_col, nnz, loss_kind, offset, loss_out, row_loss_out,
+                      rest_of(ws), st);
+}
+
+int b200kge_score_so_loss_csr_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                                       const int64_t* s_idx, const int64_t* o_idx, int64_t n, const int64_t* csr_off,
+                                       const int64_t* csr_col, int loss_kind, float offset, int64_t batch_size,
+                                       const b200kge_dropout_t* drop, float* d_ent, int64_t lde, float* d_rel,
+                                       int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+  (void)l_norm;
+  int rc = check_so_args(model, ent, rel, s_idx, o_idx, n, csr_off, loss_kind); if (rc) return rc;
+  if (!d_ent || !d_rel) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (batch_size <= 0) { set_error("batch_size must be positive"); return B200KGE_ERR_INVALID; }
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
+  if (drop && (rc = validate_so_dropout(drop, n, ent, rel))) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const Rows E = to_rows(ent), R = to_rows(rel);
+  B2K_CUDA(cudaMemsetAsync(d_ent, 0, (size_t)E.rows * lde * 4, st));
+  B2K_CUDA(cudaMemsetAsync(d_rel, 0, (size_t)R.rows * ldr * 4, st));
+  if (n == 0 || R.rows == 0) return 0;
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  if (!drop) {
+    Rows S = E; S.idx = s_idx; S.rows = n;
+    Rows O = E; O.idx = o_idx; O.rows = n;
+    return so_backward_impl(model, S, O, R, n, csr_off, csr_col, loss_kind, offset, batch_size, d_ent, lde, s_idx, d_ent,
+                            lde, o_idx, d_rel, ldr, ws, st);
+  }
+  // the masked copies' gradients land in row i of dSm / dOm and in dTm; then masked with the same draws and added
+  SoMasked m;
+  float* dSm = (float*)ws.take((size_t)n * E.dim * 4);
+  float* dOm = (float*)ws.take((size_t)n * E.dim * 4);
+  float* dTm = (float*)ws.take((size_t)R.rows * R.dim * 4);
+  if (!take_so_masked(ws, n, E, R, m) || !dSm || !dOm || !dTm) {
+    set_error("workspace too small (see b200kge_score_so_loss_csr_workspace_bytes)");
+    return B200KGE_ERR_WORKSPACE;
+  }
+  const SoMasks k = so_masks(*drop);
+  Rows S, O, T;
+  if ((rc = gather_so_masked(k, E, R, s_idx, o_idx, n, m, S, O, T, st))) return rc;
+  B2K_CUDA(cudaMemsetAsync(dSm, 0, (size_t)n * E.dim * 4, st));
+  B2K_CUDA(cudaMemsetAsync(dOm, 0, (size_t)n * E.dim * 4, st));
+  if ((rc = so_backward_impl(model, S, O, T, n, csr_off, csr_col, loss_kind, offset, batch_size, dSm, E.dim, nullptr, dOm,
+                             E.dim, nullptr, dTm, R.dim, rest_of(ws), st))) return rc;
+  if ((rc = launch_dropout_add_cols(k.t, dTm, R.dim, R.rows, R.dim, 0, R.dim, d_rel, ldr, st))) return rc;
+  if ((rc = launch_dropout_scatter(k.s, dSm, E.dim, n, E.dim, s_idx, d_ent, lde, st))) return rc;
+  return launch_dropout_scatter(k.o, dOm, E.dim, n, E.dim, o_idx, d_ent, lde, st);
 }
 
 }  // extern "C"

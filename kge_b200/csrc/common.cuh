@@ -409,6 +409,11 @@ __device__ __forceinline__ float finalize_row(const float* __restrict__ part, in
 // Internal kernels' host launchers (one per .cu file).
 int launch_fold_queries(int model, int combine, const Rows& q, const Rows& p, int64_t n,
                         int64_t row0, float* Q, int64_t ldq, cudaStream_t st);
+// s_o fold of the dot family (fold.cu): Q [n, ldq] with score(s_i, r, o_i) = Q_i . rel[r][0 : relation_dim(model, D)]
+int launch_fold_so(int model, const Rows& s, const Rows& o, int64_t n, float* Q, int64_t ldq, cudaStream_t st);
+// its VJP: dQ row i ADDED into dS[s_dst[i]] and dO[o_dst[i]] (a NULL index array: row i)
+int launch_unfold_so(int model, const Rows& s, const Rows& o, int64_t n, const float* dQ, int64_t ldq, float* dS,
+                     int64_t lds, const int64_t* s_dst, float* dO, int64_t ldo, const int64_t* o_dst, cudaStream_t st);
 // one launch: unpack triples [n,3], fold sp_ rows (0..n) and _po rows (n..2n) into Q, write the
 // stacked labels [o ; s] and zero the finalisation ticket.  num_rel > 0 (reciprocal relations): rows n..2n fold
 // (o, p + num_rel) with the sp_ fold instead

@@ -132,6 +132,110 @@ int launch_fold_queries(int model, int combine, const Rows& q, const Rows& p, in
   return 0;
 }
 
+// s_o fold (relation prediction): Q row i such that score(s_i, r, o_i) = Q_i . rel[r][0:K] for every relation r.
+//   DistMult s*o   ComplEx [s_re*o_re + s_im*o_im | s_re*o_im - s_im*o_re]   SimplE 1/2 [s_h*o_t | s_t*o_h]
+//   CP s[:h]*o[h:] (K = h)   RESCAL Q[r*D + c] = s_r o_c (K = D^2, the row-major p.view(D, D) of rescal.py)
+template <int MODEL>
+__global__ void __launch_bounds__(128)
+fold_so_kernel(Rows S, Rows O, float* __restrict__ Q, int64_t ldq, int K) {
+  const int64_t i = blockIdx.x;
+  const float* __restrict__ s = S.row(i);
+  const float* __restrict__ o = O.row(i);
+  const int D = S.dim, h = D >> 1;
+  float* __restrict__ q = Q + i * ldq;
+  if constexpr (MODEL == B200KGE_RESCAL) {
+    for (int e = threadIdx.x; e < K; e += blockDim.x) {
+      const int r = e / D;
+      q[e] = s[r] * o[e - r * D];
+    }
+  } else {
+    for (int k = threadIdx.x; k < K; k += blockDim.x) q[k] = fold_so_element<MODEL>(s, o, k, h);
+  }
+  for (int64_t k = K + threadIdx.x; k < ldq; k += blockDim.x) q[k] = 0.f;
+}
+
+// The VJP of fold_so_kernel: row i's dQ [K] ADDED (atomically: pairs share entities) into dS[s_dst[i]] and
+// dO[o_dst[i]] (NULL index: row i).
+template <int MODEL>
+__global__ void __launch_bounds__(128)
+unfold_so_kernel(Rows S, Rows O, const float* __restrict__ dQ, int64_t ldq, float* __restrict__ dS, int64_t lds,
+                 const int64_t* __restrict__ s_dst, float* __restrict__ dO, int64_t ldo,
+                 const int64_t* __restrict__ o_dst) {
+  const int64_t i = blockIdx.x;
+  const float* __restrict__ s = S.row(i);
+  const float* __restrict__ o = O.row(i);
+  const float* __restrict__ g = dQ + i * ldq;
+  float* ds = dS + (s_dst ? s_dst[i] : i) * lds;
+  float* dO_row = dO + (o_dst ? o_dst[i] : i) * ldo;
+  const int D = S.dim, h = D >> 1;
+  if constexpr (MODEL == B200KGE_RESCAL) {
+    // d_s[r] = sum_c dQ[r, c] o_c: one warp per r;  d_o[c] = sum_r dQ[r, c] s_r: one thread per c
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+    for (int r = warp; r < D; r += nw) {
+      float acc = 0.f;
+      for (int c = lane; c < D; c += 32) acc = fmaf(g[(int64_t)r * D + c], o[c], acc);
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+      if (lane == 0) atomicAdd(ds + r, acc);
+    }
+    for (int c = threadIdx.x; c < D; c += blockDim.x) {
+      float acc = 0.f;
+      for (int r = 0; r < D; ++r) acc = fmaf(g[(int64_t)r * D + c], s[r], acc);
+      atomicAdd(dO_row + c, acc);
+    }
+  } else {
+    for (int k = threadIdx.x; k < D; k += blockDim.x) {
+      if constexpr (MODEL == B200KGE_CP) {      // s[:h] pairs with o[h:]
+        if (k < h) atomicAdd(ds + k, g[k] * o[k + h]);
+        else       atomicAdd(dO_row + k, g[k - h] * s[k - h]);
+      } else {
+        float gs, go;
+        if constexpr (MODEL == B200KGE_COMPLEX) {
+          const int kk = (k < h) ? k : k - h;
+          const float g_re = g[kk], g_im = g[kk + h];
+          if (k < h) { gs = g_re * o[k] + g_im * o[k + h];  go = g_re * s[k] - g_im * s[k + h]; }
+          else       { gs = g_re * o[k] - g_im * o[kk];     go = g_re * s[k] + g_im * s[kk]; }
+        } else if constexpr (MODEL == B200KGE_DISTMULT) {
+          gs = g[k] * o[k]; go = g[k] * s[k];
+        } else {  // SIMPLE
+          const int pk = (k < h) ? k + h : k - h;   // the partner column of k in the other half
+          gs = 0.5f * g[k] * o[pk]; go = 0.5f * g[pk] * s[pk];
+        }
+        atomicAdd(ds + k, gs);
+        atomicAdd(dO_row + k, go);
+      }
+    }
+  }
+}
+
+int launch_fold_so(int model, const Rows& s, const Rows& o, int64_t n, float* Q, int64_t ldq, cudaStream_t st) {
+  if (n == 0) return 0;
+  const int K = relation_dim(model, s.dim);
+#define B2K_FOLD_SO(M) case M: fold_so_kernel<M><<<(unsigned)n, 128, 0, st>>>(s, o, Q, ldq, K); break;
+  switch (model) {
+    B2K_FOLD_SO(B200KGE_COMPLEX) B2K_FOLD_SO(B200KGE_DISTMULT) B2K_FOLD_SO(B200KGE_SIMPLE) B2K_FOLD_SO(B200KGE_CP)
+    B2K_FOLD_SO(B200KGE_RESCAL)
+    default: set_error("the s_o fold covers the dot family only (model %d)", model); return B200KGE_ERR_UNSUPPORTED;
+  }
+#undef B2K_FOLD_SO
+  B2K_LAUNCH_CHECK("fold_so_kernel");
+  return 0;
+}
+
+int launch_unfold_so(int model, const Rows& s, const Rows& o, int64_t n, const float* dQ, int64_t ldq, float* dS,
+                     int64_t lds, const int64_t* s_dst, float* dO, int64_t ldo, const int64_t* o_dst, cudaStream_t st) {
+  if (n == 0) return 0;
+#define B2K_UNFOLD_SO(M) case M: unfold_so_kernel<M><<<(unsigned)n, 128, 0, st>>>(s, o, dQ, ldq, dS, lds, s_dst, dO, ldo, o_dst); break;
+  switch (model) {
+    B2K_UNFOLD_SO(B200KGE_COMPLEX) B2K_UNFOLD_SO(B200KGE_DISTMULT) B2K_UNFOLD_SO(B200KGE_SIMPLE) B2K_UNFOLD_SO(B200KGE_CP)
+    B2K_UNFOLD_SO(B200KGE_RESCAL)
+    default: set_error("the s_o unfold covers the dot family only (model %d)", model); return B200KGE_ERR_UNSUPPORTED;
+  }
+#undef B2K_UNFOLD_SO
+  B2K_LAUNCH_CHECK("unfold_so_kernel");
+  return 0;
+}
+
 // Gather candidate rows (index subset) into a dense [m, ldd] block holding only the K columns the
 // pair op reads; used by the tensor-core path, whose TMA loads need a regular 2-D table.
 __global__ void __launch_bounds__(256)

@@ -36,6 +36,23 @@ __device__ __forceinline__ float fold_element(bool sp, const float* __restrict__
   return v;
 }
 
+// q[k] of the s_o fold (relation prediction, kge_model.py:727-747): score(s, r, o) = q . rel[r][0:K] with the
+// spo_kernel formulas (rowwise.cu) regrouped around the relation row.  Not RESCAL (fold_so_kernel).  h = D/2.
+template <int MODEL>
+__device__ __forceinline__ float fold_so_element(const float* __restrict__ s, const float* __restrict__ o, int k, int h) {
+  if constexpr (MODEL == B200KGE_COMPLEX) {
+    const int kk = (k < h) ? k : k - h;
+    const float s_re = s[kk], s_im = s[kk + h], o_re = o[kk], o_im = o[kk + h];
+    return (k < h) ? (s_re * o_re + s_im * o_im) : (s_re * o_im - s_im * o_re);
+  } else if constexpr (MODEL == B200KGE_DISTMULT) {
+    return s[k] * o[k];
+  } else if constexpr (MODEL == B200KGE_SIMPLE) {
+    return 0.5f * s[k] * o[k < h ? k + h : k - h];
+  } else {  // CP: K = h
+    return s[k] * o[k + h];
+  }
+}
+
 // RESCAL fold for one row by a whole CTA: sh_a holds the entity row (length D) in shared memory,
 // emit(k, value) receives q[k].
 template <class Emit>

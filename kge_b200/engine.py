@@ -107,7 +107,7 @@ class DropoutKey(NamedTuple):
 
 def dropout_mask(p: float, seed: int, call: int, stream: int, rows: int, dim: int, row_base: int = 0,
                  device="cuda") -> torch.Tensor:
-    """The keep mask [rows, dim] (uint8) of draw `stream` (0-5, include/b200kge.h) over global rows
+    """The keep mask [rows, dim] (uint8) of draw `stream` (0-5 and 24-26, include/b200kge.h) over global rows
     [row_base, row_base + rows)."""
     out = torch.empty((rows, dim), dtype=torch.uint8, device=device)
     _require_cuda(out)
@@ -954,3 +954,52 @@ def score_1vsN_loss_csr(model: str, combine: str, q_tab, rel, cand_tab, csr_offs
         n, offs.data_ptr(), cols.data_ptr() if nnz else None, nnz, label_smoothing, LOSS[loss], offset, out.data_ptr(),
         rows.data_ptr() if rows is not None else None, ws.data_ptr(), ws.numel(), _stream(dev)))
     return (out, rows) if return_rows else out
+
+
+def _so_workspace(lib, model, n, ent, rel, nnz, dropout, dev) -> torch.Tensor:
+    return torch.empty(lib.b200kge_score_so_loss_csr_workspace_bytes(MODELS[model], n, rel.shape[0], ent.shape[1], nnz,
+                                                                     0 if dropout is None else 1),
+                       dtype=torch.uint8, device=dev)
+
+
+def score_so_loss_csr(model: str, ent, rel, s, o, csr_offsets, csr_cols, loss: str = "kl", offset: float = 0.0,
+                      precision: str = "auto", return_rows: bool = False, dropout: Optional["DropoutKey"] = None):
+    """KvsAll loss of the s_o query type (sum over rows; relation prediction, train_KvsAll.py:251-254 with score_so): the
+    pairs (ent[s_i], ent[o_i]) against every relation, CSR labels = relation ids, no label smoothing.  With `dropout`
+    the three s_o draws (streams 24-26) are applied.  See b200kge_score_so_loss_csr; the dot family only."""
+    _require_cuda(ent, rel, csr_offsets, csr_cols)
+    lib, k = _lib.load(), _Keep()
+    re_, rr = k.rows(ent), k.rows(rel)
+    si, oi, offs, cols = _i64(s), _i64(o), _i64(csr_offsets), _i64(csr_cols)
+    n, nnz = si.numel(), int(cols.numel())
+    dev = ent.device
+    out = torch.empty((), dtype=torch.float32, device=dev)
+    rows = torch.empty(n, dtype=torch.float32, device=dev) if return_rows else None
+    ws = _so_workspace(lib, model, n, ent, rel, nnz, dropout, dev)
+    _lib.check(lib.b200kge_score_so_loss_csr(
+        MODELS[model], 1.0, PREC[precision], C.byref(re_), C.byref(rr), si.data_ptr(), oi.data_ptr(), n, offs.data_ptr(),
+        cols.data_ptr() if nnz else None, nnz, LOSS[loss], offset, None if dropout is None else C.byref(dropout.struct()),
+        out.data_ptr(), rows.data_ptr() if rows is not None else None, ws.data_ptr(), ws.numel(), _stream(dev)))
+    return (out, rows) if return_rows else out
+
+
+def score_so_loss_csr_backward(model: str, ent, rel, s, o, csr_offsets, csr_cols, loss: str = "kl",
+                               offset: float = 0.0, batch_size: Optional[int] = None,
+                               dropout: Optional["DropoutKey"] = None):
+    """(d_ent, d_rel) of score_so_loss_csr(...) / batch_size (fresh tensors), with the forward's dropout masks when
+    `dropout` is the forward's key."""
+    _require_cuda(ent, rel, csr_offsets, csr_cols)
+    lib, k = _lib.load(), _Keep()
+    re_, rr = k.rows(ent), k.rows(rel)
+    si, oi, offs, cols = _i64(s), _i64(o), _i64(csr_offsets), _i64(csr_cols)
+    n = si.numel()
+    dev = ent.device
+    d_ent = torch.empty_like(_f32(ent))
+    d_rel = torch.empty_like(_f32(rel))
+    ws = _so_workspace(lib, model, n, ent, rel, int(cols.numel()), dropout, dev)
+    _lib.check(lib.b200kge_score_so_loss_csr_backward(
+        MODELS[model], 1.0, C.byref(re_), C.byref(rr), si.data_ptr(), oi.data_ptr(), n, offs.data_ptr(),
+        cols.data_ptr() if cols.numel() else None, LOSS[loss], offset, batch_size or n,
+        None if dropout is None else C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(),
+        d_rel.stride(0), ws.data_ptr(), ws.numel(), _stream(dev)))
+    return d_ent, d_rel

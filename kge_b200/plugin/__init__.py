@@ -227,7 +227,8 @@ def _install_embedder_kernels(emb):
 
 class _KvsAllLossFn(torch.autograd.Function):
     """KvsAll loss of one query type with CSR labels / batch_size: forward = fused score + loss with the CSR consumed in
-    the epilogue; backward = the gradient kernels (b200kge_score_1vsN_loss_csr_backward).  With a dropout key both run
+    the epilogue; backward = the gradient kernels (b200kge_score_1vsN_loss_csr_backward; for combine "s_o" the pairs
+    (a, p) = (s, o) against the relation table, b200kge_score_so_loss_csr and its backward).  With a dropout key both run
     the dropout forms (b200kge_score_1vsN_loss_csr_dropout, the backward with its dropout key) under the same masks."""
 
     @staticmethod
@@ -237,6 +238,9 @@ class _KvsAllLossFn(torch.autograd.Function):
         ctx.save_for_backward(ent_w, rel_w, a, p, offs, cols)
         ln, prec = model._b200_args()
         kw = {} if dropout is None else {"dropout": dropout}
+        if combine == "s_o":      # a = s, p = o; the relation targets are never smoothed
+            return engine.score_so_loss_csr(model._b200_name, ent_w.detach(), rel_w.detach(), a, p, offs, cols, loss,
+                                            offset, prec, **kw) / batch_size
         if dropout_streams is not None:
             kw["dropout_streams"] = dropout_streams
         return engine.score_1vsN_loss_csr(model._b200_name, combine, ent_w.detach(), rel_w.detach(), ent_w.detach(), offs,
@@ -247,6 +251,10 @@ class _KvsAllLossFn(torch.autograd.Function):
         ent_w, rel_w, a, p, offs, cols = ctx.saved_tensors
         model, combine, loss, offset, smoothing, batch_size, dropout, dropout_streams = ctx.args
         kw = {} if dropout is None else {"dropout": dropout}
+        if combine == "s_o":
+            d_ent, d_rel = engine.score_so_loss_csr_backward(model._b200_name, ent_w.detach(), rel_w.detach(), a, p, offs,
+                                                             cols, loss, offset, batch_size, **kw)
+            return (d_ent * g, d_rel * g) + (None,) * 12
         if dropout_streams is not None:
             kw["dropout_streams"] = dropout_streams
         if model._b200_name in ("transe", "rotate"):
@@ -516,10 +524,14 @@ class _B200ModelMixin:
         """Sum over rows of the KvsAll loss with CSR multi-hot labels (train_KvsAll.py:242-294); forward only.
         `dropout` (an engine.DropoutKey) applies embedding dropout with the masks of that key, drawn on the streams of
         query type `dropout_streams` (default: `combine`'s; a reciprocal-relations _po query is the sp_ fold of
-        (o, p + R) on the _po streams)."""
+        (o, p + R) on the _po streams).  combine "s_o": the pairs (a, p) = (s, o) against every relation (relation
+        ids as labels, no smoothing; see b200_kvsall_so_ok)."""
         ent, rel = self._b200_tables()
         ln, prec = self._b200_args()
         kw = {} if dropout is None else {"dropout": dropout}
+        if combine == "s_o":
+            return engine.score_so_loss_csr(self._b200_name, ent, rel, a, p, csr_offsets, csr_cols, loss, offset, prec,
+                                            **kw)
         if dropout is not None and dropout_streams is not None:
             kw["dropout_streams"] = dropout_streams
         return engine.score_1vsN_loss_csr(self._b200_name, combine, ent, rel, ent, csr_offsets, csr_cols, a, p,
@@ -535,6 +547,12 @@ class _B200ModelMixin:
         if self.b200_backward != "native" or not self._b200_native_family():
             return False
         return dropout or self._b200_name not in ("transe", "rotate")
+
+    def b200_kvsall_so_ok(self):
+        """The s_o query type has fused forward and gradient kernels for the dot family, at the precisions of the
+        entity-ranking job (auto, fp32, f16x3), with the native backward.  TransE and RotatE have no s_o fold."""
+        return (self.b200_backward == "native" and self._b200_name in ("complex", "distmult", "simple", "cp", "rescal")
+                and self._b200_args()[1] in ("auto", "fp32", "f16x3"))
 
     def loss_kvsall_train(self, combine, a, p, csr_offsets, csr_cols, loss, offset, label_smoothing, batch_size,
                           dropout=None, dropout_streams=None):

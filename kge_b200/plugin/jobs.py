@@ -255,7 +255,8 @@ class B200TrainingJob1vsAll(_DropoutKeys, _BatchSplit, TrainingJob1vsAll):
 class B200TrainingJobKvsAll(_DropoutKeys, _BatchSplit, TrainingJobKvsAll):
     """`TrainingJobKvsAll` (train_KvsAll.py:205-294): per query type one fused score+loss call that consumes the
     batch's label coordinates as CSR (no dense [n, E] label matrix: job/util.py:32-60 + `.to_dense()`,
-    train_KvsAll.py:242-266 are not executed)."""
+    train_KvsAll.py:242-266 are not executed).  The s_o query type (relation prediction) is served for the dot family
+    (model.b200_kvsall_so_ok) against the relation table; otherwise a job with s_o keeps the reference step."""
 
     def __init__(self, config, dataset, parent_job=None, model=None, forward_only=False):
         super().__init__(config, dataset, parent_job, model=model, forward_only=forward_only)
@@ -273,12 +274,14 @@ class B200TrainingJobKvsAll(_DropoutKeys, _BatchSplit, TrainingJobKvsAll):
         rates = None
         if model is None:
             model, rates = _dropout_model(target)
-        qtypes = [q for q in self.query_types]
-        if (model is None or kind is None or "s_o" in qtypes or not model.b200_csr_labels_ok(self.label_smoothing)
+        # s_o: the dot family's relation-candidate kernels; a reciprocal-relations model has no score_so
+        # (reciprocal_relations_model.py), so its reference step raises before anything is computed
+        so_ok = "s_o" not in self.query_types or (recip is None and model is not None and model.b200_kvsall_so_ok())
+        if (model is None or kind is None or not so_ok or not model.b200_csr_labels_ok(self.label_smoothing)
                 or (not self.is_forward_only and not model.b200_kvsall_native_backward_ok(rates is not None))):
             return super()._process_subbatch(batch_index, batch, subbatch_slice, result)
         batch_size = result.size
-        # one key per sub-batch: the sp_ and _po query types draw disjoint mask streams under it
+        # one key per sub-batch: the sp_, _po and s_o query types draw disjoint mask streams under it
         kw = {} if rates is None else {"dropout": self._b200_dropout_key(rates, batch_index, subbatch_slice)}
 
         result.prepare_time -= time.time()
@@ -312,9 +315,12 @@ class B200TrainingJobKvsAll(_DropoutKeys, _BatchSplit, TrainingJobKvsAll):
             result.prepare_time += time.time()
 
             result.forward_time -= time.time()
-            # sp_ queries are (s, p) pairs, _po queries are (p, o) pairs (indexing.py:197-235)
-            qkw = kw
-            if query_type == "sp_":
+            # sp_ queries are (s, p) pairs, _po queries are (p, o) pairs, s_o queries (s, o) pairs (indexing.py:197-235)
+            qkw, smoothing = kw, self.label_smoothing
+            if query_type == "s_o":
+                # relation targets are never smoothed (train_KvsAll.py:263)
+                combine, ent_idx, rel_idx, smoothing = "s_o", queries[examples, 0], queries[examples, 1], 0.0
+            elif query_type == "sp_":
                 combine, ent_idx, rel_idx = "sp_", queries[examples, 0], queries[examples, 1]
             elif recip is not None:
                 # reciprocal relations: the sp_ query (o, p + R), masks on the _po streams
@@ -325,10 +331,10 @@ class B200TrainingJobKvsAll(_DropoutKeys, _BatchSplit, TrainingJobKvsAll):
                 combine, ent_idx, rel_idx = "_po", queries[examples, 1], queries[examples, 0]
             if self.is_forward_only:
                 loss_value = model.loss_kvsall(combine, ent_idx, rel_idx, offsets, ccols, kind[0], kind[1],
-                                               self.label_smoothing, **qkw) / batch_size
+                                               smoothing, **qkw) / batch_size
             else:
                 loss_value = model.loss_kvsall_train(combine, ent_idx, rel_idx, offsets, ccols, kind[0], kind[1],
-                                                     self.label_smoothing, batch_size, **qkw)
+                                                     smoothing, batch_size, **qkw)
             result.avg_loss += loss_value.item()
             result.forward_time += time.time()
             result.backward_time -= time.time()
