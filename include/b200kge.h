@@ -666,6 +666,27 @@ int b200kge_ns_backward(int model, float l_norm, const b200kge_rows_t* ent, cons
                         int64_t batch_size, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, void* workspace,
                         size_t workspace_bytes, b200kge_stream_t stream);
 
+/* b200kge_ns_backward with each table's gradient in the layout of LibKGE's lookup_embedder.sparse (nn.Embedding with
+ * sparse=True): the operands, coverage and refusals are b200kge_ns_backward's.  Per table, `*_sparse`:
+ *   0: d_ent [E, lde] / d_rel [R, ldr] is the dense gradient, ADDED into as by b200kge_ns_backward; rows / count unused.
+ *   1: row-sparse.  rows receives the sorted unique rows the reference looks up for the slot, *count (device, int64) their
+ *      number u, and rows 0 .. u-1 of the value block d_ent / d_rel (same leading dimension) their gradients,
+ *      OVERWRITTEN; rows past u are not touched.  Entity rows: the positives' s and o and every sampled id, at most
+ *      min(E, n (K + 2)); relation rows: the positives' p, at most min(R, n) (R = rel->rows, so a reciprocal-relations
+ *      S slot passed as (o, p + R', s) lists p + R').  rows and the value block must hold that many rows.  A row is in
+ *      the set whether or not dropout zeroes its elements; ids repeated within the slot are summed.
+ * The row set costs one [V] int32 map per sparse table (flags, an exclusive scan, compaction) in the workspace; no
+ * untouched row of a sparse table is read or written.  Tables of 2^31 rows or more return B200KGE_ERR_UNSUPPORTED.
+ * workspace: b200kge_ns_backward_sparse_workspace_bytes(model, n, K, D, E, R, drop != NULL). */
+size_t b200kge_ns_backward_sparse_workspace_bytes(int model, int64_t n, int64_t K, int32_t D, int64_t E, int64_t R,
+                                                  int dropout);
+int b200kge_ns_backward_sparse(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                               const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
+                               const b200kge_dropout_t* drop, const float* grad_scores, int64_t ldg, float offset,
+                               int64_t batch_size, int ent_sparse, int64_t* ent_rows, int64_t* ent_count, float* d_ent,
+                               int64_t lde, int rel_sparse, int64_t* rel_rows, int64_t* rel_count, float* d_rel,
+                               int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -126,6 +126,13 @@ SIGNATURES = {
     "b200kge_ns_backward": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
                                       C.c_int64, C.c_int, _DP, C.c_void_p, C.c_int64, C.c_float, C.c_int64, C.c_void_p,
                                       C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_ns_backward_sparse_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32, C.c_int64,
+                                                                 C.c_int64, C.c_int]),
+    "b200kge_ns_backward_sparse": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
+                                             C.c_int64, C.c_int, _DP, C.c_void_p, C.c_int64, C.c_float, C.c_int64,
+                                             C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                             C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                             C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_ns_loss_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "b200kge_ns_loss": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_float, C.c_float,
                                   C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t,

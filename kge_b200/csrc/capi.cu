@@ -1996,4 +1996,66 @@ int b200kge_ns_backward(int model, float l_norm, const b200kge_rows_t* ent, cons
                             d_rel, ldr, dQ, ldq, st);
 }
 
+size_t b200kge_ns_backward_sparse_workspace_bytes(int model, int64_t n, int64_t K, int32_t D, int64_t E, int64_t R,
+                                                  int dropout) {
+  if (n < 0 || K < 0 || D <= 0 || E < 0 || R < 0) return 0;
+  return row_set_workspace_bytes(E) + row_set_workspace_bytes(R) +
+         round_up((int64_t)b200kge_ns_backward_workspace_bytes(model, n, K, D, dropout), 256);
+}
+
+int b200kge_ns_backward_sparse(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                               const int64_t* triples, int slot, const int64_t* neg, int64_t n, int64_t K, int impl,
+                               const b200kge_dropout_t* drop, const float* grad_scores, int64_t ldg, float offset,
+                               int64_t batch_size, int ent_sparse, int64_t* ent_rows, int64_t* ent_count, float* d_ent,
+                               int64_t lde, int rel_sparse, int64_t* rel_rows, int64_t* rel_count, float* d_rel,
+                               int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+  int rc;
+  if (drop && (rc = validate_ns_dropout(model, l_norm, ent, rel, triples, slot, neg, n, K, impl, drop))) return rc;
+  if (!triples || (!neg && n * K > 0) || (drop && !grad_scores) || !d_ent || !d_rel || (ent_sparse && (!ent_rows || !ent_count)) ||
+      (rel_sparse && (!rel_rows || !rel_count))) {
+    set_error("null operand");
+    return B200KGE_ERR_INVALID;
+  }
+  if (n < 0 || K < 0) { set_error("negative sizes"); return B200KGE_ERR_INVALID; }
+  if ((rc = check_tables(model, l_norm, ent, rel))) return rc;
+  if (!grad_scores && batch_size <= 0) { set_error("batch_size must be positive"); return B200KGE_ERR_INVALID; }
+  if (grad_scores && ldg < K + 1) { set_error("grad_scores is narrower than the 1 + K columns of the block"); return B200KGE_ERR_INVALID; }
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
+  // the coverage of the gradient kernels, refused before the row sets are built
+  if (slot != 0 && slot != 2) { set_error("the fused negative-sampling backward covers the S and O slots"); return B200KGE_ERR_UNSUPPORTED; }
+  if ((model == B200KGE_TRANSE && l_norm != 1.0f && l_norm != 2.0f) || (model == B200KGE_ROTATE && l_norm != 1.0f)) {
+    set_error("the negative-sampling backward covers l_norm 1 and 2 (TransE) / 1 (RotatE)");
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  const int kf = folded_problem(model, B200KGE_SP_, ent->dim, l_norm).K;
+  if (kf > 1024) { set_error("embedding width %d exceeds the backward kernel's limit of 1024", kf); return B200KGE_ERR_UNSUPPORTED; }
+  if ((K + 64) / 64 > 65535) { set_error("too many negatives per row (%lld)", (long long)K); return B200KGE_ERR_UNSUPPORTED; }
+  if (ent->rows > INT32_MAX || rel->rows > INT32_MAX) { set_error("the row maps cover tables of fewer than 2^31 rows"); return B200KGE_ERR_UNSUPPORTED; }
+  const size_t need = b200kge_ns_backward_sparse_workspace_bytes(model, n, K, ent->dim, ent->rows, rel->rows, drop != nullptr);
+  if (!workspace || workspace_bytes < need) { set_error("workspace too small (see b200kge_ns_backward_sparse_workspace_bytes)"); return B200KGE_ERR_WORKSPACE; }
+  cudaStream_t st = (cudaStream_t)stream;
+  Rows E = to_rows(ent), R = to_rows(rel);
+  uint8_t* ws_e = (uint8_t*)workspace;
+  uint8_t* ws_r = ws_e + row_set_workspace_bytes(E.rows);
+  uint8_t* ws_ns = ws_r + row_set_workspace_bytes(R.rows);
+  const size_t ns_bytes = workspace_bytes - (size_t)(ws_ns - ws_e);
+  // the rows the reference looks up for the slot: the positives' s, o and every sampled id; the positives' p
+  const IdList le[3] = {{triples, n, 3}, {triples + 2, n, 3}, {neg, n * K, 1}};
+  const IdList lr[1] = {{triples + 1, n, 3}};
+  if ((rc = ent_sparse ? launch_row_set(E.rows, le, 3, ws_e, ent_rows, ent_count, d_ent, lde, st)
+                       : launch_identity_map(E.rows, ws_e, st))) return rc;
+  if ((rc = rel_sparse ? launch_row_set(R.rows, lr, 1, ws_r, rel_rows, rel_count, d_rel, ldr, st)
+                       : launch_identity_map(R.rows, ws_r, st))) return rc;
+  if (n == 0) return 0;
+  const int32_t* pe = (const int32_t*)ws_e;
+  const int32_t* pr = (const int32_t*)ws_r;
+  if (drop)
+    return launch_ns_dropout(model, l_norm, E, R, triples, slot, neg, n, K, impl, ns_drop_keys(*drop), grad_scores, ldg,
+                             nullptr, 0, d_ent, lde, d_rel, ldr, ws_ns, ns_bytes, st, pe, pr);
+  const int64_t ldq = round_up(folded_problem(model, B200KGE_SP_, E.dim, l_norm).K, 32);
+  return launch_ns_backward(model, l_norm, E, R, triples, slot, neg, n, K, grad_scores ? 0.f : offset,
+                            grad_scores ? 1.f : 1.0f / (float)batch_size, grad_scores, grad_scores ? ldg : 0, d_ent, lde,
+                            d_rel, ldr, (float*)ws_ns, ldq, st, pe, pr);
+}
+
 }  // extern "C"

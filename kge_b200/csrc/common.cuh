@@ -489,11 +489,12 @@ int launch_ns_masked(int model, float l_norm, const Rows& ent, const Rows& rel, 
                      float* out, int64_t ldo, int col0, cudaStream_t st);
 // ns_backward_kernel with the same masks (grad.cu): a and p are [n, D] / [n, Dr] masked copies of the fixed rows (plain
 // rows, row i of the sub-batch), so the fold and the unfold run unchanged and the row gradients land in dA / dP
-// (OVERWRITTEN); the sampled rows' gradients are masked and scattered into d_ent.  Columns 1..K of G only.
+// (OVERWRITTEN); the sampled rows' gradients are masked and scattered into d_ent (pe: into row pe[e]).  Columns 1..K of
+// G only.
 int launch_ns_backward_masked(int model, float l_norm, const Rows& a, const Rows& p, const Rows& table, int slot,
                               const int64_t* neg, int64_t n, int64_t K, const DropMask& mt, const float* G, int64_t ldg,
                               float* d_ent, int64_t lde, float* dQ, int64_t ldq, int64_t* tri_ws, float* dA, float* dP,
-                              cudaStream_t st);
+                              cudaStream_t st, const int32_t* pe = nullptr);
 // Dropout of one negative-sampling slot (ns_dropout.cu): the entity and relation draws' key and rate (stream and
 // row_base are set per draw) and the sub-batch's first global row.
 struct NsDropKeys {
@@ -502,11 +503,28 @@ struct NsDropKeys {
 };
 // G == NULL: scores of the [n, 1+K] block into out (positive in column 0); else the backward of that block with
 // grad_scores G, ADDED into d_ent / d_rel.  impl: B200KGE_NS_TRIPLE | B200KGE_NS_BATCH.
-// workspace: ns_dropout_workspace_bytes (the backward of the `batch` negatives only; the rest needs none)
+// workspace: ns_dropout_workspace_bytes (the backward of the `batch` negatives only; the rest needs none).  pe / pr (both
+// or neither): row maps of the backward, as launch_ns_backward's.
 size_t ns_dropout_workspace_bytes(int model, int64_t n, int32_t D);
 int launch_ns_dropout(int model, float l_norm, const Rows& ent, const Rows& rel, const int64_t* triples, int slot,
                       const int64_t* neg, int64_t n, int64_t K, int impl, const NsDropKeys& keys, const float* G,
                       int64_t ldg, float* out, int64_t ldo, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                      void* workspace, size_t workspace_bytes, cudaStream_t st);
+                      void* workspace, size_t workspace_bytes, cudaStream_t st, const int32_t* pe = nullptr,
+                      const int32_t* pr = nullptr);
+
+// Row set of a row-sparse table gradient (rowset.cu).  ids[i * stride], i < count: one list of looked-up rows.
+struct IdList {
+  const int64_t* ids;
+  int64_t count, stride;
+};
+// workspace of launch_row_set over V rows: the [V] int32 row map first, then per-tile counts
+size_t row_set_workspace_bytes(int64_t V);
+// The sorted unique ids of the lists into rows[0 .. u) and u into *count (device); the map at the start of the workspace
+// gets map[id] = the id's row in [0, u) for every listed id (other entries undefined); the first u rows of vals [*, ld]
+// are zeroed.
+int launch_row_set(int64_t V, const IdList* lists, int nlists, void* workspace, int64_t* rows, int64_t* count,
+                   float* vals, int64_t ld, cudaStream_t st);
+// map[id] = id for id < V at the start of the workspace: a dense table through the row-mapped kernels
+int launch_identity_map(int64_t V, void* workspace, cudaStream_t st);
 
 }  // namespace b200kge

@@ -205,11 +205,12 @@ csr_grad_fix_kernel(const float* __restrict__ z, int64_t ldz, int64_t n, const i
 // Row-wise unfold: block b handles query row b.  dir < 0: rows [0,n) are sp_ (a = subject), rows [n,2n) are
 // _po (a = object) — the stacked layout of prep_1vsall_kernel; dir = 0 / 1: all rows sp_ / _po.  RECIP (dir < 0): the
 // reciprocal layout, rows [n,2n) are sp_ with a = object and relation row p + num_rel.
-template <int MODEL, bool RECIP>
-__global__ void __launch_bounds__(128)
-unfold_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t n, int dir,
-              const float* __restrict__ dQ, int64_t ldq, float* __restrict__ d_ent, int64_t lde,
-              float* __restrict__ d_rel, int64_t ldr, int64_t num_rel) {
+// MAP (unfold_rows_kernel): the gradient rows are row-mapped, da = d_ent + pe[a] * lde and dp = d_rel + pr[p] * ldr
+template <int MODEL, bool RECIP, bool MAP>
+__device__ __forceinline__ void unfold_body(const Rows& ent, const Rows& rel, const int64_t* __restrict__ tri, int64_t n,
+                                            int dir, const float* __restrict__ dQ, int64_t ldq, float* __restrict__ d_ent,
+                                            int64_t lde, float* __restrict__ d_rel, int64_t ldr, int64_t num_rel,
+                                            const int32_t* __restrict__ pe, const int32_t* __restrict__ pr) {
   const int64_t b = blockIdx.x;
   const bool second = dir < 0 && b >= n;
   const bool sp = RECIP || (dir < 0 ? (b < n) : (dir == 0));
@@ -220,8 +221,8 @@ unfold_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t n, in
   const float* __restrict__ a = ent.base + ai * ent.ld;
   const float* __restrict__ p = rel.base + pi * rel.ld;
   const float* __restrict__ g = dQ + b * ldq;
-  float* __restrict__ da = d_ent + ai * lde;
-  float* __restrict__ dp = d_rel + pi * ldr;
+  float* __restrict__ da = d_ent + (MAP ? (int64_t)pe[ai] : ai) * lde;
+  float* __restrict__ dp = d_rel + (MAP ? (int64_t)pr[pi] : pi) * ldr;
   const int D = ent.dim, h = D >> 1;
 
   if constexpr (MODEL == B200KGE_RESCAL) {
@@ -295,6 +296,23 @@ unfold_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t n, in
       atomicAdd(dp + k, g[k] * a[ao + k]);
     }
   }
+}
+
+template <int MODEL, bool RECIP>
+__global__ void __launch_bounds__(128)
+unfold_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t n, int dir,
+              const float* __restrict__ dQ, int64_t ldq, float* __restrict__ d_ent, int64_t lde,
+              float* __restrict__ d_rel, int64_t ldr, int64_t num_rel) {
+  unfold_body<MODEL, RECIP, false>(ent, rel, tri, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, num_rel, nullptr, nullptr);
+}
+
+template <int MODEL>
+__global__ void __launch_bounds__(128)
+unfold_rows_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t n, int dir,
+                   const float* __restrict__ dQ, int64_t ldq, float* __restrict__ d_ent, int64_t lde,
+                   float* __restrict__ d_rel, int64_t ldr, const int32_t* __restrict__ pe,
+                   const int32_t* __restrict__ pr) {
+  unfold_body<MODEL, false, true>(ent, rel, tri, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, 0, pe, pr);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -393,12 +411,13 @@ constexpr int NSB_WARPS = 4, NSB_PER_BLOCK = 64, NSB_MAXK = 1024;   // lane-loca
 // MASK (ns_backward_kernel_masked, the `batch` negatives with dropout): `fa` / `rel` hold masked copies of the fixed rows
 // under identity triples, column 0 (the positive, drawn on other streams) is skipped, and every sampled row is masked
 // by its entity id (draw tm) where it is loaded and where its gradient is scattered.
-template <int MODEL, bool MASK>
+// MAP (ns_backward_rows_kernel, ns_backward_rows_kernel_masked): entity e's gradient row is d_ent + pe[e] * lde.
+template <int MODEL, bool MASK, bool MAP>
 __device__ __forceinline__ void ns_backward_body(const Rows& fa, const Rows& ent, const Rows& rel, const int64_t* __restrict__ tri,
                                                  int sp, const int64_t* __restrict__ neg, int64_t Kneg, const Folded& f,
                                                  float l_norm, float offset, float inv_batch, const float* __restrict__ G,
                                                  int64_t ldg, float* __restrict__ d_ent, int64_t lde, float* __restrict__ dQ,
-                                                 int64_t ldq, const DropMask& tm) {
+                                                 int64_t ldq, const DropMask& tm, const int32_t* __restrict__ pe) {
   extern __shared__ __align__(16) float sh[];  // q[K] | dq[K] (+ entity row for RESCAL)
   const int64_t i = blockIdx.x;
   const int64_t si = tri[3 * i], pi = tri[3 * i + 1], oi = tri[3 * i + 2];
@@ -430,7 +449,7 @@ __device__ __forceinline__ void ns_backward_body(const Rows& fa, const Rows& ent
     const int64_t e = (c == 0) ? (sp ? oi : si) : neg[i * Kneg + (c - 1)];
     const float y = (c == 0) ? 1.f : 0.f;
     const float* __restrict__ t = ent.base + e * ent.ld + f.col_off;
-    float* __restrict__ dt = d_ent + e * lde + f.col_off;
+    float* __restrict__ dt = d_ent + (MAP ? (int64_t)pe[e] : e) * lde + f.col_off;
     // T(k): element k of the sampled row, DT_ADD(k, v): its gradient — through the entity's mask under MASK
 #define T(k) (MASK ? t[k] * drop_mask1(tm, (uint64_t)e, D, f.col_off + (k)) : t[k])
 #define DT_ADD(k, v)                                                                   \
@@ -510,8 +529,18 @@ __global__ void __launch_bounds__(NSB_WARPS * 32)
 ns_backward_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int sp, const int64_t* __restrict__ neg,
                    int64_t Kneg, Folded f, float l_norm, float offset, float inv_batch, const float* __restrict__ G,
                    int64_t ldg, float* __restrict__ d_ent, int64_t lde, float* __restrict__ dQ, int64_t ldq) {
-  ns_backward_body<MODEL, false>(ent, ent, rel, tri, sp, neg, Kneg, f, l_norm, offset, inv_batch, G, ldg, d_ent, lde, dQ,
-                                 ldq, DropMask{});
+  ns_backward_body<MODEL, false, false>(ent, ent, rel, tri, sp, neg, Kneg, f, l_norm, offset, inv_batch, G, ldg, d_ent, lde,
+                                        dQ, ldq, DropMask{}, nullptr);
+}
+
+template <int MODEL>
+__global__ void __launch_bounds__(NSB_WARPS * 32)
+ns_backward_rows_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int sp, const int64_t* __restrict__ neg,
+                        int64_t Kneg, Folded f, float l_norm, float offset, float inv_batch, const float* __restrict__ G,
+                        int64_t ldg, float* __restrict__ d_ent, int64_t lde, float* __restrict__ dQ, int64_t ldq,
+                        const int32_t* __restrict__ pe) {
+  ns_backward_body<MODEL, false, true>(ent, ent, rel, tri, sp, neg, Kneg, f, l_norm, offset, inv_batch, G, ldg, d_ent, lde,
+                                       dQ, ldq, DropMask{}, pe);
 }
 
 template <int MODEL>
@@ -520,16 +549,29 @@ ns_backward_kernel_masked(Rows fa, Rows ent, Rows rel, const int64_t* __restrict
                           const int64_t* __restrict__ neg, int64_t Kneg, Folded f, float l_norm,
                           const float* __restrict__ G, int64_t ldg, float* __restrict__ d_ent, int64_t lde,
                           float* __restrict__ dQ, int64_t ldq, DropMask tm) {
-  ns_backward_body<MODEL, true>(fa, ent, rel, tri, sp, neg, Kneg, f, l_norm, 0.f, 1.f, G, ldg, d_ent, lde, dQ, ldq, tm);
+  ns_backward_body<MODEL, true, false>(fa, ent, rel, tri, sp, neg, Kneg, f, l_norm, 0.f, 1.f, G, ldg, d_ent, lde, dQ, ldq,
+                                       tm, nullptr);
+}
+
+template <int MODEL>
+__global__ void __launch_bounds__(NSB_WARPS * 32)
+ns_backward_rows_kernel_masked(Rows fa, Rows ent, Rows rel, const int64_t* __restrict__ tri, int sp,
+                               const int64_t* __restrict__ neg, int64_t Kneg, Folded f, float l_norm,
+                               const float* __restrict__ G, int64_t ldg, float* __restrict__ d_ent, int64_t lde,
+                               float* __restrict__ dQ, int64_t ldq, DropMask tm, const int32_t* __restrict__ pe) {
+  ns_backward_body<MODEL, true, true>(fa, ent, rel, tri, sp, neg, Kneg, f, l_norm, 0.f, 1.f, G, ldg, d_ent, lde, dQ, ldq,
+                                      tm, pe);
 }
 
 // unfold for the distance family (TransE: Q = a +- p; RotatE: rotation) — appended to the dot-family unfold
 // (RECIP: the reciprocal layout of unfold_kernel)
-template <int MODEL, bool RECIP>
-__global__ void __launch_bounds__(128)
-unfold_distance_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t n, int dir,
-                       const float* __restrict__ dQ, int64_t ldq, float* __restrict__ d_ent, int64_t lde,
-                       float* __restrict__ d_rel, int64_t ldr, int64_t num_rel) {
+// (MAP: row-mapped gradient rows, as unfold_body)
+template <int MODEL, bool RECIP, bool MAP>
+__device__ __forceinline__ void unfold_distance_body(const Rows& ent, const Rows& rel, const int64_t* __restrict__ tri,
+                                                     int64_t n, int dir, const float* __restrict__ dQ, int64_t ldq,
+                                                     float* __restrict__ d_ent, int64_t lde, float* __restrict__ d_rel,
+                                                     int64_t ldr, int64_t num_rel, const int32_t* __restrict__ pe,
+                                                     const int32_t* __restrict__ pr) {
   const int64_t b = blockIdx.x;
   const bool second = dir < 0 && b >= n;
   const bool sp = RECIP || (dir < 0 ? (b < n) : (dir == 0));
@@ -540,8 +582,8 @@ unfold_distance_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int6
   const float* __restrict__ a = ent.base + ai * ent.ld;
   const float* __restrict__ p = rel.base + pi * rel.ld;
   const float* __restrict__ g = dQ + b * ldq;
-  float* __restrict__ da = d_ent + ai * lde;
-  float* __restrict__ dp = d_rel + pi * ldr;
+  float* __restrict__ da = d_ent + (MAP ? (int64_t)pe[ai] : ai) * lde;
+  float* __restrict__ dp = d_rel + (MAP ? (int64_t)pr[pi] : pi) * ldr;
   const int D = ent.dim, h = D >> 1;
   if constexpr (MODEL == B200KGE_TRANSE) {      // Q = a + p | Q = a - p
     for (int k = threadIdx.x; k < D; k += blockDim.x) {
@@ -566,12 +608,30 @@ unfold_distance_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int6
   }
 }
 
+template <int MODEL, bool RECIP>
+__global__ void __launch_bounds__(128)
+unfold_distance_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t n, int dir,
+                       const float* __restrict__ dQ, int64_t ldq, float* __restrict__ d_ent, int64_t lde,
+                       float* __restrict__ d_rel, int64_t ldr, int64_t num_rel) {
+  unfold_distance_body<MODEL, RECIP, false>(ent, rel, tri, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, num_rel, nullptr,
+                                            nullptr);
+}
+
+template <int MODEL>
+__global__ void __launch_bounds__(128)
+unfold_distance_rows_kernel(Rows ent, Rows rel, const int64_t* __restrict__ tri, int64_t n, int dir,
+                            const float* __restrict__ dQ, int64_t ldq, float* __restrict__ d_ent, int64_t lde,
+                            float* __restrict__ d_rel, int64_t ldr, const int32_t* __restrict__ pe,
+                            const int32_t* __restrict__ pr) {
+  unfold_distance_body<MODEL, false, true>(ent, rel, tri, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, 0, pe, pr);
+}
+
 }  // namespace
 
 int launch_ns_backward(int model, float l_norm, const Rows& ent, const Rows& rel, const int64_t* triples, int slot,
                        const int64_t* neg, int64_t n, int64_t K, float offset, float inv_batch, const float* G,
                        int64_t ldg, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, float* dQ, int64_t ldq,
-                       cudaStream_t st) {
+                       cudaStream_t st, const int32_t* pe, const int32_t* pr) {
   if (n == 0) return 0;
   if (slot != 0 && slot != 2) { set_error("the fused negative-sampling backward covers the S and O slots"); return B200KGE_ERR_UNSUPPORTED; }
   const int sp = (slot == 2) ? 1 : 0;      // O slot: fold (s,p), candidates are objects
@@ -585,7 +645,13 @@ int launch_ns_backward(int model, float l_norm, const Rows& ent, const Rows& rel
   const int64_t by = (K + 1 + NSB_PER_BLOCK - 1) / NSB_PER_BLOCK;
   if (by > 65535) { set_error("too many negatives per row (%lld)", (long long)K); return B200KGE_ERR_UNSUPPORTED; }
   dim3 grid((unsigned)n, (unsigned)by), block(NSB_WARPS * 32);
-#define B2K_NSB(M) case M: ns_backward_kernel<M><<<grid, block, smem, st>>>(ent, rel, triples, sp, neg, K, f, l_norm, offset, inv_batch, G, ldg, d_ent, lde, dQ, ldq); break;
+#define B2K_NSB(M)                                                                                                             \
+  case M:                                                                                                                      \
+    if (pe) ns_backward_rows_kernel<M><<<grid, block, smem, st>>>(ent, rel, triples, sp, neg, K, f, l_norm, offset, inv_batch, \
+                                                                  G, ldg, d_ent, lde, dQ, ldq, pe);                            \
+    else ns_backward_kernel<M><<<grid, block, smem, st>>>(ent, rel, triples, sp, neg, K, f, l_norm, offset, inv_batch, G, ldg, \
+                                                          d_ent, lde, dQ, ldq);                                                \
+    break;
   switch (model) {
     B2K_NSB(B200KGE_COMPLEX) B2K_NSB(B200KGE_DISTMULT) B2K_NSB(B200KGE_SIMPLE) B2K_NSB(B200KGE_CP)
     B2K_NSB(B200KGE_RESCAL) B2K_NSB(B200KGE_TRANSE) B2K_NSB(B200KGE_ROTATE)
@@ -594,6 +660,11 @@ int launch_ns_backward(int model, float l_norm, const Rows& ent, const Rows& rel
 #undef B2K_NSB
   B2K_LAUNCH_CHECK("ns_backward_kernel");
   const int dir = sp ? 0 : 1;
+  if (pe) {
+    if (model == B200KGE_TRANSE || model == B200KGE_ROTATE)
+      return launch_unfold_distance(model, ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, st, 0, pe, pr);
+    return launch_unfold(model, ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, st, 0, pe, pr);
+  }
   if (model == B200KGE_TRANSE || model == B200KGE_ROTATE) {
     dim3 g2((unsigned)n), b2(128);
     if (model == B200KGE_TRANSE)
@@ -609,7 +680,7 @@ int launch_ns_backward(int model, float l_norm, const Rows& ent, const Rows& rel
 int launch_ns_backward_masked(int model, float l_norm, const Rows& a, const Rows& p, const Rows& table, int slot,
                               const int64_t* neg, int64_t n, int64_t K, const DropMask& mt, const float* G, int64_t ldg,
                               float* d_ent, int64_t lde, float* dQ, int64_t ldq, int64_t* tri_ws, float* dA, float* dP,
-                              cudaStream_t st) {
+                              cudaStream_t st, const int32_t* pe) {
   if (n == 0) return 0;
   if (slot != 0 && slot != 2) { set_error("the masked negative-sampling backward covers the S and O slots"); return B200KGE_ERR_UNSUPPORTED; }
   const int sp = (slot == 2) ? 1 : 0;
@@ -628,7 +699,13 @@ int launch_ns_backward_masked(int model, float l_norm, const Rows& a, const Rows
     const int64_t by = (K + 1 + NSB_PER_BLOCK - 1) / NSB_PER_BLOCK;
     if (by > 65535) { set_error("too many negatives per row (%lld)", (long long)K); return B200KGE_ERR_UNSUPPORTED; }
     dim3 grid((unsigned)n, (unsigned)by), block(NSB_WARPS * 32);
-#define B2K_NSBM(M) case M: ns_backward_kernel_masked<M><<<grid, block, smem, st>>>(a, table, p, tri_ws, sp, neg, K, f, l_norm, G, ldg, d_ent, lde, dQ, ldq, mt); break;
+#define B2K_NSBM(M)                                                                                                    \
+  case M:                                                                                                              \
+    if (pe) ns_backward_rows_kernel_masked<M><<<grid, block, smem, st>>>(a, table, p, tri_ws, sp, neg, K, f, l_norm, G, \
+                                                                         ldg, d_ent, lde, dQ, ldq, mt, pe);             \
+    else ns_backward_kernel_masked<M><<<grid, block, smem, st>>>(a, table, p, tri_ws, sp, neg, K, f, l_norm, G, ldg,    \
+                                                                 d_ent, lde, dQ, ldq, mt);                              \
+    break;
     switch (model) {
       B2K_NSBM(B200KGE_COMPLEX) B2K_NSBM(B200KGE_DISTMULT) B2K_NSBM(B200KGE_SIMPLE) B2K_NSBM(B200KGE_CP)
       B2K_NSBM(B200KGE_TRANSE) B2K_NSBM(B200KGE_ROTATE)
@@ -646,11 +723,16 @@ int launch_ns_backward_masked(int model, float l_norm, const Rows& a, const Rows
 
 int launch_unfold_distance(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n, int dir,
                            const float* dQ, int64_t ldq, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                           cudaStream_t st, int64_t num_rel) {
+                           cudaStream_t st, int64_t num_rel, const int32_t* pe, const int32_t* pr) {
   if (n == 0) return 0;
   if (num_rel > 0 && dir >= 0) { set_error("the reciprocal unfold needs the stacked layout"); return B200KGE_ERR_INVALID; }
+  if (pe && (num_rel > 0 || dir < 0)) { set_error("the row-mapped unfold covers one direction"); return B200KGE_ERR_INVALID; }
   dim3 g2((unsigned)(dir < 0 ? 2 * n : n)), b2(128);
-  if (model == B200KGE_TRANSE && num_rel > 0)
+  if (pe && model == B200KGE_TRANSE)
+    unfold_distance_rows_kernel<B200KGE_TRANSE><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, pe, pr);
+  else if (pe && model == B200KGE_ROTATE)
+    unfold_distance_rows_kernel<B200KGE_ROTATE><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, pe, pr);
+  else if (model == B200KGE_TRANSE && num_rel > 0)
     unfold_distance_kernel<B200KGE_TRANSE, true><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, num_rel);
   else if (model == B200KGE_ROTATE && num_rel > 0)
     unfold_distance_kernel<B200KGE_ROTATE, true><<<g2, b2, 0, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, num_rel);
@@ -741,15 +823,23 @@ int launch_grad_planes_csr(const float* z, int64_t ldz, int64_t nq, int64_t E, c
 
 int launch_unfold(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n, int dir,
                   const float* dQ, int64_t ldq, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, cudaStream_t st,
-                  int64_t num_rel) {
+                  int64_t num_rel, const int32_t* pe, const int32_t* pr) {
   if (n == 0) return 0;
   if (num_rel > 0 && dir >= 0) { set_error("the reciprocal unfold needs the stacked layout"); return B200KGE_ERR_INVALID; }
+  if (pe && (num_rel > 0 || dir < 0)) { set_error("the row-mapped unfold covers one direction"); return B200KGE_ERR_INVALID; }
   const int64_t nq = dir < 0 ? 2 * n : n;
   dim3 grid((unsigned)nq), block(128);
   const int D = ent.dim;
 #define B2K_UNFOLD(M, SM) case M: unfold_kernel<M, false><<<grid, block, SM, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, 0); break;
 #define B2K_UNFOLD_R(M, SM) case M: unfold_kernel<M, true><<<grid, block, SM, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, num_rel); break;
-  if (num_rel > 0) {
+#define B2K_UNFOLD_M(M, SM) case M: unfold_rows_kernel<M><<<grid, block, SM, st>>>(ent, rel, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, pe, pr); break;
+  if (pe) {
+    switch (model) {
+      B2K_UNFOLD_M(B200KGE_COMPLEX, 0) B2K_UNFOLD_M(B200KGE_DISTMULT, 0) B2K_UNFOLD_M(B200KGE_SIMPLE, 0)
+      B2K_UNFOLD_M(B200KGE_CP, 0) B2K_UNFOLD_M(B200KGE_RESCAL, 2 * D * sizeof(float))
+      default: set_error("the analytic backward covers the dot family only (model %d)", model); return B200KGE_ERR_UNSUPPORTED;
+    }
+  } else if (num_rel > 0) {
     switch (model) {
       B2K_UNFOLD_R(B200KGE_COMPLEX, 0) B2K_UNFOLD_R(B200KGE_DISTMULT, 0) B2K_UNFOLD_R(B200KGE_SIMPLE, 0)
       B2K_UNFOLD_R(B200KGE_CP, 0) B2K_UNFOLD_R(B200KGE_RESCAL, 2 * D * sizeof(float))
@@ -764,6 +854,7 @@ int launch_unfold(int model, const Rows& ent, const Rows& rel, const int64_t* tr
   }
 #undef B2K_UNFOLD
 #undef B2K_UNFOLD_R
+#undef B2K_UNFOLD_M
   B2K_LAUNCH_CHECK("unfold_kernel");
   return 0;
 }

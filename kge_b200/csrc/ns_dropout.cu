@@ -60,19 +60,21 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 // The lane's share of score_spo of logical triple t (BWD = false: returns the partial reduction, spo_kernel's
 // arithmetic), or of its vector-Jacobian product (BWD = true: g = dL/dscore, nrm = the L2 distance of TransE L2;
-// scatters into d_ent / d_rel and returns 0).
-template <int MODEL, bool BWD>
+// scatters into d_ent / d_rel and returns 0).  MAP: row-mapped gradient rows, d_ent + pe[id] * lde, d_rel + pr[id] * ldr.
+template <int MODEL, bool BWD, bool MAP = false>
 __device__ __forceinline__ float ns_drop_triple(const NsOp& S, const NsOp& P, const NsOp& O, int64_t t, int lane,
                                                 float l_norm, float teps, float g, float nrm, float* __restrict__ d_ent,
-                                                int64_t lde, float* __restrict__ d_rel, int64_t ldr) {
+                                                int64_t lde, float* __restrict__ d_rel, int64_t ldr,
+                                                const int32_t* __restrict__ pe = nullptr,
+                                                const int32_t* __restrict__ pr = nullptr) {
   const int64_t si = S.id(t), pi = P.id(t), oi = O.id(t);
   const uint64_t ms = S.mrow(t, si), mp = P.mrow(t, pi), mo = O.mrow(t, oi);
   const float* __restrict__ s = S.base + si * S.ld;
   const float* __restrict__ p = P.base + pi * P.ld;
   const float* __restrict__ o = O.base + oi * O.ld;
-  float* ds = BWD ? d_ent + si * lde : nullptr;
-  float* dp = BWD ? d_rel + pi * ldr : nullptr;
-  float* dO = BWD ? d_ent + oi * lde : nullptr;
+  float* ds = BWD ? d_ent + (MAP ? (int64_t)pe[si] : si) * lde : nullptr;
+  float* dp = BWD ? d_rel + (MAP ? (int64_t)pr[pi] : pi) * ldr : nullptr;
+  float* dO = BWD ? d_ent + (MAP ? (int64_t)pe[oi] : oi) * lde : nullptr;
   const int D = S.width, h = D >> 1;
   float acc = 0.f;
   if constexpr (MODEL == B200KGE_DISTMULT) {
@@ -249,11 +251,12 @@ ns_drop_score_kernel(NsOp S, NsOp P, NsOp O, int64_t N, float l_norm, float teps
 }
 
 // backward: g = G[(t / out_div) * ldg + col0 + t % out_div]; TransE L2 first recomputes the distance
-template <int MODEL>
-__global__ void __launch_bounds__(256)
-ns_drop_backward_kernel(NsOp S, NsOp P, NsOp O, int64_t N, float l_norm, float teps, const float* __restrict__ G,
-                        int64_t ldg, int64_t out_div, int64_t col0, float* __restrict__ d_ent, int64_t lde,
-                        float* __restrict__ d_rel, int64_t ldr) {
+template <int MODEL, bool MAP>
+__device__ __forceinline__ void ns_drop_backward_body(const NsOp& S, const NsOp& P, const NsOp& O, int64_t N, float l_norm,
+                                                      float teps, const float* __restrict__ G, int64_t ldg,
+                                                      int64_t out_div, int64_t col0, float* __restrict__ d_ent,
+                                                      int64_t lde, float* __restrict__ d_rel, int64_t ldr,
+                                                      const int32_t* __restrict__ pe, const int32_t* __restrict__ pr) {
   const int lane = threadIdx.x & 31;
   const int64_t t = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (t >= N) return;
@@ -263,7 +266,25 @@ ns_drop_backward_kernel(NsOp S, NsOp P, NsOp O, int64_t N, float l_norm, float t
   float nrm = 0.f;
   if (MODEL == B200KGE_TRANSE && l_norm == 2.0f)
     nrm = sqrtf(warp_sum(ns_drop_triple<MODEL, false>(S, P, O, t, lane, l_norm, teps, 0.f, 0.f, nullptr, 0, nullptr, 0)));
-  ns_drop_triple<MODEL, true>(S, P, O, t, lane, l_norm, teps, g, nrm, d_ent, lde, d_rel, ldr);
+  ns_drop_triple<MODEL, true, MAP>(S, P, O, t, lane, l_norm, teps, g, nrm, d_ent, lde, d_rel, ldr, pe, pr);
+}
+
+template <int MODEL>
+__global__ void __launch_bounds__(256)
+ns_drop_backward_kernel(NsOp S, NsOp P, NsOp O, int64_t N, float l_norm, float teps, const float* __restrict__ G,
+                        int64_t ldg, int64_t out_div, int64_t col0, float* __restrict__ d_ent, int64_t lde,
+                        float* __restrict__ d_rel, int64_t ldr) {
+  ns_drop_backward_body<MODEL, false>(S, P, O, N, l_norm, teps, G, ldg, out_div, col0, d_ent, lde, d_rel, ldr, nullptr,
+                                      nullptr);
+}
+
+template <int MODEL>
+__global__ void __launch_bounds__(256)
+ns_drop_backward_rows_kernel(NsOp S, NsOp P, NsOp O, int64_t N, float l_norm, float teps, const float* __restrict__ G,
+                             int64_t ldg, int64_t out_div, int64_t col0, float* __restrict__ d_ent, int64_t lde,
+                             float* __restrict__ d_rel, int64_t ldr, const int32_t* __restrict__ pe,
+                             const int32_t* __restrict__ pr) {
+  ns_drop_backward_body<MODEL, true>(S, P, O, N, l_norm, teps, G, ldg, out_div, col0, d_ent, lde, d_rel, ldr, pe, pr);
 }
 
 // dst[i, :] = mask(row_base + i, :) * tab[tri[3 i + c], :]  (width % 4 == 0; one thread per four-element group)
@@ -281,19 +302,33 @@ ns_drop_gather_kernel(DropMask m, const float* __restrict__ base, int64_t ld, in
   for (int j = 0; j < 4; ++j) dst[i * width + k + j] = src[k + j] * mk[j];
 }
 
-// d[tri[3 i + c], :] += mask(row_base + i, :) * src[i, :]  (atomic: rows repeat)
-__global__ void __launch_bounds__(256)
-ns_drop_scatter_kernel(DropMask m, const float* __restrict__ src, int width, const int64_t* __restrict__ tri, int c,
-                       int64_t n, float* __restrict__ d, int64_t ldd) {
+// d[tri[3 i + c], :] += mask(row_base + i, :) * src[i, :]  (atomic: rows repeat; MAP: row pos[tri[3 i + c]] of d)
+template <bool MAP>
+__device__ __forceinline__ void ns_drop_scatter_body(const DropMask& m, const float* __restrict__ src, int width,
+                                                     const int64_t* __restrict__ tri, int c, int64_t n,
+                                                     float* __restrict__ d, int64_t ldd, const int32_t* __restrict__ pos) {
   const int64_t g = blockIdx.x * (int64_t)blockDim.x + threadIdx.x, w4 = width >> 2;
   if (g >= n * w4) return;
   const int64_t i = g / w4;
   const int k = (int)(g - i * w4) * 4;
   float mk[4];
   drop_mask4(m, (uint64_t)(m.row_base + i), width, k, mk);
-  float* dst = d + tri[3 * i + c] * ldd;
+  const int64_t id = tri[3 * i + c];
+  float* dst = d + (MAP ? (int64_t)pos[id] : id) * ldd;
 #pragma unroll
   for (int j = 0; j < 4; ++j) if (mk[j] != 0.f) atomicAdd(dst + k + j, src[i * width + k + j] * mk[j]);
+}
+
+__global__ void __launch_bounds__(256)
+ns_drop_scatter_kernel(DropMask m, const float* __restrict__ src, int width, const int64_t* __restrict__ tri, int c,
+                       int64_t n, float* __restrict__ d, int64_t ldd) {
+  ns_drop_scatter_body<false>(m, src, width, tri, c, n, d, ldd, nullptr);
+}
+
+__global__ void __launch_bounds__(256)
+ns_drop_scatter_rows_kernel(DropMask m, const float* __restrict__ src, int width, const int64_t* __restrict__ tri, int c,
+                            int64_t n, float* __restrict__ d, int64_t ldd, const int32_t* __restrict__ pos) {
+  ns_drop_scatter_body<true>(m, src, width, tri, c, n, d, ldd, pos);
 }
 
 inline unsigned groups_grid(int64_t n, int width) { return (unsigned)((n * (width / 4) + 255) / 256); }
@@ -308,15 +343,19 @@ NsOp ns_op(const Rows& tab, const int64_t* idx, int64_t istride, int64_t div, co
 
 int launch_drop_triples(int model, bool bwd, const NsOp& S, const NsOp& P, const NsOp& O, int64_t N, float l_norm,
                         float teps, const float* G, int64_t ldg, float* out, int64_t ldo, int64_t out_div,
-                        int64_t col0, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, cudaStream_t st) {
+                        int64_t col0, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, cudaStream_t st,
+                        const int32_t* pe, const int32_t* pr) {
   if (N == 0) return 0;
   const int64_t blocks = (N + 7) / 8;
   if (blocks > 2147483647LL) { set_error("too many triples"); return B200KGE_ERR_UNSUPPORTED; }
   dim3 grid((unsigned)blocks), block(256);
 #define B2K_NSD(M)                                                                                                  \
   case M:                                                                                                           \
-    if (bwd) ns_drop_backward_kernel<M><<<grid, block, 0, st>>>(S, P, O, N, l_norm, teps, G, ldg, out_div, col0,    \
-                                                                d_ent, lde, d_rel, ldr);                            \
+    if (bwd && pe) ns_drop_backward_rows_kernel<M><<<grid, block, 0, st>>>(S, P, O, N, l_norm, teps, G, ldg,        \
+                                                                           out_div, col0, d_ent, lde, d_rel, ldr,   \
+                                                                           pe, pr);                                 \
+    else if (bwd) ns_drop_backward_kernel<M><<<grid, block, 0, st>>>(S, P, O, N, l_norm, teps, G, ldg, out_div,     \
+                                                                     col0, d_ent, lde, d_rel, ldr);                 \
     else ns_drop_score_kernel<M><<<grid, block, 0, st>>>(S, P, O, N, l_norm, teps, out, ldo, out_div, col0);        \
     break;
   switch (model) {
@@ -340,7 +379,8 @@ size_t ns_dropout_workspace_bytes(int model, int64_t n, int32_t D) {
 int launch_ns_dropout(int model, float l_norm, const Rows& ent, const Rows& rel, const int64_t* triples, int slot,
                       const int64_t* neg, int64_t n, int64_t K, int impl, const NsDropKeys& keys, const float* G,
                       int64_t ldg, float* out, int64_t ldo, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                      void* workspace, size_t workspace_bytes, cudaStream_t st) {
+                      void* workspace, size_t workspace_bytes, cudaStream_t st, const int32_t* pe,
+                      const int32_t* pr) {
   const bool bwd = G != nullptr;
   const int64_t rb = keys.row_base;
   const int sb = 6 + 6 * slot;                         // first stream of the slot
@@ -354,7 +394,8 @@ int launch_ns_dropout(int model, float l_norm, const Rows& ent, const Rows& rel,
   NsOp S = ns_op(ent, triples + 0, 3, 1, mk(false, 0, rb), 1, 0);
   NsOp P = ns_op(rel, triples + 1, 3, 1, mk(true, 1, rb), 1, 0);
   NsOp O = ns_op(ent, triples + 2, 3, 1, mk(false, 2, rb), 1, 0);
-  int rc = launch_drop_triples(model, bwd, S, P, O, n, l_norm, eps, G, ldg, out, ldo, 1, 0, d_ent, lde, d_rel, ldr, st);
+  int rc = launch_drop_triples(model, bwd, S, P, O, n, l_norm, eps, G, ldg, out, ldo, 1, 0, d_ent, lde, d_rel, ldr, st,
+                               pe, pr);
   if (rc || K == 0) return rc;
   const bool triple = impl == B200KGE_NS_TRIPLE;
   if (!triple && model != B200KGE_RESCAL) {
@@ -383,7 +424,14 @@ int launch_ns_dropout(int model, float l_norm, const Rows& ent, const Rows& rel,
     B2K_LAUNCH_CHECK("ns_drop_gather_kernel");
     Rows a{Am, nullptr, n, D, D}, p{Pm, nullptr, n, Dr, Dr};
     if ((rc = launch_ns_backward_masked(model, l_norm, a, p, ent, slot, neg, n, K, mt, G, ldg, d_ent, lde, dQ, ldq, tri,
-                                        dA, dP, st))) return rc;
+                                        dA, dP, st, pe))) return rc;
+    if (pe) {
+      ns_drop_scatter_rows_kernel<<<groups_grid(n, D), 256, 0, st>>>(ma, dA, D, triples, ca, n, d_ent, lde, pe);
+      B2K_LAUNCH_CHECK("ns_drop_scatter_rows_kernel");
+      ns_drop_scatter_rows_kernel<<<groups_grid(n, Dr), 256, 0, st>>>(mp, dP, Dr, triples, 1, n, d_rel, ldr, pr);
+      B2K_LAUNCH_CHECK("ns_drop_scatter_rows_kernel");
+      return 0;
+    }
     ns_drop_scatter_kernel<<<groups_grid(n, D), 256, 0, st>>>(ma, dA, D, triples, ca, n, d_ent, lde);
     B2K_LAUNCH_CHECK("ns_drop_scatter_kernel");
     ns_drop_scatter_kernel<<<groups_grid(n, Dr), 256, 0, st>>>(mp, dP, Dr, triples, 1, n, d_rel, ldr);
@@ -401,7 +449,7 @@ int launch_ns_dropout(int model, float l_norm, const Rows& ent, const Rows& rel,
       ops[c] = ns_op(tab, triples + c, 3, K, mk(c == 1, 3 + c, triple ? rb * K : rb), triple ? 1 : K, 0);
   }
   return launch_drop_triples(model, bwd, ops[0], ops[1], ops[2], n * K, l_norm, triple ? eps : 0.f, G, ldg, out, ldo,
-                             K, 1, d_ent, lde, d_rel, ldr, st);
+                             K, 1, d_ent, lde, d_rel, ldr, st, pe, pr);
 }
 
 }  // namespace b200kge

@@ -429,7 +429,8 @@ int launch_row_lse(const float* z, int64_t ldz, int64_t nq, int64_t E, const int
 // num_rel > 0 (dir < 0 only): the reciprocal layout, rows [n,2n) unfold as sp_ into d_ent[o], d_rel[p + num_rel]
 int launch_unfold_distance(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n, int dir,
                            const float* dQ, int64_t ldq, float* d_ent, int64_t lde, float* d_rel, int64_t ldr,
-                           cudaStream_t st, int64_t num_rel = 0);
+                           cudaStream_t st, int64_t num_rel = 0, const int32_t* pe = nullptr,
+                           const int32_t* pr = nullptr);
 int launch_grad_planes_csr(const float* z, int64_t ldz, int64_t nq, int64_t E, const int64_t* csr_off,
                            const int64_t* csr_col, float a, float b, float* row_stat, float offset, float inv_n,
                            void* g_hi, void* g_lo, int64_t Ep, void* gt_hi, void* gt_lo, int64_t Np, float* g_scale,
@@ -444,11 +445,12 @@ int launch_csr_rows(int loss_kind, const int64_t* off, const int64_t* col, const
 int launch_rows_sum(const float* rows, int64_t n, float scale, float* out, cudaStream_t st);
 int launch_row_score_sums(const float* Q, int64_t ldq, int64_t n, const float* T, int64_t ldt, int64_t E, int K,
                           float* scratch, float* zsum, cudaStream_t st);
-// G (optional, [n, 1+K], row stride ldg): dL/dz already scaled, read instead of the BCE gradient
+// G (optional, [n, 1+K], row stride ldg): dL/dz already scaled, read instead of the BCE gradient.  pe / pr (both or
+// neither): row maps, entity e's gradient row is d_ent + pe[e] * lde, relation r's d_rel + pr[r] * ldr.
 int launch_ns_backward(int model, float l_norm, const Rows& ent, const Rows& rel, const int64_t* triples, int slot,
                        const int64_t* neg, int64_t n, int64_t K, float offset, float inv_batch, const float* G,
                        int64_t ldg, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, float* dQ, int64_t ldq,
-                       cudaStream_t st);
+                       cudaStream_t st, const int32_t* pe = nullptr, const int32_t* pr = nullptr);
 // row-wise KgeLoss of a negative-sampling block (ns_loss.cu): part[2 i] = row loss (BCE finaliser layout), G optional
 int launch_ns_loss(int loss_kind, const float* scores, int64_t lds, int64_t n, int64_t m, const int64_t* label_idx,
                    float arg, float temperature, float scale, float* part, float* G, int64_t ldg, cudaStream_t st);
@@ -457,6 +459,6 @@ int launch_penalty(const Rows& tab, const float* counts, float p, int complex_ab
 int launch_normalize_rows(float* w, int64_t ld, int64_t rows, int dim, float p, cudaStream_t st);
 int launch_unfold(int model, const Rows& ent, const Rows& rel, const int64_t* triples, int64_t n, int dir,
                   const float* dQ, int64_t ldq, float* d_ent, int64_t lde, float* d_rel, int64_t ldr, cudaStream_t st,
-                  int64_t num_rel = 0);
+                  int64_t num_rel = 0, const int32_t* pe = nullptr, const int32_t* pr = nullptr);
 
 }  // namespace b200kge

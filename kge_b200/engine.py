@@ -883,6 +883,65 @@ def ns_backward(model: str, ent, rel, triples, negatives: dict, offset: float = 
     return d_ent, d_rel
 
 
+def ns_backward_sparse(model: str, ent, rel, triples, slot: int, negatives, offset: float = 0.0, l_norm: float = 1.0,
+                       batch_size: Optional[int] = None, grad_scores=None, dropout: Optional["DropoutKey"] = None,
+                       implementation: str = "batch", sparse=(True, True)):
+    """(d_ent, d_rel) of one slot of a negative-sampling batch, as ns_backward, with each table's gradient in the layout
+    of LibKGE's `lookup_embedder.sparse` (b200kge_ns_backward_sparse).  sparse = (entities, relations): a dense [V, D]
+    tensor where False; where True a coalesced torch.sparse_coo_tensor over the rows the reference looks up for the slot
+    (the positives' s and o and every sampled id; the positives' p), or over every row of the entity table for
+    implementation "all", whose open slot goes through embed_all().  "all" draws the dropout masks of "batch".
+    grad_scores is the slot's [n, 1+K] block (or None: BCE with `offset` / batch_size).  The two row counts are read
+    back with one device-to-host copy."""
+    _require_cuda(ent, rel, triples, negatives)
+    lib, k = _lib.load(), _Keep()
+    re_, rr = k.rows(ent), k.rows(rel)
+    tri, ng = _i64_block(triples), _i64_block(negatives)
+    n, K = tri.shape[0], ng.shape[1]
+    E, R, D = ent.shape[0], rel.shape[0], ent.shape[1]
+    dev = ent.device
+    if dropout is not None and grad_scores is None:
+        raise ValueError("ns_backward_sparse with dropout needs grad_scores (e.g. the G of ns_loss(..., want_grad=True))")
+    g = None
+    if grad_scores is not None:
+        _require_cuda(grad_scores)
+        if grad_scores.shape != (n, K + 1):
+            raise ValueError(f"grad_scores has shape {tuple(grad_scores.shape)}, expected {(n, K + 1)}")
+        g = _f32_rows(grad_scores)
+    # embed_all() looks up every entity row: the dense gradient is the value block of the full row set
+    ent_rows_all = sparse[0] and implementation == "all"
+    flags = (int(sparse[0] and not ent_rows_all), int(sparse[1]))
+    caps = (min(E, n * (K + 2)), min(R, n))
+    counts = torch.zeros(2, dtype=torch.int64, device=dev)
+    outs = []
+    for f, tab, cap in ((flags[0], ent, caps[0]), (flags[1], rel, caps[1])):
+        if f:
+            outs.append((torch.empty(cap, dtype=torch.int64, device=dev),
+                         torch.empty((cap, tab.shape[1]), dtype=torch.float32, device=dev)))
+        else:
+            outs.append((None, torch.zeros_like(_f32(tab))))
+    (er, ev), (rr_, rv) = outs
+    nbytes = lib.b200kge_ns_backward_sparse_workspace_bytes(MODELS[model], n, K, D, E, R, 0 if dropout is None else 1)
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    _lib.check(lib.b200kge_ns_backward_sparse(
+        MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), int(slot), ng.data_ptr(), n, K,
+        0 if dropout is None else NS_IMPL[implementation],
+        None if dropout is None else C.byref(dropout.struct()), g.data_ptr() if g is not None else None,
+        g.stride(0) if g is not None else 0, offset, batch_size or n,
+        flags[0], er.data_ptr() if flags[0] else None, counts.data_ptr() if flags[0] else None, ev.data_ptr(),
+        ev.stride(0), flags[1], rr_.data_ptr() if flags[1] else None, counts[1:].data_ptr() if flags[1] else None,
+        rv.data_ptr(), rv.stride(0), ws.data_ptr(), ws.numel(), _stream(dev)))
+    u = counts.tolist() if (flags[0] or flags[1]) else (0, 0)
+
+    def layout(flag, rows, vals, V, want_sparse, u_):
+        if flag:
+            return torch.sparse_coo_tensor(rows[None, :u_], vals[:u_], (V, vals.shape[1]), is_coalesced=True)
+        if want_sparse:       # "all": every row
+            return torch.sparse_coo_tensor(torch.arange(V, device=dev)[None, :], vals, vals.shape, is_coalesced=True)
+        return vals
+    return (layout(flags[0], er, ev, E, ent_rows_all, u[0]), layout(flags[1], rr_, rv, R, False, u[1]))
+
+
 def ns_loss(scores, loss: str, arg: float = 0.0, temperature: float = 1.0, label_idx=None,
             batch_size: Optional[int] = None, want_grad: bool = False, return_rows: bool = False):
     """KgeLoss of a negative-sampling block (train_negative_sampling.py:126-156): scores [n, m] with one positive per

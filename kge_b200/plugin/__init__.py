@@ -167,8 +167,18 @@ def _penalty_torch(emb, w, regularize, rw, p, weighted, indexes):
     return (rw / p * (par ** p * counts.float().view(-1, 1))).sum() / len(indexes)
 
 
+def _sparse_scaled(d, g):
+    """d * g for a dense or a coalesced sparse COO gradient (only the values are scaled)."""
+    if not d.is_sparse:
+        return d * g
+    return torch.sparse_coo_tensor(d._indices(), d._values() * g, d.shape, is_coalesced=True)
+
+
 class _PenaltyFn(torch.autograd.Function):
-    """Forward: the Lp / N3 row kernel (b200kge_lookup_penalty).  Backward: autograd of the reference expression."""
+    """Forward: the Lp / N3 row kernel (b200kge_lookup_penalty).  Backward: autograd of the reference expression; for
+    a `sparse: True` embedder row-sparse over the rows the reference looks up: the unique indexes of the weighted
+    penalty (self._embeddings(unique_indexes), lookup_embedder.py:155), every row of the unweighted one
+    (self._embeddings_all(), :139)."""
 
     @staticmethod
     def forward(ctx, w, emb, regularize, rw, p, weighted, indexes):
@@ -182,6 +192,16 @@ class _PenaltyFn(torch.autograd.Function):
         wd = w.detach().requires_grad_(True)
         with torch.enable_grad():
             (gw,) = torch.autograd.grad(_penalty_torch(ctx.args[0], wd, *ctx.args[1:]), wd)
+        emb, weighted, indexes = ctx.args[0], ctx.args[4], ctx.args[5]
+        if emb.sparse:
+            if weighted:
+                rows = torch.unique(indexes).long()
+                vals = gw[rows] * g
+            else:
+                rows = torch.arange(gw.shape[0], device=gw.device)
+                vals = gw * g
+            return (torch.sparse_coo_tensor(rows[None, :], vals, gw.shape, is_coalesced=True),
+                    None, None, None, None, None, None)
         return gw * g, None, None, None, None, None, None
 
 
@@ -271,7 +291,8 @@ class _NsSlotLossFn(torch.autograd.Function):
     writes G = dL/dscores, and the backward reads G (b200kge_ns_backward with grad_scores).  With a dropout key (engine.DropoutKey)
     the forward scores the masked block (b200kge_ns_score_dropout, draws of `implementation`), every loss BCE included
     runs the row-loss kernel, and the backward regenerates the same masks from the key (b200kge_ns_backward with the
-    key)."""
+    key).  When an embedder has `sparse: True` the backward is b200kge_ns_backward_sparse instead: that table's
+    gradient is row-sparse over the rows the reference looks up (every entity row for `implementation` "all")."""
 
     @staticmethod
     def forward(ctx, ent_w, rel_w, model, triples, negatives, slot, offset, batch_size, loss="bce", temperature=1.0,
@@ -297,6 +318,16 @@ class _NsSlotLossFn(torch.autograd.Function):
     def backward(ctx, g):
         model, slot, offset, batch_size, loss, dropout, implementation = ctx.args
         ent_w, rel_w, triples, negatives = ctx.saved_tensors[:4]
+        sparse = model.b200_sparse_grads()
+        if any(sparse):
+            kw = {"sparse": sparse, "implementation": implementation}
+            if dropout is not None or loss != "bce":
+                kw["grad_scores"] = ctx.saved_tensors[4]
+            if dropout is not None:
+                kw["dropout"] = dropout
+            d_ent, d_rel = engine.ns_backward_sparse(model._b200_name, ent_w.detach(), rel_w.detach(), triples, slot,
+                                                     negatives, offset, model._b200_args()[0], batch_size, **kw)
+            return (_sparse_scaled(d_ent, g), _sparse_scaled(d_rel, g)) + (None,) * 10
         if dropout is not None:
             kw = {"grad_scores": {slot: ctx.saved_tensors[4]}, "dropout": dropout, "implementation": implementation}
         else:
@@ -585,6 +616,11 @@ class _B200ModelMixin:
     def loss_dense(self, scores, labels, loss="bce", offset=0.0):
         return engine.loss_dense(scores, labels, loss, offset)
 
+    def b200_sparse_grads(self):
+        """(entities, relations): whether each table's embedder asks for row-sparse gradients (`lookup_embedder.sparse`,
+        nn.Embedding(sparse=True), lookup_embedder.py:36,45)."""
+        return bool(self.get_s_embedder().sparse), bool(self.get_p_embedder().sparse)
+
     def b200_ns_native_backward_ok(self, slot):
         """The fused NS gradient kernel covers the S / O slots of the dot family, TransE (L1, L2) and RotatE (L1)."""
         if self.b200_backward != "native" or slot not in (0, 2):
@@ -597,7 +633,9 @@ class _B200ModelMixin:
         """KgeLoss of one slot's [n, 1+K] block (positive first) / batch_size, differentiable through the gradient
         kernel (train_negative_sampling.py:139-164).  `loss` is a name of engine.ns_loss; `offset` its argument (the BCE
         offset, or the margin of margin_ranking), `temperature` that of bce_self_adversarial.  `dropout` (an
-        engine.DropoutKey) applies the slot's embedding-dropout draws of `implementation` in forward and backward."""
+        engine.DropoutKey) applies the slot's embedding-dropout draws of `implementation` in forward and backward; "all"
+        draws those of "batch".  With a `sparse: True` embedder `implementation` also picks the row set of the sparse
+        gradients (see _NsSlotLossFn)."""
         ent_w, rel_w = self._b200_weights()
         return _NsSlotLossFn.apply(ent_w, rel_w, self, triples.long().contiguous(), negatives.long().contiguous(),
                                    int(slot), float(offset), int(batch_size), loss, float(temperature), dropout,

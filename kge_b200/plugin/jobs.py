@@ -513,6 +513,9 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
         # "all" draws the masks of "batch" (embed_all() gives the same distribution); `auto` is resolved by _prepare
         impl = "triple" if getattr(self, "_implementation", "batch") == "triple" else "batch"
         dkw = {} if drop is None else {"dropout": drop, "implementation": impl}
+        if model is not None and any(model.b200_sparse_grads()):
+            # the row set of a sparse gradient: `all` scores against embed_all(), so every entity row is in it
+            dkw["implementation"] = getattr(self, "_implementation", "batch")
         if model is None or (not self.is_forward_only and not trainable):
             if self._device_sampling:
                 raise NotImplementedError("user.b200_device_sampling needs a b200_* model whose slots the fused "
