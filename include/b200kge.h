@@ -687,6 +687,46 @@ int b200kge_ns_backward_sparse(int model, float l_norm, const b200kge_rows_t* en
                                int64_t lde, int rel_sparse, int64_t* rel_rows, int64_t* rel_count, float* d_rel,
                                int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
 
+/* ---- Optimizer steps: torch.optim.Adagrad and torch.optim.SparseAdam (torch 2.11) on one fp32 parameter ----------------
+ * param and its state tensors are [rows, dim], contiguous.  The gradient is
+ *   dense      (grad_rows == NULL): grad [rows, dim], contiguous; nnz and coalesced are unused;
+ *   row-sparse (a torch.sparse_coo_tensor with one sparse dimension): grad_rows [nnz] row ids and grad [nnz, dim] their
+ *              value rows.  coalesced != 0 promises sorted unique ids (torch's is_coalesced()): the block is read in
+ *              place and no workspace is needed.  Otherwise ids may repeat in any order; their rows are summed (in
+ *              any order, with atomics) into a [min(rows, nnz), dim] block of the workspace first, over the row set of
+ *              the ids (rowset.cu); tables of 2^31 rows or more then return B200KGE_ERR_UNSUPPORTED.
+ * Rows not in a sparse gradient are neither read nor written.  Every operation rounds to nearest in the order written
+ * below, with a single rounding exactly where torch's compiled kernels use an FMA (fma(...) below); with a dense or
+ * coalesced gradient the result is then torch's bit for bit, as far as torch's kernels keep that rounding.
+ * The caller computes the scalars in double precision, as torch does, and passes them rounded to float.
+ * workspace: b200kge_optim_step_workspace_bytes(rows, dim, nnz, coalesced) (0 for a coalesced gradient; pass
+ * coalesced = 1 for a dense one).  NULL operands, negative sizes and a short workspace are refused before any launch. */
+size_t b200kge_optim_step_workspace_bytes(int64_t rows, int64_t dim, int64_t nnz, int coalesced);
+
+/* One parameter of torch.optim.Adagrad.step() (adagrad.py), after the caller has incremented the step and computed
+ * clr = lr / (1 + (step - 1) lr_decay).  Dense: g' = fma(weight_decay, p, g) when weight_decay != 0,
+ * sum = fma(g', g', sum), then
+ *   foreach_order != 0 (_multi_tensor_adagrad, torch's default on CUDA):  p = p + (g' (-clr)) / (sqrt(sum) + eps)
+ *   foreach_order == 0 (_single_tensor_adagrad: foreach=False, or a group with a sparse gradient on the device):
+ *                                                                        p = fma(g' / (sqrt(sum) + eps), -clr, p)
+ * Row-sparse, per row of the coalesced gradient, value v: sum = sum + v v, p = p + (-clr) (v / (sqrt(sum) + eps)),
+ * every operation rounded on its own; weight_decay != 0 is refused
+ * (B200KGE_ERR_INVALID, torch's "weight_decay option is not compatible with sparse gradients"). */
+int b200kge_adagrad_step(float* param, float* state_sum, int64_t rows, int64_t dim, const float* grad,
+                         const int64_t* grad_rows, int64_t nnz, int coalesced, int foreach_order, float clr, float eps,
+                         float weight_decay, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+
+/* One parameter of torch.optim.SparseAdam.step() (_functional.sparse_adam) with the step t already incremented and
+ * step_size = lr sqrt(1 - beta2^t) / (1 - beta1^t).  one_minus_beta1 / one_minus_beta2 are 1 - beta computed in double,
+ * as torch's scalars are.  Per row of the coalesced gradient, value v:
+ *   m_u = (v - m)(1 - beta1), m += m_u;  q_u = (v v - q)(1 - beta2), q += q_u;
+ *   p += (-step_size) ((m_u + m_old) / (sqrt(q_u + q_old) + eps))
+ * with m = exp_avg, q = exp_avg_sq.  A dense gradient (grad_rows == NULL) is refused (B200KGE_ERR_INVALID). */
+int b200kge_sparse_adam_step(float* param, float* exp_avg, float* exp_avg_sq, int64_t rows, int64_t dim,
+                             const float* grad, const int64_t* grad_rows, int64_t nnz, int coalesced,
+                             float one_minus_beta1, float one_minus_beta2, float eps, float step_size, void* workspace,
+                             size_t workspace_bytes, b200kge_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

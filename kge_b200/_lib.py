@@ -133,6 +133,13 @@ SIGNATURES = {
                                              C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                              C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                              C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_optim_step_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64, C.c_int]),
+    "b200kge_adagrad_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
+                                       C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_size_t,
+                                       C.c_void_p]),
+    "b200kge_sparse_adam_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
+                                           C.c_void_p, C.c_int64, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float,
+                                           C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_ns_loss_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "b200kge_ns_loss": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_float, C.c_float,
                                   C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t,

@@ -2058,4 +2058,55 @@ int b200kge_ns_backward_sparse(int model, float l_norm, const b200kge_rows_t* en
                             d_rel, ldr, (float*)ws_ns, ldq, st, pe, pr);
 }
 
+
+// The checks shared by the two optimizer steps: operands, sizes and the workspace of a row-sparse gradient
+static int check_optim_step(const float* param, const float* state0, const float* state1, int64_t rows, int64_t dim,
+                            const float* grad, const int64_t* grad_rows, int64_t nnz, int coalesced, void* workspace,
+                            size_t workspace_bytes) {
+  if (rows < 0 || dim <= 0 || (grad_rows && nnz < 0)) { set_error("negative sizes"); return B200KGE_ERR_INVALID; }
+  const bool any = grad_rows ? nnz > 0 : rows > 0;
+  if (!param || !state0 || !state1 || (any && !grad)) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (!grad_rows) return 0;
+  if (!coalesced && rows > INT32_MAX) { set_error("the row map covers tables of fewer than 2^31 rows"); return B200KGE_ERR_UNSUPPORTED; }
+  const size_t need = b200kge_optim_step_workspace_bytes(rows, dim, nnz, coalesced);
+  if (need && (!workspace || workspace_bytes < need)) {
+    set_error("workspace too small (need b200kge_optim_step_workspace_bytes = %zu bytes)", need);
+    return B200KGE_ERR_WORKSPACE;
+  }
+  return 0;
+}
+
+size_t b200kge_optim_step_workspace_bytes(int64_t rows, int64_t dim, int64_t nnz, int coalesced) {
+  return optim_step_workspace_bytes(rows, dim, nnz, coalesced);
+}
+
+int b200kge_adagrad_step(float* param, float* state_sum, int64_t rows, int64_t dim, const float* grad,
+                         const int64_t* grad_rows, int64_t nnz, int coalesced, int foreach_order, float clr, float eps,
+                         float weight_decay, void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+  int rc = check_optim_step(param, state_sum, state_sum, rows, dim, grad, grad_rows, nnz, coalesced, workspace,
+                            workspace_bytes);
+  if (rc) return rc;
+  if (grad_rows && weight_decay != 0.f) {
+    set_error("weight_decay option is not compatible with sparse gradients");
+    return B200KGE_ERR_INVALID;
+  }
+  return launch_adagrad_step(param, state_sum, rows, dim, grad, grad_rows, nnz, coalesced, foreach_order, clr, eps,
+                             weight_decay, workspace, (cudaStream_t)stream);
+}
+
+int b200kge_sparse_adam_step(float* param, float* exp_avg, float* exp_avg_sq, int64_t rows, int64_t dim,
+                             const float* grad, const int64_t* grad_rows, int64_t nnz, int coalesced,
+                             float one_minus_beta1, float one_minus_beta2, float eps, float step_size, void* workspace,
+                             size_t workspace_bytes, b200kge_stream_t stream) {
+  if (!grad_rows) {
+    set_error("SparseAdam does not support dense gradients, please consider Adam instead");
+    return B200KGE_ERR_INVALID;
+  }
+  int rc = check_optim_step(param, exp_avg, exp_avg_sq, rows, dim, grad, grad_rows, nnz, coalesced, workspace,
+                            workspace_bytes);
+  if (rc) return rc;
+  return launch_sparse_adam_step(param, exp_avg, exp_avg_sq, rows, dim, grad, grad_rows, nnz, coalesced,
+                                 one_minus_beta1, one_minus_beta2, eps, step_size, workspace, (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -527,4 +527,14 @@ int launch_row_set(int64_t V, const IdList* lists, int nlists, void* workspace, 
 // map[id] = id for id < V at the start of the workspace: a dense table through the row-mapped kernels
 int launch_identity_map(int64_t V, void* workspace, cudaStream_t st);
 
+// Optimizer steps (optim.cu), operands as b200kge_adagrad_step / b200kge_sparse_adam_step; arguments already checked.
+size_t optim_step_workspace_bytes(int64_t rows, int64_t dim, int64_t nnz, int coalesced);
+int launch_adagrad_step(float* param, float* state_sum, int64_t rows, int64_t dim, const float* grad,
+                        const int64_t* grad_rows, int64_t nnz, int coalesced, int foreach_order, float clr, float eps,
+                        float weight_decay, void* workspace, cudaStream_t st);
+int launch_sparse_adam_step(float* param, float* exp_avg, float* exp_avg_sq, int64_t rows, int64_t dim,
+                            const float* grad, const int64_t* grad_rows, int64_t nnz, int coalesced,
+                            float one_minus_beta1, float one_minus_beta2, float eps, float step_size, void* workspace,
+                            cudaStream_t st);
+
 }  // namespace b200kge

@@ -1062,3 +1062,69 @@ def score_so_loss_csr_backward(model: str, ent, rel, s, o, csr_offsets, csr_cols
         None if dropout is None else C.byref(dropout.struct()), d_ent.data_ptr(), d_ent.stride(0), d_rel.data_ptr(),
         d_rel.stride(0), ws.data_ptr(), ws.numel(), _stream(dev)))
     return d_ent, d_rel
+
+
+def _optim_operands(param, state, grad):
+    """(rows, dim, grad values, grad row ids or None, nnz, coalesced) of one optimizer step: param and its state as
+    contiguous fp32 CUDA tensors viewed [rows, dim], the gradient dense or a COO tensor with one sparse dimension."""
+    _require_cuda(param, grad, *state)
+    for t in (param, *state):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.layout != torch.strided:
+            raise TypeError("the optimizer step takes contiguous float32 parameters and state")
+        if t.shape != param.shape:
+            raise ValueError(f"state of shape {tuple(t.shape)} for a parameter of shape {tuple(param.shape)}")
+    if grad.shape != param.shape:
+        raise ValueError(f"gradient of shape {tuple(grad.shape)} for a parameter of shape {tuple(param.shape)}")
+    rows = param.shape[0] if param.dim() > 0 and param.numel() > 0 else (1 if param.numel() else 0)
+    dim = param.numel() // rows if rows > 0 else 1
+    if not grad.is_sparse:
+        g = grad if (grad.dtype == torch.float32 and grad.is_contiguous()) else grad.float().contiguous()
+        return rows, dim, g, None, 0, 1
+    if grad.sparse_dim() != 1:
+        raise NotImplementedError(f"a sparse gradient with {grad.sparse_dim()} sparse dimensions (the optimizer step "
+                                  "takes row-sparse gradients: one sparse dimension)")
+    idx, vals = grad._indices()[0], grad._values()
+    idx = idx if idx.is_contiguous() else idx.contiguous()
+    vals = vals if (vals.dtype == torch.float32 and vals.is_contiguous()) else vals.float().contiguous()
+    return rows, dim, vals, idx, idx.numel(), int(grad.is_coalesced())
+
+
+def _optim_workspace(lib, rows, dim, nnz, coalesced, idx, dev):
+    nbytes = lib.b200kge_optim_step_workspace_bytes(rows, dim, nnz, coalesced) if idx is not None else 0
+    return torch.empty(nbytes, dtype=torch.uint8, device=dev) if nbytes else None
+
+
+def adagrad_step(param, state_sum, grad, clr: float, eps: float, weight_decay: float = 0.0,
+                 foreach_order: bool = True) -> None:
+    """One parameter of torch.optim.Adagrad.step() in place (b200kge_adagrad_step): param and state_sum (the state's
+    "sum") are updated with grad, dense or a torch.sparse_coo_tensor of value rows, coalesced or not.  clr is
+    lr / (1 + (step - 1) lr_decay) after the step count was incremented; foreach_order selects the order of torch's
+    _multi_tensor_adagrad (True) or _single_tensor_adagrad (False) for a dense gradient.  Runs on the parameter's
+    current stream; the workspace of an uncoalesced gradient comes from torch's caching allocator."""
+    lib = _lib.load()
+    rows, dim, g, idx, nnz, coalesced = _optim_operands(param, (state_sum,), grad)
+    if rows * dim == 0 or (idx is not None and nnz == 0):
+        return
+    ws = _optim_workspace(lib, rows, dim, nnz, coalesced, idx, param.device)
+    _lib.check(lib.b200kge_adagrad_step(
+        param.data_ptr(), state_sum.data_ptr(), rows, dim, g.data_ptr(), None if idx is None else idx.data_ptr(), nnz,
+        coalesced, int(bool(foreach_order)), float(clr), float(eps), float(weight_decay),
+        None if ws is None else ws.data_ptr(), 0 if ws is None else ws.numel(), _stream(param.device)))
+
+
+def sparse_adam_step(param, exp_avg, exp_avg_sq, grad, beta1: float, beta2: float, eps: float,
+                     step_size: float) -> None:
+    """One parameter of torch.optim.SparseAdam.step() in place (b200kge_sparse_adam_step) with a torch.sparse_coo_tensor
+    gradient, coalesced or not: step_size = lr sqrt(1 - beta2^t) / (1 - beta1^t) after the step count t was
+    incremented.  1 - beta is formed here in double precision, as torch forms it."""
+    lib = _lib.load()
+    if not grad.is_sparse:
+        raise RuntimeError("SparseAdam does not support dense gradients, please consider Adam instead")
+    rows, dim, g, idx, nnz, coalesced = _optim_operands(param, (exp_avg, exp_avg_sq), grad)
+    if rows * dim == 0 or nnz == 0:
+        return
+    ws = _optim_workspace(lib, rows, dim, nnz, coalesced, idx, param.device)
+    _lib.check(lib.b200kge_sparse_adam_step(
+        param.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(), rows, dim, g.data_ptr(), idx.data_ptr(), nnz,
+        coalesced, float(1.0 - beta1), float(1.0 - beta2), float(eps), float(step_size),
+        None if ws is None else ws.data_ptr(), 0 if ws is None else ws.numel(), _stream(param.device)))

@@ -46,6 +46,7 @@ from kge.util.loss import (BCEWithLogitsKgeLoss, KLDivWithSoftmaxKgeLoss, Margin
 from kge.util.sampler import KgeSampler
 
 from .. import engine
+from ..optim import install_native_step
 
 S, P, O = 0, 1, 2
 SLOT_STR = ["s", "p", "o"]
@@ -133,6 +134,21 @@ def _user_option(config, key, default=None):
         return default
 
 
+class _NativeOptimizer:
+    """`user.b200_native_optimizer: true`: the training job's optimizer (Adagrad or SparseAdam) steps on the library's
+    kernels (kge_b200.optim).  Only `step` of the instance is replaced; its state and state_dict() stay torch's, so
+    checkpoints resume with the option on or off.  A configuration the native step cannot serve raises when the job
+    is created."""
+
+    def _b200_native_optimizer(self):
+        if self.is_forward_only or not _user_option(self.config, "b200_native_optimizer", False):
+            return
+        try:
+            install_native_step(self.optimizer)
+        except NotImplementedError as e:
+            raise NotImplementedError(f"user.b200_native_optimizer: {e}") from None
+
+
 class _BatchSplit:
     """Replicas + batch split over the processes of a torch.distributed group (SURVEY 8e, "small tables": every GPU
     holds the whole tables, scores its share of the batch's rows against them, and the dense table gradients are
@@ -189,12 +205,13 @@ class _BatchSplit:
         return result
 
 
-class B200TrainingJob1vsAll(_DropoutKeys, _BatchSplit, TrainingJob1vsAll):
+class B200TrainingJob1vsAll(_DropoutKeys, _NativeOptimizer, _BatchSplit, TrainingJob1vsAll):
     """`TrainingJob1vsAll` (train_1vsAll.py:10-82) with the sub-batch step as ONE fused call:
     (loss(score_sp, o) + loss(score_po, s)) / batch_size, both directions stacked into one problem."""
 
     def __init__(self, config, dataset, parent_job=None, model=None, forward_only=False):
         super().__init__(config, dataset, parent_job, model=model, forward_only=forward_only)
+        self._b200_native_optimizer()
         if self.__class__ == B200TrainingJob1vsAll:
             for f in Job.job_created_hooks:
                 f(self)
@@ -252,7 +269,7 @@ class B200TrainingJob1vsAll(_DropoutKeys, _BatchSplit, TrainingJob1vsAll):
         result.backward_time += time.time()
 
 
-class B200TrainingJobKvsAll(_DropoutKeys, _BatchSplit, TrainingJobKvsAll):
+class B200TrainingJobKvsAll(_DropoutKeys, _NativeOptimizer, _BatchSplit, TrainingJobKvsAll):
     """`TrainingJobKvsAll` (train_KvsAll.py:205-294): per query type one fused score+loss call that consumes the
     batch's label coordinates as CSR (no dense [n, E] label matrix: job/util.py:32-60 + `.to_dense()`,
     train_KvsAll.py:242-266 are not executed).  The s_o query type (relation prediction) is served for the dot family
@@ -260,6 +277,7 @@ class B200TrainingJobKvsAll(_DropoutKeys, _BatchSplit, TrainingJobKvsAll):
 
     def __init__(self, config, dataset, parent_job=None, model=None, forward_only=False):
         super().__init__(config, dataset, parent_job, model=model, forward_only=forward_only)
+        self._b200_native_optimizer()
         if self.__class__ == B200TrainingJobKvsAll:
             for f in Job.job_created_hooks:
                 f(self)
@@ -367,7 +385,7 @@ class B200FrequencySampler(KgeSampler):
                                   "B200TrainingJobNegativeSampling with user.b200_device_sampling: true")
 
 
-class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNegativeSampling):
+class B200TrainingJobNegativeSampling(_DropoutKeys, _NativeOptimizer, _BatchSplit, TrainingJobNegativeSampling):
     """`TrainingJobNegativeSampling` (train_negative_sampling.py:103-164): per slot ONE kernel gathers the sampled
     rows and scores them, with the positive triple in column 0 — neither `[n*K, D]` gathers (`triple`
     implementation, sampler.py:294-305) nor scoring against all unique targets (`batch`, :306-339).
@@ -401,6 +419,7 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _BatchSplit, TrainingJobNega
         self._frequency = self._b200_frequency_tables() if frequency else {}
         self._filter_index = self._b200_filter_indexes() if self._device_sampling else {}
         self._sample_calls = 0
+        self._b200_native_optimizer()
         if self.__class__ == B200TrainingJobNegativeSampling:
             for f in Job.job_created_hooks:
                 f(self)
