@@ -687,6 +687,36 @@ int b200kge_ns_backward_sparse(int model, float l_norm, const b200kge_rows_t* en
                                int64_t lde, int rel_sparse, int64_t* rel_rows, int64_t* rel_count, float* d_rel,
                                int64_t ldr, void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
 
+/* Backward of the P slot of a negative-sampling batch (relation negatives; train_negative_sampling.py:139-164 with
+ * sampler.py:263-356 through score_so): row i of the [n, 1+K] block scores (s_i, r, o_i) for r = p_i (column 0) and for
+ * the K sampled relation ids neg [n, K].  grad_scores [n, 1+K] (row stride ldg) is dL/dz, required for every loss (BCE
+ * included: the grad_out of b200kge_ns_loss with scale = 1 / batch_size).
+ * The score depends on (i, r) only, so G is first summed exactly into C [n, R] with C[i, r] = the sum of row i's
+ * columns whose id is r; the backward is then the all-relations backward with weights C:
+ *   dot family (ComplEx, DistMult, SimplE, CP, RESCAL): the s_o fold Q [n, K_r], d_rel = C^T Q and dQ = C rel on the
+ *     split-K tensor-core GEMMs, the s_o unfold into the rows s_i and o_i;
+ *   TransE (l_norm 1, 2) and RotatE (l_norm 1): the VJP of the row score over the nonzero C[i, r] on the CUDA cores,
+ *     one block per row for the entity rows and one per (relation, chunk of rows) for the relation rows.
+ * No per-sample contribution is added atomically into the relation table.  Per table, `*_sparse`:
+ *   0: d_ent [E, lde] / d_rel [R, ldr] is the dense gradient, ADDED into; rows / count unused.
+ *   1: row-sparse, as b200kge_ns_backward_sparse: rows receives the sorted unique rows the reference looks up for the
+ *      slot, *count (device, int64) their number u, and rows 0 .. u-1 of the value block their gradients, OVERWRITTEN.
+ *      Entity rows: the positives' s and o, at most min(E, 2n); relation rows: the positives' p and every sampled id,
+ *      at most min(R, n (K + 1)).  (With the reference's `implementation: all` score_so looks up every relation row:
+ *      pass rel_sparse = 0 and read the dense gradient as the values of all R rows.)
+ * Ids must lie in their tables.  Other models and norms, R > B200KGE_NS_P_MAX_RELATIONS and tables of 2^31 rows or
+ * more return B200KGE_ERR_UNSUPPORTED before any launch; there is no dropout form.
+ * workspace: b200kge_ns_p_backward_workspace_bytes(model, n, K, D, E, R): C [n, R] floats, four [n] id vectors, the
+ * row-set maps, and the dot family's fold and GEMM operands (about 2 n R + R K_r + 3 n K_r floats beyond C) or the
+ * distance family's relation partials (at most max(R, 4096) K_r floats).  0 for R > B200KGE_NS_P_MAX_RELATIONS. */
+#define B200KGE_NS_P_MAX_RELATIONS 4096
+size_t b200kge_ns_p_backward_workspace_bytes(int model, int64_t n, int64_t K, int32_t D, int64_t E, int64_t R);
+int b200kge_ns_p_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                          const int64_t* triples, const int64_t* neg, int64_t n, int64_t K, const float* grad_scores,
+                          int64_t ldg, int ent_sparse, int64_t* ent_rows, int64_t* ent_count, float* d_ent, int64_t lde,
+                          int rel_sparse, int64_t* rel_rows, int64_t* rel_count, float* d_rel, int64_t ldr,
+                          void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
+
 /* ---- Optimizer steps: torch.optim.Adagrad and torch.optim.SparseAdam (torch 2.11) on one fp32 parameter ----------------
  * param and its state tensors are [rows, dim], contiguous.  The gradient is
  *   dense      (grad_rows == NULL): grad [rows, dim], contiguous; nnz and coalesced are unused;

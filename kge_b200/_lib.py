@@ -133,6 +133,12 @@ SIGNATURES = {
                                              C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                              C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                              C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_ns_p_backward_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32, C.c_int64,
+                                                            C.c_int64]),
+    "b200kge_ns_p_backward": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                        C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                        C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                        C.c_size_t, C.c_void_p]),
     "b200kge_optim_step_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64, C.c_int]),
     "b200kge_adagrad_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
                                        C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_size_t,
@@ -167,6 +173,9 @@ SIGNATURES = {
                                                      C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                                                      C.c_size_t, C.c_void_p]),
 }
+
+#: the most relations b200kge_ns_p_backward serves (B200KGE_NS_P_MAX_RELATIONS)
+NS_P_MAX_RELATIONS = 4096
 
 #: negative-sampling scoring implementations of the dropout entry points (B200KGE_NS_*); "all" draws like "batch"
 NS_IMPL = {"triple": 0, "batch": 1, "all": 1}

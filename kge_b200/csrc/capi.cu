@@ -2058,6 +2058,90 @@ int b200kge_ns_backward_sparse(int model, float l_norm, const b200kge_rows_t* en
                             d_rel, ldr, (float*)ws_ns, ldq, st, pe, pr);
 }
 
+size_t b200kge_ns_p_backward_workspace_bytes(int model, int64_t n, int64_t K, int32_t D, int64_t E, int64_t R) {
+  if (n < 0 || K < 0 || D <= 0 || E < 0 || R < 0 || R > B200KGE_NS_P_MAX_RELATIONS) return 0;
+  const int64_t Kr = relation_dim(model, D), ldc = round_up(R > 0 ? R : 1, 4);
+  // row-set maps, C, s / o ids and destination rows
+  size_t b = row_set_workspace_bytes(E) + row_set_workspace_bytes(R) + (size_t)n * ldc * 4 + 4 * ((size_t)n * 8 + 256) + 4 * 256;
+  if (model == B200KGE_TRANSE || model == B200KGE_ROTATE)
+    return b + (size_t)ns_p_parts(n, R) * R * Kr * 4 + 256;
+  const int64_t ldq = round_up(Kr, 32);
+  // Q, dQ, dT [R, ldq], the backward block
+  return b + 2 * ((size_t)n * ldq * 4 + 256) + (size_t)R * ldq * 4 + 256 + backward_block_bytes(n, R, Kr, ldq);
+}
+
+int b200kge_ns_p_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                          const int64_t* triples, const int64_t* neg, int64_t n, int64_t K, const float* grad_scores,
+                          int64_t ldg, int ent_sparse, int64_t* ent_rows, int64_t* ent_count, float* d_ent, int64_t lde,
+                          int rel_sparse, int64_t* rel_rows, int64_t* rel_count, float* d_rel, int64_t ldr,
+                          void* workspace, size_t workspace_bytes, b200kge_stream_t stream) {
+  if (!triples || (!neg && n * K > 0) || !grad_scores || !d_ent || !d_rel || (ent_sparse && (!ent_rows || !ent_count)) ||
+      (rel_sparse && (!rel_rows || !rel_count))) {
+    set_error("null operand");
+    return B200KGE_ERR_INVALID;
+  }
+  if (n < 0 || K < 0) { set_error("negative sizes"); return B200KGE_ERR_INVALID; }
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
+  if (ldg < K + 1) { set_error("grad_scores is narrower than the 1 + K columns of the block"); return B200KGE_ERR_INVALID; }
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
+  const bool distance = model == B200KGE_TRANSE || model == B200KGE_ROTATE;
+  if ((model == B200KGE_TRANSE && l_norm != 1.0f && l_norm != 2.0f) || (model == B200KGE_ROTATE && l_norm != 1.0f)) {
+    set_error("the P-slot backward covers l_norm 1 and 2 (TransE) / 1 (RotatE)");
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  if (rel->rows > B200KGE_NS_P_MAX_RELATIONS) {
+    set_error("the P-slot backward covers up to %d relations (got %lld)", B200KGE_NS_P_MAX_RELATIONS, (long long)rel->rows);
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  if (ent->rows > INT32_MAX) { set_error("the row maps cover tables of fewer than 2^31 rows"); return B200KGE_ERR_UNSUPPORTED; }
+  const size_t need = b200kge_ns_p_backward_workspace_bytes(model, n, K, ent->dim, ent->rows, rel->rows);
+  if (!workspace || workspace_bytes < need) { set_error("workspace too small (see b200kge_ns_p_backward_workspace_bytes)"); return B200KGE_ERR_WORKSPACE; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const Rows E = to_rows(ent), Rl = to_rows(rel);
+  uint8_t* ws_e = (uint8_t*)workspace;
+  uint8_t* ws_r = ws_e + row_set_workspace_bytes(E.rows);
+  uint8_t* ws_rest = ws_r + row_set_workspace_bytes(Rl.rows);
+  // the rows score_so looks up: the positives' s and o; the positives' p and every sampled id
+  const IdList le[2] = {{triples, n, 3}, {triples + 2, n, 3}};
+  const IdList lr[2] = {{triples + 1, n, 3}, {neg, n * K, 1}};
+  if (ent_sparse && (rc = launch_row_set(E.rows, le, 2, ws_e, ent_rows, ent_count, d_ent, lde, st))) return rc;
+  if (rel_sparse && (rc = launch_row_set(Rl.rows, lr, 2, ws_r, rel_rows, rel_count, d_rel, ldr, st))) return rc;
+  if (n == 0 || Rl.rows == 0) return 0;
+  Arena ws{ws_rest, workspace_bytes - (size_t)(ws_rest - ws_e), 0};
+  const int64_t R = Rl.rows, Kr = Rl.dim, ldc = round_up(R, 4);
+  float* Cw = (float*)ws.take((size_t)n * ldc * 4);
+  int64_t* s_idx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* o_idx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* s_dst = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* o_dst = (int64_t*)ws.take((size_t)n * 8);
+  if (!Cw || !s_idx || !o_idx || !s_dst || !o_dst) { set_error("workspace too small (see b200kge_ns_p_backward_workspace_bytes)"); return B200KGE_ERR_WORKSPACE; }
+  if ((rc = launch_ns_p_unpack(triples, n, ent_sparse ? (const int32_t*)ws_e : nullptr, s_idx, o_idx, s_dst, o_dst, st))) return rc;
+  if ((rc = launch_ns_p_collapse(triples, neg, n, K, grad_scores, ldg, R, Cw, ldc, st))) return rc;
+  const int64_t* rows = rel_sparse ? rel_rows : nullptr;
+  const int64_t* count = rel_sparse ? rel_count : nullptr;
+  if (distance) {
+    const int P = ns_p_parts(n, R);
+    float* parts = (float*)ws.take((size_t)P * R * Kr * 4);
+    if (!parts) { set_error("workspace too small (see b200kge_ns_p_backward_workspace_bytes)"); return B200KGE_ERR_WORKSPACE; }
+    if ((rc = launch_ns_p_distance(model, l_norm, E, Rl, s_idx, o_idx, n, Cw, ldc, d_ent, lde, s_dst, o_dst, parts, st))) return rc;
+    return launch_ns_p_rel_add(parts, Kr, R * Kr, P, R, (int)Kr, rows, count, d_rel, ldr, st);
+  }
+  // dot family: the s_o fold against the relation table, C as the dense gradient of the block
+  const int64_t ldq = round_up(Kr, 32);
+  float* Q = (float*)ws.take((size_t)n * ldq * 4);
+  float* dQ = (float*)ws.take((size_t)n * ldq * 4);
+  float* dT = (float*)ws.take((size_t)R * ldq * 4);
+  if (!Q || !dQ || !dT) { set_error("workspace too small (see b200kge_ns_p_backward_workspace_bytes)"); return B200KGE_ERR_WORKSPACE; }
+  Rows S = E; S.idx = s_idx; S.rows = n;
+  Rows O = E; O.idx = o_idx; O.rows = n;
+  if ((rc = launch_fold_so(model, S, O, n, Q, ldq, st))) return rc;
+  GradSpec g;
+  g.G = Cw; g.ldg = ldc;
+  if ((rc = backward_block(B200KGE_DISTMULT, Rl, Rl, n, B200KGE_SP_, false, Q, ldq, 0, (int)Kr, g, dT, ldq, dQ, ws, st))) return rc;
+  if ((rc = launch_ns_p_rel_add(dT, ldq, 0, 1, R, (int)Kr, rows, count, d_rel, ldr, st))) return rc;
+  return launch_unfold_so(model, S, O, n, dQ, ldq, d_ent, lde, s_dst, d_ent, lde, o_dst, st);
+}
+
 
 // The checks shared by the two optimizer steps: operands, sizes and the workspace of a row-sparse gradient
 static int check_optim_step(const float* param, const float* state0, const float* state1, int64_t rows, int64_t dim,

@@ -527,6 +527,25 @@ int launch_row_set(int64_t V, const IdList* lists, int nlists, void* workspace, 
 // map[id] = id for id < V at the start of the workspace: a dense table through the row-mapped kernels
 int launch_identity_map(int64_t V, void* workspace, cudaStream_t st);
 
+// Negative-sampling P slot (ns_p.cu), operands as b200kge_ns_p_backward; arguments already checked.
+// C [n, ldc] with C[i, r] = the sum of G[i, c] over the columns c of row i whose id (p_i, then neg[i, :]) is r
+int launch_ns_p_collapse(const int64_t* triples, const int64_t* neg, int64_t n, int64_t K, const float* G, int64_t ldg,
+                         int64_t R, float* C, int64_t ldc, cudaStream_t st);
+// s_idx, o_idx = the triples' s and o; s_dst, o_dst = pe[s], pe[o] (pe NULL: s, o)
+int launch_ns_p_unpack(const int64_t* triples, int64_t n, const int32_t* pe, int64_t* s_idx, int64_t* o_idx,
+                       int64_t* s_dst, int64_t* o_dst, cudaStream_t st);
+// chunks of rows of the distance family's relation pass: its partials take ns_p_parts(n, R) * R * rel.dim floats
+int ns_p_parts(int64_t n, int64_t R);
+// TransE (l_norm 1, 2), RotatE (l_norm 1) with weights C (scaled in place for L2): d s_i, d o_i ADDED into rows
+// s_dst[i], o_dst[i] of d_ent; the relation gradient as ns_p_parts(n, R) partials [R, rel.dim] STORED into parts
+int launch_ns_p_distance(int model, float l_norm, const Rows& E, const Rows& Rl, const int64_t* s_idx,
+                         const int64_t* o_idx, int64_t n, float* C, int64_t ldc, float* d_ent, int64_t lde,
+                         const int64_t* s_dst, const int64_t* o_dst, float* parts, cudaStream_t st);
+// out[j] += sum over the nparts partials (rows ldp apart, partials part_stride apart) of relation row rows[j], for
+// j < *count; rows / count NULL: out[r] += ... for every r < R
+int launch_ns_p_rel_add(const float* parts, int64_t ldp, int64_t part_stride, int nparts, int64_t R, int Dr,
+                        const int64_t* rows, const int64_t* count, float* out, int64_t ldo, cudaStream_t st);
+
 // Optimizer steps (optim.cu), operands as b200kge_adagrad_step / b200kge_sparse_adam_step; arguments already checked.
 size_t optim_step_workspace_bytes(int64_t rows, int64_t dim, int64_t nnz, int coalesced);
 int launch_adagrad_step(float* param, float* state_sum, int64_t rows, int64_t dim, const float* grad,

@@ -942,6 +942,56 @@ def ns_backward_sparse(model: str, ent, rel, triples, slot: int, negatives, offs
     return (layout(flags[0], er, ev, E, ent_rows_all, u[0]), layout(flags[1], rr_, rv, R, False, u[1]))
 
 
+def ns_p_backward(model: str, ent, rel, triples, negatives, grad_scores, l_norm: float = 1.0,
+                  implementation: str = "batch", sparse=(False, False)):
+    """(d_ent, d_rel) of the P slot of a negative-sampling batch (b200kge_ns_p_backward): triples [n, 3], negatives
+    [n, K] relation ids, grad_scores = dL/dscores of the [n, 1+K] block (positive first), e.g. the G of
+    ns_loss(..., want_grad=True).  sparse = (entities, relations) as in ns_backward_sparse: a dense [V, D] tensor where
+    False; where True a coalesced torch.sparse_coo_tensor over the rows the reference looks up for the slot (the
+    positives' s and o; the positives' p and every sampled id, or every relation row for implementation "all", whose
+    score_so goes through embed_all()).  Raises NotImplementedError for an unserved model or norm and for more than
+    NS_P_MAX_RELATIONS relations."""
+    _require_cuda(ent, rel, triples, negatives, grad_scores)
+    lib, k = _lib.load(), _Keep()
+    re_, rr = k.rows(ent), k.rows(rel)
+    tri, ng = _i64_block(triples), _i64_block(negatives)
+    n, K = tri.shape[0], ng.shape[1]
+    E, R, D = ent.shape[0], rel.shape[0], ent.shape[1]
+    dev = ent.device
+    if grad_scores.shape != (n, K + 1):
+        raise ValueError(f"grad_scores has shape {tuple(grad_scores.shape)}, expected {(n, K + 1)}")
+    g = _f32_rows(grad_scores)
+    rel_rows_all = sparse[1] and implementation == "all"
+    flags = (int(sparse[0]), int(sparse[1] and not rel_rows_all))
+    caps = (min(E, 2 * n), min(R, n * (K + 1)))
+    counts = torch.zeros(2, dtype=torch.int64, device=dev)
+    outs = []
+    for f, tab, cap in ((flags[0], ent, caps[0]), (flags[1], rel, caps[1])):
+        if f:
+            outs.append((torch.empty(cap, dtype=torch.int64, device=dev),
+                         torch.empty((cap, tab.shape[1]), dtype=torch.float32, device=dev)))
+        else:
+            outs.append((None, torch.zeros_like(_f32(tab))))
+    (er, ev), (rr_, rv) = outs
+    nbytes = lib.b200kge_ns_p_backward_workspace_bytes(MODELS[model], n, K, D, E, R)
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    _lib.check(lib.b200kge_ns_p_backward(
+        MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), ng.data_ptr(), n, K, g.data_ptr(),
+        g.stride(0), flags[0], er.data_ptr() if flags[0] else None, counts.data_ptr() if flags[0] else None,
+        ev.data_ptr(), ev.stride(0), flags[1], rr_.data_ptr() if flags[1] else None,
+        counts[1:].data_ptr() if flags[1] else None, rv.data_ptr(), rv.stride(0), ws.data_ptr(), ws.numel(),
+        _stream(dev)))
+    u = counts.tolist() if (flags[0] or flags[1]) else (0, 0)
+
+    def layout(flag, rows, vals, V, want_sparse, u_):
+        if flag:
+            return torch.sparse_coo_tensor(rows[None, :u_], vals[:u_], (V, vals.shape[1]), is_coalesced=True)
+        if want_sparse:       # "all": every relation row
+            return torch.sparse_coo_tensor(torch.arange(V, device=dev)[None, :], vals, vals.shape, is_coalesced=True)
+        return vals
+    return (layout(flags[0], er, ev, E, False, u[0]), layout(flags[1], rr_, rv, R, rel_rows_all, u[1]))
+
+
 def ns_loss(scores, loss: str, arg: float = 0.0, temperature: float = 1.0, label_idx=None,
             batch_size: Optional[int] = None, want_grad: bool = False, return_rows: bool = False):
     """KgeLoss of a negative-sampling block (train_negative_sampling.py:126-156): scores [n, m] with one positive per

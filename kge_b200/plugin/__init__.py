@@ -45,6 +45,7 @@ from kge.model.simple import SimplEScorer
 from kge.model.transe import TransEScorer
 
 from .. import engine
+from .._lib import NS_P_MAX_RELATIONS
 
 
 class _ScoreEmbFn(torch.autograd.Function):
@@ -335,6 +336,31 @@ class _NsSlotLossFn(torch.autograd.Function):
         d_ent, d_rel = engine.ns_backward(model._b200_name, ent_w.detach(), rel_w.detach(), triples, {slot: negatives},
                                           offset, model._b200_args()[0], batch_size, **kw)
         return (d_ent * g, d_rel * g) + (None,) * 10
+
+
+class _NsPSlotLossFn(torch.autograd.Function):
+    """The P slot of a negative-sampling batch (relation negatives): forward = the fused gather+score [n, 1+K]
+    (b200kge_ns_score, slot 1) and the row-loss kernel, which writes G = dL/dscores for every loss, BCE included;
+    backward = b200kge_ns_p_backward, which sums G into one coefficient per (row, relation) before any table gradient is
+    formed.  A `sparse: True` embedder gets its gradient row-sparse over the rows score_so looks up (every relation row
+    for `implementation` "all")."""
+
+    @staticmethod
+    def forward(ctx, ent_w, rel_w, model, triples, negatives, offset, batch_size, loss, temperature, implementation):
+        ctx.args = (model, implementation)
+        scores = engine.ns_score(model._b200_name, ent_w.detach(), rel_w.detach(), triples, negatives, 1, True,
+                                 model._b200_args()[0])
+        value, G = engine.ns_loss(scores, loss, offset, temperature, batch_size=batch_size, want_grad=True)
+        ctx.save_for_backward(ent_w, rel_w, triples, negatives, G)
+        return value
+
+    @staticmethod
+    def backward(ctx, g):
+        model, implementation = ctx.args
+        ent_w, rel_w, triples, negatives, G = ctx.saved_tensors
+        d_ent, d_rel = engine.ns_p_backward(model._b200_name, ent_w.detach(), rel_w.detach(), triples, negatives, G,
+                                            model._b200_args()[0], implementation, sparse=model.b200_sparse_grads())
+        return (_sparse_scaled(d_ent, g), _sparse_scaled(d_rel, g)) + (None,) * 8
 
 
 class _B200ModelMixin:
@@ -640,6 +666,21 @@ class _B200ModelMixin:
         return _NsSlotLossFn.apply(ent_w, rel_w, self, triples.long().contiguous(), negatives.long().contiguous(),
                                    int(slot), float(offset), int(batch_size), loss, float(temperature), dropout,
                                    implementation)
+
+    def b200_ns_p_slot_ok(self):
+        """The P-slot backward (b200kge_ns_p_backward) covers the dot family, TransE (L1, L2) and RotatE (L1) with at most
+        NS_P_MAX_RELATIONS relations, and needs b200_backward = "native"."""
+        return (self.b200_backward == "native" and self._b200_native_family()
+                and self._b200_weights()[1].shape[0] <= NS_P_MAX_RELATIONS)
+
+    def loss_negatives_p(self, triples, negatives, offset, batch_size, loss="bce", temperature=1.0,
+                         implementation="batch"):
+        """loss_negatives of the P slot: `negatives` [n, K] are relation ids, and the gradient comes from
+        b200kge_ns_p_backward (see _NsPSlotLossFn; `implementation` only picks the row set of a sparse relation
+        gradient).  No embedding dropout."""
+        ent_w, rel_w = self._b200_weights()
+        return _NsPSlotLossFn.apply(ent_w, rel_w, self, triples.long().contiguous(), negatives.long().contiguous(),
+                                    float(offset), int(batch_size), loss, float(temperature), implementation)
 
     def loss_negatives_forward(self, scores, loss, arg=0.0, temperature=1.0):
         """Sum over rows of the KgeLoss of a scored [n, 1+K] block (positive first); forward only."""

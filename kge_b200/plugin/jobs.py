@@ -399,7 +399,11 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _NativeOptimizer, _BatchSpli
 
     `negative_sampling.sampling_type: frequency` (not shared) is served on this route only: the job builds
     B200FrequencySampler instead of the reference's KgeFrequencySampler, uploads one weight table per sampled slot and
-    draws with engine.sample_frequency, or engine.sample_frequency_filtered for a filtered slot."""
+    draws with engine.sample_frequency, or engine.sample_frequency_filtered for a filtered slot.
+
+    With `user.b200_ns_p_slot: true` a sampled P slot (relation negatives) trains natively too, through
+    model.loss_negatives_p (b200kge_ns_p_backward), when the model passes b200_ns_p_slot_ok(); without the option a P slot
+    sends the whole sub-batch to the reference step, as before."""
 
     def __init__(self, config, dataset, parent_job=None, model=None, forward_only=False):
         want = bool(_user_option(config, "b200_device_sampling", False))
@@ -520,8 +524,12 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _NativeOptimizer, _BatchSpli
                        "embedding dropout is not served" if base.b200_dropout_rates() is not None else
                        "the base model's tables cannot be read in place")
                 raise NotImplementedError(f"user.b200_device_sampling with reciprocal_relations_model: {why}")
+        # user.b200_ns_p_slot: the P slot trains through b200kge_ns_p_backward where the model serves it
+        p_native = (model is not None and P in slots and _user_option(self.config, "b200_ns_p_slot", False)
+                    and model.b200_ns_p_slot_ok())
         trainable = (model is not None and kind is not None
-                     and all(model.b200_ns_native_backward_ok(O if recip is not None else sl) for sl in slots))
+                     and all((p_native if sl == P else model.b200_ns_native_backward_ok(O if recip is not None else sl))
+                             for sl in slots))
         drop = None
         if model is None and base is None:
             model, rates = self._b200_ns_dropout_route(kind, slots)
@@ -538,7 +546,7 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _NativeOptimizer, _BatchSpli
         if model is None or (not self.is_forward_only and not trainable):
             if self._device_sampling:
                 raise NotImplementedError("user.b200_device_sampling needs a b200_* model whose slots the fused "
-                                          "gradient kernel covers (S / O slots)")
+                                          "gradient kernel covers (S / O slots; the P slot with user.b200_ns_p_slot)")
             return super()._process_subbatch(batch_index, batch, subbatch_slice, result)
         batch_size = result.size
         result.prepare_time -= time.time()
@@ -575,8 +583,12 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _NativeOptimizer, _BatchSpli
             result.forward_time -= time.time()
             if not self.is_forward_only:
                 # training: forward + the fused NS gradient kernel behind one autograd node
-                loss_value = model.loss_negatives(tri, negatives.to(self.device), kslot, kind[1], batch_size,
-                                                  kind[0], kind[2], **dkw)
+                if slot == P:
+                    loss_value = model.loss_negatives_p(tri, negatives.to(self.device), kind[1], batch_size, kind[0],
+                                                        kind[2], getattr(self, "_implementation", "batch"))
+                else:
+                    loss_value = model.loss_negatives(tri, negatives.to(self.device), kslot, kind[1], batch_size,
+                                                      kind[0], kind[2], **dkw)
                 result.avg_loss += loss_value.item()
                 result.forward_time += time.time()
                 result.backward_time -= time.time()
