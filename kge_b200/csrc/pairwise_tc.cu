@@ -240,6 +240,13 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           const int s = (int)(cc % NSTAGE);
           ptx::mbar_wait_bounded(&full[s], (cc / NSTAGE) & 1);
           if constexpr (C::SPLIT) ptx::mbar_wait_bounded(&split[s], (cc / NSTAGE) & 1);
+          // Hand the ring to the other warpgroup as soon as this tile's last chunk has landed, before its wgmmas are
+          // issued, so the other warpgroup's first chunk queues behind this one's last.  Safe: this thread has waited
+          // on every chunk of the tile in order, and before the tile (through turn[g]) the other warpgroup's thread 0
+          // had waited on every earlier chunk, so every full[] phase up to this one has completed.  The other
+          // warpgroup's next waits are on phases at most one ring pass ahead; the stages it waits on cannot be
+          // refilled beyond that before every warp of this warpgroup releases them through empty[].
+          if (C::PP && kk == nkc - 1 && tg == 0) ptx::mbar_arrive(&turn[g ^ 1]);
           ptx::wg_fence();
 #pragma unroll
           for (int h = 0; h < C::MH; ++h) mma_chunk<MODE>(d[h], ptx::smem_u32(smem + s * STAGE_BYTES), C::PP ? h : g);
@@ -250,30 +257,40 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
             if (lane == 0) ptx::mbar_arrive(&empty[(cc - 1) % NSTAGE]);
           }
         }
-        if (C::PP && tg == 0) ptx::mbar_arrive(&turn[g ^ 1]);   // this tile's chunks all landed: the other may go
+        // The epilogue's operands do not depend on the accumulators: load them before the wait, so their latency runs
+        // under this tile's last wgmmas instead of after them.
+        const int64_t e0 = (int64_t)it.et * TN;
+        float qs[2 * C::MH];      // F16X3 row factors
+        float2 ts[16];            // F16X3 column factors of columns e0 + 2q + 8j (+1)
+        int64_t lab[2 * C::MH];   // BCE / KL with label_idx: the row's label
+#pragma unroll
+        for (int rr = 0; rr < 2 * C::MH; ++rr) {
+          const int64_t row = (int64_t)it.qt * TM + row_in_tile + 64 * (rr >> 1) + 8 * (rr & 1);
+          if constexpr (MODE == MODE_F16X3) qs[rr] = row < prm.nq ? __ldg(prm.q_scale + row) : 0.f;
+          lab[rr] = -1;
+          if constexpr (EPI == EPI_BCE || EPI == EPI_KL)
+            if (P.label_idx && row < prm.nq) lab[rr] = P.label_idx[row];
+        }
+        if constexpr (MODE == MODE_F16X3) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const int64_t col = e0 + 2 * q + 8 * j;
+            ts[j] = col < prm.m ? __ldg(reinterpret_cast<const float2*>(prm.t_scale + col)) : make_float2(0.f, 0.f);
+          }
+        }
         ptx::wg_wait<0>();
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(&empty[(c + nkc - 1) % NSTAGE]);
 
-        const int64_t e0 = (int64_t)it.et * TN;
         if constexpr (MODE == MODE_F16X3) {
-          // score = acc * (row factor * column factor), both exact powers of two; one column pair at a time, so the
-          // factors do not hold registers next to the accumulators
-          float qs[2 * C::MH];
-#pragma unroll
-          for (int rr = 0; rr < 2 * C::MH; ++rr) {
-            const int64_t row = (int64_t)it.qt * TM + row_in_tile + 64 * (rr >> 1) + 8 * (rr & 1);
-            qs[rr] = row < prm.nq ? __ldg(prm.q_scale + row) : 0.f;
-          }
+          // score = acc * (row factor * column factor), both exact powers of two
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
-            const int64_t col = e0 + 2 * q + 8 * j;
-            const float2 ts = col < prm.m ? __ldg(reinterpret_cast<const float2*>(prm.t_scale + col)) : make_float2(0.f, 0.f);
 #pragma unroll
             for (int rr = 0; rr < 2 * C::MH; ++rr) {
               float* a = &d[rr >> 1][4 * j + 2 * (rr & 1)];
-              a[0] = a[0] * (qs[rr] * ts.x);
-              a[1] = a[1] * (qs[rr] * ts.y);
+              a[0] = a[0] * (qs[rr] * ts[j].x);
+              a[1] = a[1] * (qs[rr] * ts[j].y);
             }
           }
         }
@@ -288,7 +305,7 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
               v[2 * j + 1] = d[rr >> 1][4 * j + 2 * (rr & 1) + 1];
             }
             RowState<EPI> rs = st[256 * rr];
-            tc::epi_row<EPI>(P, rs, v, row, e0, prm.m, q);
+            tc::epi_row<EPI>(P, rs, v, row, e0, prm.m, q, lab[rr]);
             st[256 * rr] = rs;
           }
         }

@@ -135,22 +135,25 @@ __device__ __forceinline__ float frag_get(const float (&v)[32], int k) {
 // FULL: all 128 columns of the tile are < m (then nvalid is not read)
 template <int EPI, bool FULL>
 __device__ __forceinline__ void epi_row_body(const EpiParams& P, RowState<EPI>& st, const float (&v)[32], int64_t row,
-                                             int64_t e0, int64_t c0, int nvalid, int q) {
+                                             int64_t e0, int64_t c0, int nvalid, int q, int64_t lab) {
   if constexpr (EPI == EPI_BCE) {
     // sum softplus(z) - sum y*z,  softplus(z) = max(z,0) + log(1 + exp(-|z|))   (loss.py:150-157;
     // torch's kernel also evaluates log(1+e) with a plain log, so tiny e drop out identically)
+    // The lane's 32 logarithms are taken as one: log(prod(1 + e)).  Each factor 1 + e lies in [1, 2], so the product
+    // of 32 stays within [1, 2^32] (no overflow, no denormal), a NaN score still propagates and z = +-inf still adds
+    // a factor of exactly 1.
     const float off = P.offset;
-    float amax = 0.f, alg = 0.f;
+    float amax = 0.f, prod = 1.f;
 #pragma unroll
     for (int k = 0; k < 32; ++k) {
       if (FULL || frag_col(k) < nvalid) {
         const float z = v[k] + off;
         const float e = fast_ex2(-fabsf(z) * LOG2E);
-        alg += __log2f(1.0f + e);
+        prod *= 1.0f + e;
         amax += fmaxf(z, 0.f);
       }
     }
-    st.a += fmaf(alg, LN2, amax);
+    st.a += fmaf(__log2f(prod), LN2, amax);
     if (P.label_dense) {
       const float* __restrict__ y = P.label_dense + row * P.ldl + c0;
       float b = 0.f;
@@ -159,7 +162,6 @@ __device__ __forceinline__ void epi_row_body(const EpiParams& P, RowState<EPI>& 
         if (FULL || frag_col(k) < nvalid) b = fmaf(__ldg(y + frag_col(k)), v[k] + off, b);
       st.b += b;
     } else if (P.label_idx) {
-      const int64_t lab = P.label_idx[row];
       const int k = (lab >= e0 && lab < e0 + 128 && (FULL || lab - c0 < nvalid)) ? frag_elem((int)(lab - e0), q) : -1;
       if (k >= 0) st.b += frag_get(v, k) + off;
     }
@@ -191,7 +193,6 @@ __device__ __forceinline__ void epi_row_body(const EpiParams& P, RowState<EPI>& 
         }
       }
     } else if (P.label_idx) {
-      const int64_t lab = P.label_idx[row];
       const int k = (lab >= e0 && lab < e0 + 128 && (FULL || lab - c0 < nvalid)) ? frag_elem((int)(lab - e0), q) : -1;
       if (k >= 0) { st.y_sum += 1.0f; st.yx += frag_get(v, k); }
     }
@@ -273,15 +274,16 @@ __device__ __forceinline__ void rank_eval_row(const EpiParams& P, const float (&
   fix.commit(P, row);
 }
 
-// One row's share of a tile: e0 = first column of the tile, q = lane % 4, c0 = e0 + 2q.  v is clobbered (rank: CSR
-// filtered columns become -inf).
+// One row's share of a tile: e0 = first column of the tile, q = lane % 4, c0 = e0 + 2q.  lab = P.label_idx[row], loaded
+// by the caller ahead of the accumulators (read by BCE / KL with label_idx only).  v is clobbered (rank: CSR filtered
+// columns become -inf).
 template <int EPI>
 __device__ __forceinline__ void epi_row(const EpiParams& P, RowState<EPI>& st, float (&v)[32], int64_t row,
-                                        int64_t e0, int64_t m, int q) {
+                                        int64_t e0, int64_t m, int q, int64_t lab) {
   const int64_t c0 = e0 + 2 * q;
   if constexpr (EPI == EPI_RANK_EVAL) {
-    if (e0 + 128 <= m) epi_row_body<EPI, true>(P, st, v, row, e0, c0, 128, q);
-    else               epi_row_body<EPI, false>(P, st, v, row, e0, c0, (int)(m - c0), q);
+    if (e0 + 128 <= m) epi_row_body<EPI, true>(P, st, v, row, e0, c0, 128, q, lab);
+    else               epi_row_body<EPI, false>(P, st, v, row, e0, c0, (int)(m - c0), q, lab);
     rank_eval_row(P, v, row, e0, m, q);
     return;
   }
@@ -312,8 +314,8 @@ __device__ __forceinline__ void epi_row(const EpiParams& P, RowState<EPI>& st, f
       if (P.csr_extra && e0 == 0 && q == 0) P.csr_out[P.csr_nnz + row] = v[0];
     }
   }
-  if (e0 + 128 <= m) epi_row_body<EPI, true>(P, st, v, row, e0, c0, 128, q);
-  else               epi_row_body<EPI, false>(P, st, v, row, e0, c0, (int)(m - c0), q);
+  if (e0 + 128 <= m) epi_row_body<EPI, true>(P, st, v, row, e0, c0, 128, q, lab);
+  else               epi_row_body<EPI, false>(P, st, v, row, e0, c0, (int)(m - c0), q, lab);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
