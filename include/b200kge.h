@@ -717,6 +717,58 @@ int b200kge_ns_p_backward(int model, float l_norm, const b200kge_rows_t* ent, co
                           int rel_sparse, int64_t* rel_rows, int64_t* rel_count, float* d_rel, int64_t ldr,
                           void* workspace, size_t workspace_bytes, b200kge_stream_t stream);
 
+/* ---- Shared negative sampling (negative_sampling.shared: True) -------------------------------------------------------
+ * Every row of a batch draws its K negatives for slot 0 (S) or 2 (O) from the same num_unique = U' distinct entity ids
+ * unique [U'] (KgeUniformSampler._sample_shared, sampler.py:597-698).  Column 1 + c of row i holds the sample
+ * j = c < U ? c : repeat[c - U] (repeat [K - U], indexes into [0, U)), and the id unique[u(i, c)] with
+ *   drop == NULL ("naive", U = U'):          u = j                                        (sampler.py:412-463)
+ *   drop [n] ("default", U = U' - 1):        u = (j == drop[i]) ? U : j, drop[i] in [0, U] (sampler.py:503-578)
+ * drop is the sub-batch's slice of the batch's drop_index; unique and repeat are the batch's.  Every column's score is
+ * a score against one of the U' shared rows, so the slot is the dense problem Z [n, U'] (row i's fixed pair against
+ * unique[u]) plus a gather of its columns, and its backward is a dense backward with the block's gradient summed per
+ * shared id:  C[i, u] = sum over the columns c with u(i, c) = u of G[i, 1 + c].
+ * impl: B200KGE_NS_TRIPLE or B200KGE_NS_BATCH (the reference's `batch` and `all`).  It matters to TransE, whose `triple`
+ * scores go through F.pairwise_distance and add its eps = 1e-6 to the difference (transe.py:18): folded into the query as
+ * s + p + eps (O slot) or o - p - eps (S slot); `batch` scores are cdist, without eps.  The positive column is
+ * score_spo, with eps, in every case.  Coverage: the dot family, TransE (l_norm 1, 2), RotatE (l_norm 1), a folded
+ * width of at most 1024, tables of fewer than 2^31 rows; anything else returns B200KGE_ERR_UNSUPPORTED before a launch.
+ * Requirements (else B200KGE_ERR_INVALID): U >= 1 when K > U, K >= U, ids inside their tables. */
+
+/* The [n, 1 + K] block of one slot into out (row stride ldo >= 1 + K): column 0 the positive triple (score_spo), columns
+ * 1.. the assembled negatives.  Z is the 1-vs-N scorer against the gathered shared rows (the pre-split tensor-core path
+ * where `precision` and the shape allow it, else the CUDA-core scorer), written to z_out [n, ldz >= U'] when z_out is
+ * not NULL (b200kge_ns_shared_backward needs it for TransE l_norm 2).
+ * workspace: b200kge_ns_shared_score_workspace_bytes(model, n, U', D). */
+size_t b200kge_ns_shared_score_workspace_bytes(int model, int64_t n, int64_t num_unique, int32_t D);
+int b200kge_ns_shared_score(int model, float l_norm, int precision, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                            const int64_t* triples, int slot, const int64_t* unique, int64_t num_unique,
+                            const int64_t* repeat, const int64_t* drop, int64_t n, int64_t K, int impl, float* out,
+                            int64_t ldo, float* z_out, int64_t ldz, void* workspace, size_t workspace_bytes,
+                            b200kge_stream_t stream);
+
+/* Backward of b200kge_ns_shared_score's block: grad_scores [n, 1 + K] (row stride ldg) is dL/dz, e.g. the grad_out of
+ * b200kge_ns_loss with scale = 1 / batch_size.  C is summed from it per row, in column order, without atomics; then
+ *   dot family: the query fold Q, the shared rows T gathered, dT = C^T Q and dQ = C T on the split-K tensor-core GEMMs
+ *     (the backward block with C as its gradient), dT ADDED into the U' distinct rows unique[u], dQ unfolded;
+ *   TransE (l_norm 1, 2), RotatE (l_norm 1): the distance row-gradient passes with weights C (divided by z for
+ *     l_norm 2: z [n, ldz] is the z_out of the forward, required there), the same adds and unfold;
+ * and the positive column's VJP per row.  No per-sample contribution is added atomically into the shared rows.
+ * Per table, `*_sparse` as b200kge_ns_p_backward (0: dense, ADDED into; 1: row-sparse, rows / *count / the first *count
+ * value rows OVERWRITTEN) with the rows the reference looks up for the slot: entities the positives' s and o plus
+ * every shared id (B200KGE_NS_BATCH: score_sp / score_po(..., unique)) or the shared ids the sub-batch's rows use
+ * (B200KGE_NS_TRIPLE), at most min(E, 2n + U'); relations the positives' p, at most min(R, n).  (`implementation: all`
+ * looks up every entity row: pass ent_sparse = 0.)
+ * workspace: b200kge_ns_shared_backward_workspace_bytes(model, n, U', D, E, R). */
+size_t b200kge_ns_shared_backward_workspace_bytes(int model, int64_t n, int64_t num_unique, int32_t D, int64_t E,
+                                                  int64_t R);
+int b200kge_ns_shared_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                               const int64_t* triples, int slot, const int64_t* unique, int64_t num_unique,
+                               const int64_t* repeat, const int64_t* drop, int64_t n, int64_t K, int impl,
+                               const float* z, int64_t ldz, const float* grad_scores, int64_t ldg, int ent_sparse,
+                               int64_t* ent_rows, int64_t* ent_count, float* d_ent, int64_t lde, int rel_sparse,
+                               int64_t* rel_rows, int64_t* rel_count, float* d_rel, int64_t ldr, void* workspace,
+                               size_t workspace_bytes, b200kge_stream_t stream);
+
 /* ---- Optimizer steps: torch.optim.Adagrad and torch.optim.SparseAdam (torch 2.11) on one fp32 parameter ----------------
  * param and its state tensors are [rows, dim], contiguous.  The gradient is
  *   dense      (grad_rows == NULL): grad [rows, dim], contiguous; nnz and coalesced are unused;

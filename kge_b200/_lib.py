@@ -139,6 +139,17 @@ SIGNATURES = {
                                         C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                         C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                         C.c_size_t, C.c_void_p]),
+    "b200kge_ns_shared_score_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32]),
+    "b200kge_ns_shared_score": (C.c_int, [C.c_int, C.c_float, C.c_int, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p,
+                                          C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
+                                          C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200kge_ns_shared_backward_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64, C.c_int32, C.c_int64,
+                                                                 C.c_int64]),
+    "b200kge_ns_shared_backward": (C.c_int, [C.c_int, C.c_float, _RP, _RP, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
+                                             C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
+                                             C.c_int64, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200kge_optim_step_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64, C.c_int]),
     "b200kge_adagrad_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
                                        C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_size_t,

@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200kge.so")
-SOURCES = ["capi.cu", "fold.cu", "pairwise_simt.cu", "pairwise_tc.cu", "presplit.cu", "rowwise.cu", "epilogue_dense.cu", "hostindex.cu", "grad.cu", "grad_distance.cu", "csr_loss.cu", "ns_loss.cu", "dropout.cu", "ns_dropout.cu", "rowset.cu", "optim.cu", "ns_p.cu"]
+SOURCES = ["capi.cu", "fold.cu", "pairwise_simt.cu", "pairwise_tc.cu", "presplit.cu", "rowwise.cu", "epilogue_dense.cu", "hostindex.cu", "grad.cu", "grad_distance.cu", "csr_loss.cu", "ns_loss.cu", "dropout.cu", "ns_dropout.cu", "rowset.cu", "optim.cu", "ns_p.cu", "ns_shared.cu"]
 HEADERS = ["common.cuh", "dropmask.cuh", "fold.cuh", "philox.cuh", "ptx.cuh", "tc_common.cuh", os.path.join("..", "..", "include", "b200kge.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

@@ -2142,6 +2142,204 @@ int b200kge_ns_p_backward(int model, float l_norm, const b200kge_rows_t* ent, co
   return launch_unfold_so(model, S, O, n, dQ, ldq, d_ent, lde, s_dst, d_ent, lde, o_dst, st);
 }
 
+// The checks shared by the two shared-sampling entry points; *U = the shared samples before the repeats
+static int check_ns_shared(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                           const int64_t* triples, int slot, const int64_t* unique, int64_t num_unique,
+                           const int64_t* repeat, const int64_t* drop, int64_t n, int64_t K, int impl, int64_t* U) {
+  if (!triples && n > 0) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (n < 0 || K < 0 || num_unique < 0) { set_error("negative sizes"); return B200KGE_ERR_INVALID; }
+  int rc = check_tables(model, l_norm, ent, rel); if (rc) return rc;
+  if (impl != B200KGE_NS_TRIPLE && impl != B200KGE_NS_BATCH) { set_error("unknown implementation %d", impl); return B200KGE_ERR_INVALID; }
+  *U = drop ? num_unique - 1 : num_unique;
+  if (*U < 0 || *U > K || (*U == 0 && K > 0)) {
+    set_error("%lld unique ids do not fit %lld samples per row (%s)", (long long)num_unique, (long long)K,
+              drop ? "default: U + 1 ids, 1 <= U <= K" : "naive: 1 <= U <= K");
+    return B200KGE_ERR_INVALID;
+  }
+  if ((!unique && num_unique > 0) || (!repeat && K > *U)) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (slot != 0 && slot != 2) { set_error("shared negative sampling covers the S and O slots"); return B200KGE_ERR_UNSUPPORTED; }
+  if ((model == B200KGE_TRANSE && l_norm != 1.0f && l_norm != 2.0f) || (model == B200KGE_ROTATE && l_norm != 1.0f)) {
+    set_error("shared negative sampling covers l_norm 1 and 2 (TransE) / 1 (RotatE)");
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  const int kf = folded_problem(model, B200KGE_SP_, ent->dim, l_norm).K;
+  if (kf > 1024) { set_error("embedding width %d exceeds the backward kernel's limit of 1024", kf); return B200KGE_ERR_UNSUPPORTED; }
+  if (ent->rows > INT32_MAX || rel->rows > INT32_MAX) { set_error("shared negative sampling covers tables of fewer than 2^31 rows"); return B200KGE_ERR_UNSUPPORTED; }
+  return 0;
+}
+
+// The slot's folded queries Q [n, ldq] (O slot: sp_ of (s, p); S slot: _po of (o, p)), with pairwise_distance's eps for
+// TransE's `triple` scores: (s + p) - o' + eps = (s + p + eps) - o',  s' + p - o + eps = s' - (o - p - eps)
+static int ns_shared_queries(int model, int slot, int impl, const Rows& E, const Rows& Rl, const int64_t* triples,
+                             int64_t n, Arena& ws, Rows& S, Rows& P, Rows& O, float** Q, int64_t ldq, cudaStream_t st) {
+  int64_t* sidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* pidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* oidx = (int64_t*)ws.take((size_t)n * 8);
+  int64_t* lab = (int64_t*)ws.take((size_t)n * 16);
+  *Q = (float*)ws.take((size_t)n * ldq * 4);
+  if (!sidx || !pidx || !oidx || !lab || !*Q) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
+  int rc = unpack_triples(triples, n, sidx, pidx, oidx, lab, E, Rl, S, O, P, st); if (rc) return rc;
+  const bool sp = slot == 2;
+  if ((rc = launch_fold_queries(model, sp ? B200KGE_SP_ : B200KGE__PO, sp ? S : O, P, n, 0, *Q, ldq, st))) return rc;
+  if (model == B200KGE_TRANSE && impl == B200KGE_NS_TRIPLE)
+    return launch_ns_shared_eps(*Q, ldq, n, E.dim, sp ? 1e-6f : -1e-6f, st);
+  return 0;
+}
+
+size_t b200kge_ns_shared_score_workspace_bytes(int model, int64_t n, int64_t num_unique, int32_t D) {
+  if (n < 0 || num_unique < 0 || D <= 0) return 0;
+  const int64_t ldq = round_up(D, 32), ldz = round_up(num_unique > 0 ? num_unique : 1, 4);
+  // s, p, o, labels, Q, Z, the scorer's workspace
+  return 5 * ((size_t)n * 8 + 256) + (size_t)n * ldq * 4 + 256 + (size_t)n * ldz * 4 + 256 +
+         b200kge_workspace_bytes(model, n, num_unique, D, 1);
+}
+
+int b200kge_ns_shared_score(int model, float l_norm, int precision, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                            const int64_t* triples, int slot, const int64_t* unique, int64_t num_unique,
+                            const int64_t* repeat, const int64_t* drop, int64_t n, int64_t K, int impl, float* out,
+                            int64_t ldo, float* z_out, int64_t ldz, void* workspace, size_t workspace_bytes,
+                            b200kge_stream_t stream) {
+  int64_t U = 0;
+  int rc = check_ns_shared(model, l_norm, ent, rel, triples, slot, unique, num_unique, repeat, drop, n, K, impl, &U);
+  if (rc) return rc;
+  if (!out && n > 0) { set_error("null operand"); return B200KGE_ERR_INVALID; }
+  if (ldo < K + 1) { set_error("out is narrower than the 1 + K columns of the block"); return B200KGE_ERR_INVALID; }
+  if (z_out && ldz < num_unique) { set_error("z_out is narrower than the %lld unique ids", (long long)num_unique); return B200KGE_ERR_INVALID; }
+  const Folded f = folded_problem(model, slot == 2 ? B200KGE_SP_ : B200KGE__PO, ent->dim, l_norm);
+  if (precision != B200KGE_PREC_AUTO && precision != B200KGE_PREC_FP32 &&
+      (precision != B200KGE_PREC_F16X3 || f.pair_op != PAIR_DOT || f.K < 16)) {
+    set_error("shared negative sampling scores at precision auto, fp32 or (dot family, K >= 16) f16x3");
+    return B200KGE_ERR_UNSUPPORTED;
+  }
+  if (!workspace || workspace_bytes < b200kge_ns_shared_score_workspace_bytes(model, n, num_unique, ent->dim)) {
+    set_error("workspace too small (see b200kge_ns_shared_score_workspace_bytes)");
+    return B200KGE_ERR_WORKSPACE;
+  }
+  if (n == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const Rows E = to_rows(ent), Rl = to_rows(rel);
+  Arena ws{(uint8_t*)workspace, workspace_bytes, 0};
+  Rows S, P, O;
+  float* Q = nullptr;
+  const int64_t ldq = round_up(f.K, 32);
+  if ((rc = ns_shared_queries(model, slot, impl, E, Rl, triples, n, ws, S, P, O, &Q, ldq, st))) return rc;
+  // column 0: score_spo of the positive (train_negative_sampling.py:141-143)
+  if ((rc = launch_spo(model, l_norm, S, P, O, n, out, ldo, st))) return rc;
+  if (K == 0) return 0;
+  float* Z = z_out;
+  if (!Z) {
+    ldz = round_up(num_unique, 4);
+    if (!(Z = (float*)ws.take((size_t)n * ldz * 4))) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
+  }
+  // Z = score_sp(s, p, unique) / score_po(p, o, unique) (sampler.py:347-356)
+  Rows cand = E; cand.idx = unique; cand.rows = num_unique;
+  EpiParams Pz = empty_epi();
+  Pz.out = Z; Pz.ldo = ldz;
+  Block B{model, slot == 2 ? B200KGE_SP_ : B200KGE__PO, slot == 2 ? &S : &O, nullptr, &P, &cand, n};
+  B.Qpre = Q;
+  if ((rc = run_block(B, l_norm, precision, EPI_STORE, Pz, ws, st, nullptr))) return rc;
+  return launch_ns_shared_assemble(Z, ldz, n, K, U, repeat, drop, out, ldo, st);
+}
+
+size_t b200kge_ns_shared_backward_workspace_bytes(int model, int64_t n, int64_t num_unique, int32_t D, int64_t E,
+                                                  int64_t R) {
+  if (n < 0 || num_unique < 0 || D <= 0 || E < 0 || R < 0) return 0;
+  const int64_t nu = num_unique > 0 ? num_unique : 1, ldq = round_up(D, 32), ldc = round_up(nu, 4);
+  // row-set maps; s, p, o, labels, Q; used ids and drop counts; C; dQ of the shared columns and of the positive;
+  // T and dT of the shared rows
+  size_t b = row_set_workspace_bytes(E) + row_set_workspace_bytes(R) + 5 * ((size_t)n * 8 + 256) +
+             (size_t)n * ldq * 4 + 256 + (size_t)nu * 12 + 512 + (size_t)n * ldc * 4 + 256 +
+             2 * ((size_t)n * ldq * 4 + 256) + 2 * ((size_t)nu * ldq * 4 + 256);
+  if (model == B200KGE_TRANSE || model == B200KGE_ROTATE) return b + (size_t)nu * round_up(n, 4) * 4 + 256;   // C^T
+  return b + backward_block_bytes(n, nu, D, ldq);
+}
+
+int b200kge_ns_shared_backward(int model, float l_norm, const b200kge_rows_t* ent, const b200kge_rows_t* rel,
+                               const int64_t* triples, int slot, const int64_t* unique, int64_t num_unique,
+                               const int64_t* repeat, const int64_t* drop, int64_t n, int64_t K, int impl,
+                               const float* z, int64_t ldz, const float* grad_scores, int64_t ldg, int ent_sparse,
+                               int64_t* ent_rows, int64_t* ent_count, float* d_ent, int64_t lde, int rel_sparse,
+                               int64_t* rel_rows, int64_t* rel_count, float* d_rel, int64_t ldr, void* workspace,
+                               size_t workspace_bytes, b200kge_stream_t stream) {
+  int64_t U = 0;
+  int rc = check_ns_shared(model, l_norm, ent, rel, triples, slot, unique, num_unique, repeat, drop, n, K, impl, &U);
+  if (rc) return rc;
+  if ((!grad_scores && n > 0) || !d_ent || !d_rel || (ent_sparse && (!ent_rows || !ent_count)) ||
+      (rel_sparse && (!rel_rows || !rel_count))) {
+    set_error("null operand");
+    return B200KGE_ERR_INVALID;
+  }
+  if (ldg < K + 1) { set_error("grad_scores is narrower than the 1 + K columns of the block"); return B200KGE_ERR_INVALID; }
+  if ((rc = check_grad_ld(ent, lde, rel, ldr))) return rc;
+  const Folded f = folded_problem(model, slot == 2 ? B200KGE_SP_ : B200KGE__PO, ent->dim, l_norm);
+  if (f.pair_op == PAIR_L2 && K > 0 && (!z || ldz < num_unique)) {
+    set_error("TransE l_norm 2 needs the forward's scores z [n, >= %lld]", (long long)num_unique);
+    return B200KGE_ERR_INVALID;
+  }
+  const size_t need = b200kge_ns_shared_backward_workspace_bytes(model, n, num_unique, ent->dim, ent->rows, rel->rows);
+  if (!workspace || workspace_bytes < need) { set_error("workspace too small (see b200kge_ns_shared_backward_workspace_bytes)"); return B200KGE_ERR_WORKSPACE; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const Rows E = to_rows(ent), Rl = to_rows(rel);
+  uint8_t* ws_e = (uint8_t*)workspace;
+  uint8_t* ws_r = ws_e + row_set_workspace_bytes(E.rows);
+  uint8_t* ws_rest = ws_r + row_set_workspace_bytes(Rl.rows);
+  Arena ws{ws_rest, workspace_bytes - (size_t)(ws_rest - ws_e), 0};
+  const int64_t nu = num_unique;
+  int64_t* used = (int64_t*)ws.take((size_t)(nu > 0 ? nu : 1) * 8);
+  int* cnt = (int*)ws.take((size_t)(nu > 0 ? nu : 1) * 4);
+  if (!used || !cnt) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
+  // the rows the reference looks up for the slot: the positives' s, o and the shared ids (`batch`: all of them, as
+  // score_sp / score_po(..., unique) embeds them; `triple`: those the sub-batch's rows use); the positives' p
+  const int64_t* ids = unique;
+  if (ent_sparse && impl == B200KGE_NS_TRIPLE && drop && n > 0) {     // naive: every row uses every shared id
+    if ((rc = launch_ns_shared_used(unique, nu, drop, n, triples, cnt, used, st))) return rc;
+    ids = used;
+  }
+  const IdList le[3] = {{triples, n, 3}, {triples + 2, n, 3}, {ids, n > 0 ? nu : 0, 1}};
+  const IdList lr[1] = {{triples + 1, n, 3}};
+  const bool mapped = ent_sparse || rel_sparse;
+  if (mapped && (rc = ent_sparse ? launch_row_set(E.rows, le, 3, ws_e, ent_rows, ent_count, d_ent, lde, st)
+                                 : launch_identity_map(E.rows, ws_e, st))) return rc;
+  if (mapped && (rc = rel_sparse ? launch_row_set(Rl.rows, lr, 1, ws_r, rel_rows, rel_count, d_rel, ldr, st)
+                                 : launch_identity_map(Rl.rows, ws_r, st))) return rc;
+  if (n == 0) return 0;
+  const int32_t* pe = mapped ? (const int32_t*)ws_e : nullptr;
+  const int32_t* pr = mapped ? (const int32_t*)ws_r : nullptr;
+  Rows S, P, O;
+  float* Q = nullptr;
+  const int64_t ldq = round_up(f.K, 32), ldc = round_up(nu > 0 ? nu : 1, 4);
+  if ((rc = ns_shared_queries(model, slot, impl, E, Rl, triples, n, ws, S, P, O, &Q, ldq, st))) return rc;
+  float* dQp = (float*)ws.take((size_t)n * ldq * 4);
+  if (!dQp) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
+  // the positive column (G[:, 0]) through the row-wise kernel, unfolded into its rows
+  if ((rc = launch_ns_backward(model, l_norm, E, Rl, triples, slot, nullptr, n, 0, 0.f, 1.f, grad_scores, ldg, d_ent, lde,
+                               d_rel, ldr, dQp, ldq, st, pe, pr))) return rc;
+  if (K == 0) return 0;
+  float* C = (float*)ws.take((size_t)n * ldc * 4);
+  float* dQ = (float*)ws.take((size_t)n * ldq * 4);
+  float* T = (float*)ws.take((size_t)nu * ldq * 4);
+  float* dT = (float*)ws.take((size_t)nu * ldq * 4);
+  if (!C || !dQ || !T || !dT) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
+  if ((rc = launch_ns_shared_collapse(grad_scores, ldg, n, K, U, nu, repeat, drop, C, ldc, st))) return rc;
+  Rows cand = E; cand.idx = unique; cand.rows = nu;
+  if ((rc = launch_gather_rows(cand, f.col_off, f.K, T, ldq, st))) return rc;
+  const Rows Tr{T, nullptr, nu, ldq, f.K};
+  const int dir = slot == 2 ? 0 : 1;
+  if (model == B200KGE_TRANSE || model == B200KGE_ROTATE) {
+    float* Ct = (float*)ws.take((size_t)nu * round_up(n, 4) * 4);
+    if (!Ct) { set_error("workspace too small"); return B200KGE_ERR_WORKSPACE; }
+    if (f.pair_op == PAIR_L2 && (rc = launch_div_scores(C, ldc, z, ldz, n, nu, C, ldc, st))) return rc;
+    if ((rc = distance_rowgrads(f.pair_op, Q, ldq, n, Tr, f.K, C, ldc, Ct, dQ, dT, ldq, st))) return rc;
+    if ((rc = launch_ns_shared_row_add(dT, ldq, nu, f.K, unique, pe, d_ent, lde, f.col_off, st))) return rc;
+    return launch_unfold_distance(model, E, Rl, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, st, 0, pe, pr);
+  }
+  GradSpec g;
+  g.G = C; g.ldg = ldc;
+  if ((rc = backward_block(B200KGE_DISTMULT, Tr, Rl, n, B200KGE_SP_, false, Q, ldq, 0, f.K, g, dT, ldq, dQ, ws, st))) return rc;
+  if ((rc = launch_ns_shared_row_add(dT, ldq, nu, f.K, unique, pe, d_ent, lde, f.col_off, st))) return rc;
+  return launch_unfold(model, E, Rl, triples, n, dir, dQ, ldq, d_ent, lde, d_rel, ldr, st, 0, pe, pr);
+}
+
 
 // The checks shared by the two optimizer steps: operands, sizes and the workspace of a row-sparse gradient
 static int check_optim_step(const float* param, const float* state0, const float* state1, int64_t rows, int64_t dim,

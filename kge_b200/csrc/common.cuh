@@ -546,6 +546,24 @@ int launch_ns_p_distance(int model, float l_norm, const Rows& E, const Rows& Rl,
 int launch_ns_p_rel_add(const float* parts, int64_t ldp, int64_t part_stride, int nparts, int64_t R, int Dr,
                         const int64_t* rows, const int64_t* count, float* out, int64_t ldo, cudaStream_t st);
 
+// Shared negative sampling (ns_shared.cu), operands as b200kge_ns_shared_score / _backward; arguments already checked.
+// U = the shared samples before the repeats, nu = U' = the unique ids (U + 1 with drop, else U).
+// out[i, 1 + c] = Z[i, u(i, c)] for c < K
+int launch_ns_shared_assemble(const float* Z, int64_t ldz, int64_t n, int64_t K, int64_t U, const int64_t* repeat,
+                              const int64_t* drop, float* out, int64_t ldo, cudaStream_t st);
+// C [n, ldc] with C[i, u] = the sum of G[i, 1 + c] over the columns c with u(i, c) = u, in column order
+int launch_ns_shared_collapse(const float* G, int64_t ldg, int64_t n, int64_t K, int64_t U, int64_t nu,
+                              const int64_t* repeat, const int64_t* drop, float* C, int64_t ldc, cudaStream_t st);
+// used[u] = unique[u] where some row of the sub-batch uses it (default type: drop [n]), else *fill; cnt: [nu] ints of
+// scratch
+int launch_ns_shared_used(const int64_t* unique, int64_t nu, const int64_t* drop, int64_t n, const int64_t* fill,
+                          int* cnt, int64_t* used, cudaStream_t st);
+// Q[i, k] += eps for k < D
+int launch_ns_shared_eps(float* Q, int64_t ldq, int64_t n, int D, float eps, cudaStream_t st);
+// d_ent[pe ? pe[unique[u]] : unique[u], col_off + k] += dT[u, k] for u < nu, k < K
+int launch_ns_shared_row_add(const float* dT, int64_t ldt, int64_t nu, int K, const int64_t* unique, const int32_t* pe,
+                             float* d_ent, int64_t lde, int col_off, cudaStream_t st);
+
 // Optimizer steps (optim.cu), operands as b200kge_adagrad_step / b200kge_sparse_adam_step; arguments already checked.
 size_t optim_step_workspace_bytes(int64_t rows, int64_t dim, int64_t nnz, int coalesced);
 int launch_adagrad_step(float* param, float* state_sum, int64_t rows, int64_t dim, const float* grad,

@@ -992,6 +992,98 @@ def ns_p_backward(model: str, ent, rel, triples, negatives, grad_scores, l_norm:
     return (layout(flags[0], er, ev, E, False, u[0]), layout(flags[1], rr_, rv, R, rel_rows_all, u[1]))
 
 
+def _shared_operands(unique, repeat, drop, n: int, K: int):
+    """unique [U'], repeat [K - U] and drop [n] (None: "naive") of a shared sample as contiguous int64 device blocks."""
+    un = _i64(unique)
+    rp = _i64(repeat) if repeat is not None and repeat.numel() else None
+    dr = _i64(drop) if drop is not None else None
+    if dr is not None and dr.numel() != n:
+        raise ValueError(f"drop has {dr.numel()} entries, expected one per row ({n})")
+    U = un.numel() - (1 if dr is not None else 0)
+    if K - U != (rp.numel() if rp is not None else 0):
+        raise ValueError(f"repeat has {0 if rp is None else rp.numel()} entries, expected K - U = {K - U}")
+    return un, rp, dr
+
+
+def ns_shared_score(model: str, ent, rel, triples, slot: int, unique, repeat, drop, K: int, l_norm: float = 1.0,
+                    precision: str = "auto", implementation: str = "batch", want_z: bool = False):
+    """The [n, 1+K] block of one slot (0 = S, 2 = O) under shared negative sampling (b200kge_ns_shared_score): column 0
+    the positive triple, column 1 + c the score of the shared id unique[u(i, c)] with j = c < U ? c : repeat[c - U] and
+    u = j, or U where j == drop[i] ("default"; drop None: "naive").  unique, repeat and drop are the shared sample's
+    _unique_samples, _repeat_indexes and the sub-batch's rows of _drop_index (sampler.py:383-585).  `implementation`
+    "triple" adds F.pairwise_distance's eps to TransE's negatives.  want_z: also return Z [n, U'], the scores against
+    the shared rows (the backward of TransE l_norm 2 needs them)."""
+    _require_cuda(ent, rel, triples, unique)
+    lib, k = _lib.load(), _Keep()
+    re_, rr = k.rows(ent), k.rows(rel)
+    tri = _i64_block(triples)
+    n = tri.shape[0]
+    un, rp, dr = _shared_operands(unique, repeat, drop, n, K)
+    dev = ent.device
+    out = torch.empty((n, K + 1), dtype=torch.float32, device=dev)
+    z = torch.empty((n, max(un.numel(), 1)), dtype=torch.float32, device=dev) if want_z else None
+    nbytes = lib.b200kge_ns_shared_score_workspace_bytes(MODELS[model], n, un.numel(), ent.shape[1])
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    _lib.check(lib.b200kge_ns_shared_score(
+        MODELS[model], l_norm, PREC[precision], C.byref(re_), C.byref(rr), tri.data_ptr(), int(slot), un.data_ptr(),
+        un.numel(), rp.data_ptr() if rp is not None else None, dr.data_ptr() if dr is not None else None, n, K,
+        NS_IMPL[implementation], out.data_ptr(), out.stride(0), z.data_ptr() if want_z else None,
+        z.stride(0) if want_z else 0, ws.data_ptr(), ws.numel(), _stream(dev)))
+    return (out, z[:, :un.numel()]) if want_z else out
+
+
+def ns_shared_backward(model: str, ent, rel, triples, slot: int, unique, repeat, drop, K: int, grad_scores, z=None,
+                       l_norm: float = 1.0, implementation: str = "batch", sparse=(False, False)):
+    """(d_ent, d_rel) of ns_shared_score's block (b200kge_ns_shared_backward) for grad_scores = dL/dscores [n, 1+K],
+    e.g. the G of ns_loss(..., want_grad=True); z is ns_shared_score's Z (required for TransE l_norm 2).  sparse =
+    (entities, relations) as in ns_backward_sparse: where True a coalesced torch.sparse_coo_tensor over the rows the
+    reference looks up for the slot (the positives' s and o with every shared id for "batch", the shared ids the rows
+    use for "triple", every entity row for "all"; the positives' p)."""
+    _require_cuda(ent, rel, triples, unique, grad_scores)
+    lib, k = _lib.load(), _Keep()
+    re_, rr = k.rows(ent), k.rows(rel)
+    tri = _i64_block(triples)
+    n = tri.shape[0]
+    un, rp, dr = _shared_operands(unique, repeat, drop, n, K)
+    E, R, D = ent.shape[0], rel.shape[0], ent.shape[1]
+    dev = ent.device
+    if grad_scores.shape != (n, K + 1):
+        raise ValueError(f"grad_scores has shape {tuple(grad_scores.shape)}, expected {(n, K + 1)}")
+    g = _f32_rows(grad_scores)
+    zz = _f32_rows(z) if z is not None else None
+    ent_rows_all = sparse[0] and implementation == "all"
+    flags = (int(sparse[0] and not ent_rows_all), int(sparse[1]))
+    caps = (min(E, 2 * n + un.numel()), min(R, n))
+    counts = torch.zeros(2, dtype=torch.int64, device=dev)
+    outs = []
+    for f, tab, cap in ((flags[0], ent, caps[0]), (flags[1], rel, caps[1])):
+        if f:
+            outs.append((torch.empty(cap, dtype=torch.int64, device=dev),
+                         torch.empty((cap, tab.shape[1]), dtype=torch.float32, device=dev)))
+        else:
+            outs.append((None, torch.zeros_like(_f32(tab))))
+    (er, ev), (rr_, rv) = outs
+    nbytes = lib.b200kge_ns_shared_backward_workspace_bytes(MODELS[model], n, un.numel(), D, E, R)
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    _lib.check(lib.b200kge_ns_shared_backward(
+        MODELS[model], l_norm, C.byref(re_), C.byref(rr), tri.data_ptr(), int(slot), un.data_ptr(), un.numel(),
+        rp.data_ptr() if rp is not None else None, dr.data_ptr() if dr is not None else None, n, K,
+        NS_IMPL[implementation], zz.data_ptr() if zz is not None else None, zz.stride(0) if zz is not None else 0,
+        g.data_ptr(), g.stride(0), flags[0], er.data_ptr() if flags[0] else None,
+        counts.data_ptr() if flags[0] else None, ev.data_ptr(), ev.stride(0), flags[1],
+        rr_.data_ptr() if flags[1] else None, counts[1:].data_ptr() if flags[1] else None, rv.data_ptr(),
+        rv.stride(0), ws.data_ptr(), ws.numel(), _stream(dev)))
+    u = counts.tolist() if (flags[0] or flags[1]) else (0, 0)
+
+    def layout(flag, rows, vals, V, want_sparse, u_):
+        if flag:
+            return torch.sparse_coo_tensor(rows[None, :u_], vals[:u_], (V, vals.shape[1]), is_coalesced=True)
+        if want_sparse:       # "all": every entity row
+            return torch.sparse_coo_tensor(torch.arange(V, device=dev)[None, :], vals, vals.shape, is_coalesced=True)
+        return vals
+    return (layout(flags[0], er, ev, E, ent_rows_all, u[0]), layout(flags[1], rr_, rv, R, False, u[1]))
+
+
 def ns_loss(scores, loss: str, arg: float = 0.0, temperature: float = 1.0, label_idx=None,
             batch_size: Optional[int] = None, want_grad: bool = False, return_rows: bool = False):
     """KgeLoss of a negative-sampling block (train_negative_sampling.py:126-156): scores [n, m] with one positive per

@@ -363,6 +363,37 @@ class _NsPSlotLossFn(torch.autograd.Function):
         return (_sparse_scaled(d_ent, g), _sparse_scaled(d_rel, g)) + (None,) * 8
 
 
+class _NsSharedLossFn(torch.autograd.Function):
+    """One S / O slot of a negative-sampling batch under shared sampling (`negative_sampling.shared: True`): forward =
+    b200kge_ns_shared_score (the fixed pair of every row scored against the U' shared rows, assembled into the
+    [n, 1+K] block in the reference's column order) and the row-loss kernel, which writes G = dL/dscores for every
+    loss; backward = b200kge_ns_shared_backward, which sums G per shared id before any table gradient is formed.  The
+    scores against the shared rows are kept for TransE l_norm 2, whose backward divides by them.  A `sparse: True`
+    embedder gets its gradient row-sparse over the rows the reference looks up under `implementation`."""
+
+    @staticmethod
+    def forward(ctx, ent_w, rel_w, model, triples, slot, unique, repeat, drop, K, offset, batch_size, loss, temperature,
+                implementation):
+        ln, prec = model._b200_args()
+        l2 = model._b200_name == "transe" and ln == 2.0
+        out = engine.ns_shared_score(model._b200_name, ent_w.detach(), rel_w.detach(), triples, slot, unique, repeat,
+                                     drop, K, ln, prec, implementation, want_z=l2)
+        scores, z = out if l2 else (out, None)
+        value, G = engine.ns_loss(scores, loss, offset, temperature, batch_size=batch_size, want_grad=True)
+        ctx.args = (model, slot, K, implementation)
+        ctx.save_for_backward(ent_w, rel_w, triples, unique, repeat, drop, G, z)
+        return value
+
+    @staticmethod
+    def backward(ctx, g):
+        model, slot, K, implementation = ctx.args
+        ent_w, rel_w, triples, unique, repeat, drop, G, z = ctx.saved_tensors
+        d_ent, d_rel = engine.ns_shared_backward(model._b200_name, ent_w.detach(), rel_w.detach(), triples, slot, unique,
+                                                 repeat, drop, K, G, z, model._b200_args()[0], implementation,
+                                                 sparse=model.b200_sparse_grads())
+        return (_sparse_scaled(d_ent, g), _sparse_scaled(d_rel, g)) + (None,) * 12
+
+
 class _B200ModelMixin:
     """Index-level overrides (kge_model.py:663-789): read the tables in place when possible."""
 
@@ -681,6 +712,26 @@ class _B200ModelMixin:
         ent_w, rel_w = self._b200_weights()
         return _NsPSlotLossFn.apply(ent_w, rel_w, self, triples.long().contiguous(), negatives.long().contiguous(),
                                     float(offset), int(batch_size), loss, float(temperature), implementation)
+
+    def b200_ns_shared_ok(self):
+        """The shared-sampling kernels (b200kge_ns_shared_score / _backward) cover the dot family, TransE (L1, L2) and
+        RotatE (L1) at the precisions auto, fp32 and f16x3 with a folded width of at most 1024, and need
+        b200_backward = "native"."""
+        ent_w = self._b200_weights()[0]
+        width = ent_w.shape[1] // (2 if self._b200_name == "cp" else 1)
+        return (self.b200_backward == "native" and self._b200_native_family() and width <= 1024
+                and self._b200_args()[1] in ("auto", "fp32", "f16x3"))
+
+    def loss_negatives_shared(self, triples, slot, unique, repeat, drop, num_samples, offset, batch_size, loss="bce",
+                              temperature=1.0, implementation="batch"):
+        """loss_negatives of one S / O slot under shared negative sampling: row i's K = num_samples negatives are the
+        shared ids unique[u(i, c)] of engine.ns_shared_score (unique, repeat: the batch's _unique_samples and
+        _repeat_indexes; drop: the sub-batch's rows of _drop_index, None for the naive type).  The gradient comes from
+        b200kge_ns_shared_backward (see _NsSharedLossFn).  No embedding dropout."""
+        ent_w, rel_w = self._b200_weights()
+        return _NsSharedLossFn.apply(ent_w, rel_w, self, triples.long().contiguous(), int(slot), unique, repeat, drop,
+                                     int(num_samples), float(offset), int(batch_size), loss, float(temperature),
+                                     implementation)
 
     def loss_negatives_forward(self, scores, loss, arg=0.0, temperature=1.0):
         """Sum over rows of the KgeLoss of a scored [n, 1+K] block (positive first); forward only."""

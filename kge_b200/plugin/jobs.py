@@ -403,7 +403,13 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _NativeOptimizer, _BatchSpli
 
     With `user.b200_ns_p_slot: true` a sampled P slot (relation negatives) trains natively too, through
     model.loss_negatives_p (b200kge_ns_p_backward), when the model passes b200_ns_p_slot_ok(); without the option a P slot
-    sends the whole sub-batch to the reference step, as before."""
+    sends the whole sub-batch to the reference step, as before.
+
+    With `user.b200_ns_shared: true` and the reference's uniform sampler with `shared: True` (naive or default, with
+    or without replacement), the S and O slots train through model.loss_negatives_shared (b200kge_ns_shared_score /
+    _backward) when the model passes b200_ns_shared_ok(): each row's pair is scored against the U' shared rows once, and
+    the backward sums the block's gradient per shared id.  The host sampler, and so every draw, is the reference's.
+    A sampled P slot, embedding dropout and frequency sampling keep the route they take without the option."""
 
     def __init__(self, config, dataset, parent_job=None, model=None, forward_only=False):
         want = bool(_user_option(config, "b200_device_sampling", False))
@@ -540,6 +546,10 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _NativeOptimizer, _BatchSpli
         # "all" draws the masks of "batch" (embed_all() gives the same distribution); `auto` is resolved by _prepare
         impl = "triple" if getattr(self, "_implementation", "batch") == "triple" else "batch"
         dkw = {} if drop is None else {"dropout": drop, "implementation": impl}
+        # user.b200_ns_shared: the S / O slots of a shared uniform sample train through b200kge_ns_shared_*
+        shared = (model is not None and drop is None and P not in slots and trainable and not self.is_forward_only
+                  and self._sampler.shared and type(self._sampler).__name__ == "KgeUniformSampler"
+                  and _user_option(self.config, "b200_ns_shared", False) and model.b200_ns_shared_ok())
         if model is not None and any(model.b200_sparse_grads()):
             # the row set of a sparse gradient: `all` scores against embed_all(), so every entity row is in it
             dkw["implementation"] = getattr(self, "_implementation", "batch")
@@ -573,8 +583,13 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _NativeOptimizer, _BatchSpli
                 if negs[slot] is None:          # drawn once per batch and slot, sliced per sub-batch
                     negs[slot] = self._device_negatives(batch_size, slot, batch_index, batch.get("b200_triples"))
                 negatives = negs[slot][subbatch_slice]
+            elif shared:
+                negatives = None
             else:
-                negatives = negs[slot].samples(subbatch_slice if (subbatch_size != batch_size) else None)
+                # the whole batch's samples, sliced: NaiveSharedNegativeSample.samples takes no slice (sampler.py:414)
+                negatives = negs[slot].samples()
+                if subbatch_size != batch_size:
+                    negatives = negatives[subbatch_slice]
             tri, kslot = triples, slot
             if recip is not None and slot == S:
                 tri, kslot = torch.stack((triples[:, 2], triples[:, 1] + recip, triples[:, 0]), dim=1), O
@@ -583,7 +598,16 @@ class B200TrainingJobNegativeSampling(_DropoutKeys, _NativeOptimizer, _BatchSpli
             result.forward_time -= time.time()
             if not self.is_forward_only:
                 # training: forward + the fused NS gradient kernel behind one autograd node
-                if slot == P:
+                if shared:
+                    sm = negs[slot]
+                    drop_index = getattr(sm, "_drop_index", None)        # DefaultSharedNegativeSample only
+                    if drop_index is not None:
+                        drop_index = drop_index.to(self.device)[subbatch_slice]
+                    loss_value = model.loss_negatives_shared(
+                        tri, kslot, sm._unique_samples.to(self.device), sm._repeat_indexes.to(self.device),
+                        drop_index, num_samples, kind[1], batch_size, kind[0], kind[2],
+                        getattr(self, "_implementation", "batch"))
+                elif slot == P:
                     loss_value = model.loss_negatives_p(tri, negatives.to(self.device), kind[1], batch_size, kind[0],
                                                         kind[2], getattr(self, "_implementation", "batch"))
                 else:
